@@ -70,6 +70,8 @@ def parse_args():
     ap.add_argument("--no-parity", action="store_true", help="skip the oracle checks (they run outside the timed regions)")
     ap.add_argument("--no-secondary", action="store_true", help="N > 1: skip the other scaling mode's short measurement")
     ap.add_argument("--print-config", action="store_true", help="print the `config` object of this command line and exit")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last device-resident step computed as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -82,11 +84,11 @@ def workload_config(args):
     return {"workload": (f"config#3 forest {args.trees}x{PER_TREE} (BFS, depth {LEVELS}) + {args.lights} point lights"
                          + (" per GPU" if weak else "") + ", 4 views 1920x1080, default ClusterConfig, all roots move every frame"),
             "scaling": "weak" if weak else "strong", "entities_total": total_e, "lights_total": total_l, "views": 4,
-            "l2": "working set 167 MB/frame > 126 MB L2 at 1M entities per GPU (inputs larger than L2, no flush)"}
+            "l2": "working set 167 MB/frame > 50 MB L2 at 1M entities per GPU (inputs larger than L2, no flush)"}
 
 
 # ---------------------------------------------------------------------------------------------
-# clocks sampling (B200_PROFILING.md): sampled DURING the timed region
+# clocks sampling: sampled DURING the timed region
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = "clocks.sm,clocks.max.sm,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
@@ -260,7 +262,7 @@ def run_reference(args):
 
 
 # ---------------------------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # ---------------------------------------------------------------------------------------------
 class Rig:
     """One rank's context + the precomputed animation + pinned result buffers for one scaling mode."""
@@ -543,7 +545,61 @@ def measure_pcie(torch, dev, stream):
     return out
 
 
-def measure_next_rows(torch, bb, rig, tile_ms, expand_ms, cluster_ms, e2e_resident_ms, W):
+def device_info(torch, index):
+    """The card a number was measured on: name and the power limit it ran under (both belong beside every absolute figure)."""
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             capture_output=True, text=True, timeout=30).stdout.strip()
+        info["power_limit_w"] = float(out.splitlines()[0])
+    except (OSError, ValueError, IndexError, subprocess.SubprocessError):
+        pass
+    return info
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(rig, out_dir, prefix=""):
+    """What the caller of the device-resident path receives after its last step, as float32 / float64 .npy files: the
+    GlobalTransform rows, both change columns and ViewVisibility of a fixed, seeded sample of rows (all rows when they fit),
+    each view's sorted visible list and cluster CSR, and the frame's feedback counters.  Row ids and counts are float64
+    (exact for every u32).  Lists longer than their share are cut to a fixed, seeded sample of positions."""
+    ctx, n, V = rig.ctx, rig.n, rig.V
+
+    def sample(length, cap, seed):
+        if length <= cap:
+            return np.arange(length)
+        return np.sort(np.random.default_rng(seed).choice(length, cap, replace=False))
+
+    arrays = {}
+    rows = sample(n, 1 << 18, 0)
+    gt, gch = ctx.download_global_transforms(0, n)
+    vv, vch = ctx.download_view_visibility(0, n)
+    arrays["sample_rows"] = rows.astype(np.float64)
+    arrays["global_transform"] = gt[rows].astype(np.float32)
+    arrays["global_transform_changed"] = gch[rows].astype(np.float32)
+    arrays["view_visibility"] = vv[rows].astype(np.float32)
+    arrays["view_visibility_changed"] = vch[rows].astype(np.float32)
+    st = ctx.download_frame_stats()
+    arrays["visible_count"] = np.array([st.visible_count[v] for v in range(V)], np.float64)
+    arrays["cluster_index_count"] = np.array([st.cluster_index_count[v] for v in range(V)], np.float64)
+    arrays["cluster_farthest_z"] = np.array([st.cluster_farthest_z[v] for v in range(V)], np.float32)
+    arrays["gt_changed_count"] = np.array([st.gt_changed_count], np.float64)
+    for v in range(V):
+        vis = ctx.download_visible(v)
+        arrays[f"visible_view{v}"] = vis[sample(len(vis), 1 << 20, 1 + v)].astype(np.float64)
+        off, idx = ctx.download_clusters(v)
+        arrays[f"cluster_offsets_view{v}"] = off[:ctx.cluster_dims(v) + 1].astype(np.float64)
+        arrays[f"cluster_indices_view{v}"] = idx[sample(len(idx), 1 << 18, 101 + v)].astype(np.float64)
+    total = sum(a.nbytes for a in arrays.values())
+    assert total <= DUMP_MAX_BYTES, f"dump of {total} bytes exceeds {DUMP_MAX_BYTES}"
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, prefix + name + ".npy"), a)
+
+
+def measure_next_rows(torch, bb, rig, tile_ms, expand_ms, cluster_ms, e2e_resident_ms, K, W):
     """Cost of the SURVEY.md 8(f) rows on the bench workload (1 GPU): stage times with the row switched on against the
     base numbers measured above (same CUDA-event stage timers), plus the e2e frame when the shim takes the added /
     removed lists (N1) instead of the full visible lists."""
@@ -575,12 +631,11 @@ def measure_next_rows(torch, bb, rig, tile_ms, expand_ms, cluster_ms, e2e_reside
     for f in range(W):
         rig.e2e_step(f % WIN, writeback=False)
     torch.cuda.synchronize()
-    KD = 300
     t0 = time.perf_counter()
-    for f in range(W, W + KD):
+    for f in range(W, W + K):
         rig.e2e_step(f % WIN, writeback=False)
     torch.cuda.synchronize()
-    e2e_diff_ms = (time.perf_counter() - t0) * 1e3 / KD
+    e2e_diff_ms = (time.perf_counter() - t0) * 1e3 / K
     d2h = int(np.mean([4 * (counts_h[v, 0].item() + counts_h[v, 1].item()) for v in range(V)]) * V)
     ctx.set_result_sink(None, None, None, None)
     ctx.set_visible_diff_sink(None, None)
@@ -737,12 +792,11 @@ def main():
     ctx.set_profiling(False)
     e2e_breakdown = {"tile_ms": pt / max(pn, 1) * 2, "expand_ms": pe_ / max(pn, 1) * 2, "cluster_ms": pc / max(pn, 1) * 2}
     # A2: the same without the column write-back (round 1's e2e), A3: the reference bench's sparse mutation pattern
-    K2 = max(50, min(K, 500))
     rig.sinks(True, False)
-    res_dev_ms, res_wall = rig.timed(lambda f: rig.e2e_step(f % WIN, False), K2, W)
+    res_dev_ms, res_wall = rig.timed(lambda f: rig.e2e_step(f % WIN, False), K, W)
     res_d2h = rig.d2h_bytes(False)
     rig.sinks(True, True)
-    sp_dev_ms, sp_wall = rig.timed(lambda f: rig.e2e_step(f % WIN, True, n_changed=8), K2, W)
+    sp_dev_ms, sp_wall = rig.timed(lambda f: rig.e2e_step(f % WIN, True, n_changed=8), K, W)
     sp_d2h = rig.d2h_bytes(True)
     sp_changed = int(rig.stats.gt_changed_count)
     rig.sinks(False, False)
@@ -763,6 +817,9 @@ def main():
     value_launches = (abi.kernel_launch_count() - launches0) / K
     ts1 = time.time()
     clocks = sampler.stop(ts0, ts1)
+    if args.dump_outputs:
+        ctx.synchronize()
+        dump_outputs(rig, args.dump_outputs, f"rank{rank}_" if world > 1 else "")
     if not args.no_parity:
         fchk = W + K
         if fchk % WIN == 0:        # slot 0's recorded constants carry the feedback of the frame before the recording run
@@ -811,7 +868,7 @@ def main():
     # ---- SURVEY 8(f) rows (N1, N2, N4): what each costs on this workload; outside every timed region above ------------
     next_rows = None
     if world == 1 and not args.no_next_rows:
-        next_rows = measure_next_rows(torch, bb, rig, tile_ms_avg, expand_ms_avg, cluster_ms_avg, res_ms / K2, W)
+        next_rows = measure_next_rows(torch, bb, rig, tile_ms_avg, expand_ms_avg, cluster_ms_avg, res_ms / K, K, W)
 
     # ---- N > 1: a short measurement of the other scaling mode, reported beside the primary one -----------------------------
     secondary = None
@@ -821,15 +878,14 @@ def main():
         rig2 = Rig(args, torch, dist, bb, scenes, parallel, other, world, rank, local_rank, dev, stream)
         rig2.ctx.run(bb.STAGE_ALL); rig2.pipe.read_feedback()
         rig2.value_setup()
-        K3 = max(100, min(K, 500))
-        d_ms, _ = rig2.timed(rig2.value_step, K3, W)
+        d_ms, _ = rig2.timed(rig2.value_step, K, W)
         rig2.sinks(True, True)
-        e_dev, e_wall = rig2.timed(lambda f: rig2.e2e_step(f % WIN, True), K3, W)
+        e_dev, e_wall = rig2.timed(lambda f: rig2.e2e_step(f % WIN, True), K, W)
         rig2.sinks(False, False)
         d_ms, e_ms = rig2.max_over_ranks(d_ms, max(e_wall, e_dev / 1e3) * 1e3)
         tot = (args.trees * PER_TREE + args.lights) * (world if other == "weak" else 1)
-        secondary = {"scaling": other, "entities_total": tot, "steps": K3, "value": tot / (d_ms / K3 * 1e-3), "ms_per_step": d_ms / K3,
-                     "e2e_value": tot / (e_ms / K3 * 1e-3), "e2e_ms_per_step": e_ms / K3}
+        secondary = {"scaling": other, "entities_total": tot, "steps": K, "value": tot / (d_ms / K * 1e-3), "ms_per_step": d_ms / K,
+                     "e2e_value": tot / (e_ms / K * 1e-3), "e2e_ms_per_step": e_ms / K}
         rig = rig2
 
     if rank == 0:
@@ -837,18 +893,11 @@ def main():
         if os.path.exists(peaks_path):
             peak = json.load(open(peaks_path))["hbm_gbs"]; peak_src = "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
         else:
-            peak = 6650.0; peak_src = "fallback (B200_PROFILING.md)"
-        # DRAM bytes of one launch of the dominant kernel, from the committed `ncu --set full` capture of this workload
-        traffic, traffic_src = None, None
-        tp = os.path.join(ROOT, "profiles", "tile_kernel_traffic.json")
-        if os.path.exists(tp) and world == 1:
-            tj = json.load(open(tp))
-            if tj.get("entities") == n:
-                traffic, traffic_src = tj["dram_bytes_per_launch"], tj["source"]
+            peak = 3350.0; peak_src = "data sheet (H100 SXM HBM3, 3.35 TB/s; not a measured peak)"
         algo_bytes = n * ALGO_BYTES_PER_ENTITY + 4 * visible_pairs_rank
         achieved = algo_bytes / (tile_ms_avg * 1e-3) / 1e9
         tile_kernel = {"c": "k_propagate_cull", "s": "k_propagate_cull_scout", "w": "k_tile_warp", "f": "k_propagate_cull_flow",
-                       "t": "k_propagate_cull_tma"}.get(os.environ.get("B200VIS_TILE_KERNEL", "l")[:1], "k_propagate_cull_lean")
+                       "l": "k_propagate_cull_lean"}.get(os.environ.get("B200VIS_TILE_KERNEL", "t")[:1], "k_propagate_cull_tma")
         cfg_out = dict(cfg)
         line = {
             "metric": METRIC, "value": value, "unit": "entities/s", "n_gpus": world, "steps": K, "warmup": W,
@@ -863,6 +912,7 @@ def main():
                                  ("peer stores over NVLink (CUDA IPC) + per-frame stamps" if rig.exchange == "p2p" else "one ncclAllGather"))
                     if world > 1 else "single GPU",
                     "visible_pairs_last_frame": int(visible_pairs), "cluster_indices_last_frame": int(cluster_indices)},
+            "device": device_info(torch, local_rank),
             "clocks": clocks,
             "parity_checked": parity_ok,
             "parity": {"what": "the frame after each timed loop (e2e pass and device-resident pass), every rank, bit-exact vs the CPU oracle: "
@@ -875,16 +925,16 @@ def main():
                     "note": "one b200vis_step per frame: root Transforms from pinned host memory, per-view constants on the host, all kernels, "
                             "the GPU writes stats + sorted visible lists + cluster lists + every changed GlobalTransform (64-byte Affine3A) + "
                             "ViewVisibility bytes + both change-bit sets into host memory; one stream sync"},
-            "e2e_resident": {"value": total_entities / (res_ms / K2 * 1e-3), "unit": "entities/s", "ms_per_step": res_ms / K2, "steps": K2,
+            "e2e_resident": {"value": total_entities / (res_ms / K * 1e-3), "unit": "entities/s", "ms_per_step": res_ms / K, "steps": K,
                              "d2h_bytes_per_step": int(res_d2h),
                              "note": "GlobalTransform / ViewVisibility columns stay on the device (round 1's e2e)"},
-            "e2e_sparse": {"value": total_entities / (sp_ms / K2 * 1e-3), "unit": "entities/s", "ms_per_step": sp_ms / K2, "steps": K2,
+            "e2e_sparse": {"value": total_entities / (sp_ms / K * 1e-3), "unit": "entities/s", "ms_per_step": sp_ms / K, "steps": K,
                            "d2h_bytes_per_step": int(sp_d2h), "gt_rows_written_back_per_step": sp_changed,
                            "note": "the reference bench's own mutation pattern: 8 roots move per frame (propagate.rs:115-128), full write-back"},
             "gpu_launches": int(round(value_launches * K)), "gpu_launches_per_step": value_launches, "gpu_launches_per_e2e_step": e2e_launches,
             "host_enqueue_ms_per_step": host_ms,
             "roofline": {"bound": "hbm", "kernel": tile_kernel, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                         "frac": achieved / peak, "traffic": traffic, "traffic_source": traffic_src, "peak_source": peak_src,
+                         "frac": achieved / peak, "peak_source": peak_src,
                          "kernel_ms": tile_ms_avg, "expand_ms": expand_ms_avg, "cluster_ms": cluster_ms_avg,
                          "gt_changed_rows_last_frame": int(sanity.gt_changed_count),
                          "algorithmic_bytes_per_entity": ALGO_BYTES_PER_ENTITY, "note": EXTRA_BYTES_NOTE},

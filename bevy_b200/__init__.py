@@ -1,6 +1,6 @@
-"""bevy_b200 -- B200-native per-frame visibility pipeline (propagate -> cull -> cluster).
+"""bevy_b200 -- H100-native per-frame visibility pipeline (propagate -> cull -> cluster).
 
-The product is ``libb200vis.so`` (CUDA kernels for sm_100a behind the C ABI of
+The product is ``libb200vis.so`` (CUDA kernels for sm_90a behind the C ABI of
 ``include/b200vis.h``).  This package is its Python host binding: ctypes
 plumbing for tests and benchmarks plus a thin mirror of the reference's three
 systems.  It never imports ``oracle`` and has no CPU fallback: creating a

@@ -1,4 +1,4 @@
-"""Builds libb200vis.so (CUDA kernels + C ABI) in-tree for sm_100a.
+"""Builds libb200vis.so (CUDA kernels + C ABI) in-tree for sm_90a (H100).
 
 nvcc cross-compiles without a GPU.  Numerics flags are part of the parity
 contract (see csrc/kernels.cu): no FMA contraction on device or host, IEEE
@@ -15,7 +15,7 @@ SOURCES = ["kernels.cu", "api.cu", "host_view.cpp"]
 HEADERS = ["device_types.cuh", "kernels.cuh", "host_view.hpp", os.path.join("..", "..", "include", "b200vis.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-fmad=false", "-prec-div=true", "-prec-sqrt=true", "-ftz=false",
     "-Xcompiler", "-fPIC,-O2,-ffp-contract=off,-fno-fast-math,-fvisibility=hidden",

@@ -1,4 +1,4 @@
-// kernels.cu -- the sm_100a kernels of libb200vis: propagate -> cull -> cluster.
+// kernels.cu -- the sm_90a kernels of libb200vis: propagate -> cull -> cluster.
 //
 // Numerics contract: every float operation below is IEEE-754 binary32 in the
 // operation order of glam's x86-64/SSE2 backend (SURVEY.md Appendix A), with
@@ -774,8 +774,8 @@ k_propagate_cull_tma(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, c
 }
 
 // ------------------------------------------------------------------------------------------
-// Kernel 1L (the DEFAULT tile kernel; B200VIS_TILE_KERNEL=tma selects 1b): kernel 1b on an instruction and exposed-latency diet.
-// ncu's source view of 1b (profiles/r02b_tma_basic_blocks.txt) shows ~820 warp instructions per 32 rows of which half are
+// Kernel 1L (B200VIS_TILE_KERNEL=lean; kernel 1b is the default): kernel 1b on an instruction and exposed-latency diet.
+// ncu's source view of 1b shows ~820 warp instructions per 32 rows of which half are
 // bookkeeping, an SM that issues ~2 warp instructions per cycle whatever the occupancy (DESIGN.md section 7), and four places where
 // a long latency is exposed on every tile:
 //   * the tile descriptor (LDG of tiles[t]) at the top of a tile                  -> descriptors travel through shared memory:
@@ -785,12 +785,12 @@ k_propagate_cull_tma(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, c
 //     (a leaf warp that idles while the levels above it are walked), the ticket is drawn one tile further ahead and the
 //     prefetch goes out at the top of the tile, a whole walk earlier;
 //   * the view-rejection test reads its planes with register-indexed LDC          -> planes are staged in shared memory once
-//     per CTA; the box is built with f32 warp reductions (CREDUX.F32) instead of order-preserving integer transforms;
+//     per CTA; the box is built with warp min / max reductions (redux_min_f32 / redux_max_f32);
 //   * the per-view loop was unrolled 8x with the plane operands in the constant bank (48 KB of code, a test + branch per
 //     view even when the warp rejected it)                                         -> one rolled loop over the set bits of
 //     (active views & ~rejected), planes from shared memory: a warp that rejects every view skips the loop in 3 instructions.
 // On top of that: the tile's top levels are walked in registers with warp shuffles; B200VIS_LEAN_PROBE=8 bounds the warp's rows
-// with a sphere (3 shuffles + 1 reduction) instead of a box (7 reductions) in the warp-level view rejection (measured: +1 %).
+// with a sphere (3 shuffles + 1 reduction) instead of a box (7 reductions) in the warp-level view rejection.
 // Same results bit for bit (tests/test_gpu_bench_scale.py runs the bench workload through it).
 // ------------------------------------------------------------------------------------------
 // MINB = 4: the whole tile (Transform, GlobalTransform, topo, flags, state: 94 B/row) is staged in both stages, as in kernel 1b.
@@ -858,8 +858,15 @@ __device__ __forceinline__ void issue_lean_loads(const Rows &R, const Tile &t, L
 __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t cnt) { asm volatile(B200VIS_BAR_SEQ("bar.sync") ::"r"(id), "r"(cnt) : "memory"); }
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t cnt) { asm volatile(B200VIS_BAR_SEQ("bar.arrive") ::"r"(id), "r"(cnt) : "memory"); }
 #undef B200VIS_BAR_SEQ
-__device__ __forceinline__ float redux_min_f32(float x) { float r; asm volatile("redux.sync.min.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ float redux_max_f32(float x) { float r; asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(x)); return r; }
+// warp-wide f32 min / max: sm_90 has redux.sync only for integers, so the float goes through an order-preserving s32 key
+// (flip the magnitude bits of negatives; the map is its own inverse).  Exact for every non-NaN input, which is all callers pass.
+__device__ __forceinline__ int f32_order_key(int i) { return i ^ ((i >> 31) & 0x7FFFFFFF); }
+__device__ __forceinline__ float redux_min_f32(float x) {
+    return __int_as_float(f32_order_key(__reduce_min_sync(0xFFFFFFFFu, f32_order_key(__float_as_int(x)))));
+}
+__device__ __forceinline__ float redux_max_f32(float x) {
+    return __int_as_float(f32_order_key(__reduce_max_sync(0xFFFFFFFFu, f32_order_key(__float_as_int(x)))));
+}
 __device__ __forceinline__ void cp_async_tile_desc(Tile *dst, const Tile *src) {     // 24 bytes, 8-byte aligned on both sides
     const uint32_t d = smem_u32(dst);
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(d), "l"(src) : "memory");
@@ -3807,11 +3814,11 @@ static bool first_call_on_device(unsigned long long &seen) {
     seen |= bit;
     return true;
 }
-static int g_tile_kernel = -1;   // 5 lean (default: TMA-staged, bookkeeping thread, top levels in registers, rolled view loop), 0 classic (one tile per CTA, LDG), 1 kernel 1b (persistent TMA-staged CTA per tile), 2 warp per tile, 3 TMA + scout warp, 4 TMA flow (no inter-tile barrier)
+static int g_tile_kernel = -1;   // 1 kernel 1b (default: persistent TMA-staged CTA per tile), 5 lean (TMA-staged, bookkeeping thread, top levels in registers, rolled view loop), 0 classic (one tile per CTA, LDG), 2 warp per tile, 3 TMA + scout warp, 4 TMA flow (no inter-tile barrier)
 static int tile_kernel_choice() {
     if (g_tile_kernel < 0) {
         const char *e = getenv("B200VIS_TILE_KERNEL");
-        g_tile_kernel = (e && e[0] == 'c') ? 0 : (e && e[0] == 'w') ? 2 : (e && e[0] == 's') ? 3 : (e && e[0] == 'f') ? 4 : (e && e[0] == 't') ? 1 : 5;      // default: lean (kernel 1L); tma = kernel 1b
+        g_tile_kernel = (e && e[0] == 'c') ? 0 : (e && e[0] == 'w') ? 2 : (e && e[0] == 's') ? 3 : (e && e[0] == 'f') ? 4 : (e && e[0] == 'l') ? 5 : 1;      // default: kernel 1b (on H100 ~4 % faster per frame than lean, DESIGN.md section 7)
     }
     return g_tile_kernel;
 }
@@ -3820,7 +3827,7 @@ static int lean_ctas_per_sm() {       // B200VIS_LEAN_CTAS = 4 | 5 | 6 resident 
     if (!n) { const char *e = getenv("B200VIS_LEAN_CTAS"); n = (e && (atoi(e) == 5 || atoi(e) == 6)) ? atoi(e) : 4; }
     return n;
 }
-static bool lean_pipe() {       // B200VIS_LEAN_PIPE=1: the CTA's warps are not held together at tile boundaries (measured slower: DESIGN.md section 7)
+static bool lean_pipe() {       // B200VIS_LEAN_PIPE=1: the CTA's warps are not held together at tile boundaries
     static int v = -1;
     if (v < 0) { const char *e = getenv("B200VIS_LEAN_PIPE"); v = (e && atoi(e) == 1) ? 1 : 0; }
     return v != 0;
@@ -3981,7 +3988,7 @@ static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32
     ++g_launches;
     with_kernel([&](auto kern) {
         if constexpr (KIND >= 4) {
-            static int flip = -1;     // B200VIS_LEAN_WARP_FLIP=1 reverses the CTA's warp order (no measurable effect: DESIGN.md section 7)
+            static int flip = -1;     // B200VIS_LEAN_WARP_FLIP=1 reverses the CTA's warp order
             if (flip < 0) { const char *e = getenv("B200VIS_LEAN_WARP_FLIP"); flip = (e && atoi(e) == 1) ? 0xE0 : 0; }
             static int probe = -1;    // B200VIS_LEAN_PROBE: timing probes, wrong results (tools/ only)
             if (probe < 0) { const char *e = getenv("B200VIS_LEAN_PROBE"); probe = e ? atoi(e) : 0; }
@@ -4099,7 +4106,9 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
 void launch_publish_visible(cudaStream_t st, const VisibleBufs &vb, const DevStats *stats, uint32_t *host_rows, uint32_t host_stride,
                             uint32_t n_rows, uint32_t n_views, uint8_t *host_classes) {
     if (!n_views || !n_rows) return;
-    ++g_launches; k_publish_visible<<<dim3(min(cdiv(n_rows, 256), 296u), n_views), 256, 0, st>>>(vb.lists, vb.list_stride, stats, host_rows, host_stride, n_views, vb.classes, host_classes);
+    static int sms = 0;    // two CTAs per SM per view
+    if (!sms) { int dev = 0; cudaGetDevice(&dev); cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev); if (sms <= 0) sms = 132; }
+    ++g_launches; k_publish_visible<<<dim3(min(cdiv(n_rows, 256), 2u * (uint32_t)sms), n_views), 256, 0, st>>>(vb.lists, vb.list_stride, stats, host_rows, host_stride, n_views, vb.classes, host_classes);
 }
 void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, uint32_t *host_offsets, uint32_t *host_indices,
                              uint32_t host_cap, const DevStats *stats, uint32_t *host_stats, uint32_t changed_slot, uint32_t frame, uint32_t max_views) {

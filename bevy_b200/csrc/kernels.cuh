@@ -1,4 +1,4 @@
-// kernels.cuh -- launchers of the sm_100a kernels (kernels.cu)
+// kernels.cuh -- launchers of the sm_90a kernels (kernels.cu)
 #pragma once
 #include <cuda_runtime.h>
 #include "device_types.cuh"

@@ -1,5 +1,5 @@
 /*
- * b200vis.h -- C ABI of libb200vis.so: the B200-native replacement for the
+ * b200vis.h -- C ABI of libb200vis.so: the H100-native replacement for the
  * per-frame visibility pipeline of bevyengine/bevy 0.20.0-dev
  * (propagate -> cull -> cluster).
  *

@@ -10,8 +10,8 @@
  * PINNING STATUS
  *   The reference is 100% Rust and cannot be built here (no rustc/cargo), and
  *   its arithmetic lives in the third-party crate glam = "0.33.2"
- *   (crates/bevy_math/Cargo.toml:13), which is not vendored under
- *   /root/reference.  This file restates glam's published x86-64/SSE2
+ *   (crates/bevy_math/Cargo.toml:13), which is not vendored in
+ *   the reference checkout.  This file restates glam's published x86-64/SSE2
  *   operation order (see each helper) and is pinned against every golden
  *   vector the reference's own tests hold for this path:
  *     - frustum/sphere known answers    crates/bevy_camera/src/primitives.rs:462-611
