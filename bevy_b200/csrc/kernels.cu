@@ -4091,7 +4091,9 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
     }
     if (!enabled) return false;
     const uint32_t words = (L.n + 31u) / 32u;
-    uint32_t nrank = (nrank_env == 2 || nrank_env == 4 || nrank_env == 8 || nrank_env == 16) ? (uint32_t)nrank_env : 8u;
+    // every CTA popcounts, scans and emits its kMaxClusters / nrank owned clusters with one thread each: nrank >= 4
+    static_assert(kMaxClusters / 4 <= kFusedThreads, "a CTA of the fused cluster kernel owns more clusters than it has threads");
+    uint32_t nrank = (nrank_env == 4 || nrank_env == 8 || nrank_env == 16) ? (uint32_t)nrank_env : 8u;
     size_t smem = (size_t)words * (kMaxClusters / nrank) * 4;
     if (smem > 200u * 1024u) { nrank = 16; smem = (size_t)words * (kMaxClusters / nrank) * 4; }
     if (smem > 200u * 1024u) return false;                    // more lights than the distributed matrix can hold: split path
@@ -4101,7 +4103,23 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = nrank; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
     cfg.attrs = attr; cfg.numAttrs = 1;
-    ++g_launches; return cudaLaunchKernelEx(&cfg, k_cluster_fused, R, L, fc, cb, stats) == cudaSuccess;
+    // Whether the device can co-schedule nrank CTAs of ~200 KB shared memory each (16 is a non-portable cluster size) is
+    // asked once per cluster size at the largest shared-memory footprint; a size it cannot hold goes to the split path.
+    // A refusal by the runtime is not the frame's error (the caller falls back to the split kernels): it is cleared again.
+    static int schedulable[17] = {};           // 0 unknown, 1 yes, -1 no
+    if (schedulable[nrank] == 0) {
+        cudaLaunchConfig_t probe = cfg;
+        probe.dynamicSmemBytes = 200u * 1024u;
+        int n_clusters = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveClusters(&n_clusters, k_cluster_fused, &probe);
+        schedulable[nrank] = (e == cudaSuccess && n_clusters > 0) ? 1 : -1;
+        if (e != cudaSuccess) (void)cudaGetLastError();
+    }
+    if (schedulable[nrank] < 0) return false;
+    ++g_launches;
+    if (cudaLaunchKernelEx(&cfg, k_cluster_fused, R, L, fc, cb, stats) == cudaSuccess) return true;
+    (void)cudaGetLastError();
+    return false;
 }
 void launch_publish_visible(cudaStream_t st, const VisibleBufs &vb, const DevStats *stats, uint32_t *host_rows, uint32_t host_stride,
                             uint32_t n_rows, uint32_t n_views, uint8_t *host_classes) {

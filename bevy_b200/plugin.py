@@ -37,7 +37,8 @@ class VisibilityPipeline:
     def update_views(self, clusters=True):
         views = []
         for v, cam in enumerate(self.scene.cameras):
-            cfv = abi.host_perspective(cam.fov, cam.aspect, cam.near)
+            cfv = abi.host_perspective(cam.fov, cam.aspect, cam.near) if cam.clip_from_view is None \
+                else np.ascontiguousarray(cam.clip_from_view, np.float32)
             frustum = abi.host_compute_frustum(cfv, cam.gt, cam.far)
             sc = self.scene
             layers = 1 if sc.view_layers is None else int(sc.view_layers[v])
@@ -53,8 +54,11 @@ class VisibilityPipeline:
         self.views = views
 
     def update_views_fast(self):
-        """Same as update_views through b200vis_update_camera: one C call per camera, no numpy on the way."""
+        """Same as update_views through b200vis_update_camera: one C call per camera, no numpy on the way.  The camera
+        descriptor has no projection field, so this path is perspective only."""
         sc = self.scene
+        if any(cam.clip_from_view is not None for cam in sc.cameras):
+            raise ValueError("update_views_fast builds perspective projections only: use update_views for a camera with clip_from_view")
         if not hasattr(self, "_cam_desc"):
             self._cam_desc = [abi.CameraDesc() for _ in sc.cameras]
             self.cluster_views = [abi.ClusterView() for _ in sc.cameras]

@@ -23,6 +23,27 @@ class Camera:
     near: float = 0.1
     far: float = 1000.0
     quat: np.ndarray = None        # [4] rotation, kept for animation
+    clip_from_view: np.ndarray = None   # [16] column-major; None => the perspective above (e.g. orthographic_clip_from_view)
+
+
+def orthographic_clip_from_view(left, right, bottom, top, near=0.0, far=1000.0):
+    """OrthographicProjection::get_clip_from_view (crates/bevy_camera/src/projection.rs:638-649): glam's right-handed
+    [0, 1]-depth orthographic matrix with near and far swapped (reverse z), in float32 as glam computes it."""
+    f = np.float32
+    left, right, bottom, top, near, far = (f(v) for v in (left, right, bottom, top, near, far))
+    rcp_width, rcp_height = f(1.0) / (right - left), f(1.0) / (top - bottom)
+    r = f(1.0) / (far - near)                  # 1 / (near' - far') with near' = far, far' = near
+    m = np.zeros(16, np.float32)
+    m[0], m[5], m[10] = rcp_width + rcp_width, rcp_height + rcp_height, r
+    m[12], m[13], m[14], m[15] = -(left + right) * rcp_width, -(top + bottom) * rcp_height, r * far, 1.0
+    return m
+
+
+def orthographic_window(width, height, scale=1.0, near=0.0, far=1000.0):
+    """ScalingMode::WindowSize with viewport_origin (0.5, 0.5): the area is the window centred on the camera, `scale`
+    world units per pixel (OrthographicProjection::default_3d has near 0)."""
+    hw, hh = np.float32(width) * np.float32(0.5) * np.float32(scale), np.float32(height) * np.float32(0.5) * np.float32(scale)
+    return orthographic_clip_from_view(-hw, hw, -hh, hh, near, far)
 
 
 @dataclass

@@ -2,6 +2,8 @@
 frame by frame.  Bit-exact for GlobalTransform bits, change flags, ViewVisibility bytes, visible lists
 and cluster index lists (north_star: bit-exact bits/indices; 1e-5 abs on GlobalTransform floats -- we
 hold the floats to bit equality too and report the max abs difference if that ever fails)."""
+from dataclasses import dataclass
+
 import numpy as np
 
 import bevy_b200 as bb
@@ -9,6 +11,48 @@ from bevy_b200 import scenes
 import oracle as orc
 
 IDENTITY = np.array([1, 0, 0, 0, 1, 0, 0, 0, 1, 0, 0, 0], np.float32)
+CONFIG_KINDS = {"none": 0, "single": 1, "xyz": 2, "fixedz": 3}
+
+
+@dataclass
+class ClusterSpec:
+    """One ClusterConfig (crates/bevy_light/src/cluster/mod.rs:107-139) + viewport + GlobalClusterSettings max indices, from
+    which both sides are built: `abi_config()` for the device, `oracle_kwargs()` for orc.default_cluster_view_in."""
+    kind: str = "fixedz"
+    dims: tuple = (0, 0, 0)            # XYZ
+    total: int = 4096                  # FixedZ
+    z_slices: int = 24                 # FixedZ
+    first_slice_depth: float = 5.0
+    far_z_constant: float = None       # None => ClusterFarZMode::MaxClusterableObjectRange
+    dynamic_resizing: bool = True
+    screen: tuple = (1920, 1080)
+    max_indices: int = 16384
+
+    def abi_config(self):
+        c = bb.ClusterConfig()
+        c.kind = CONFIG_KINDS[self.kind]
+        c.dims[:] = list(self.dims)
+        c.total, c.z_slices, c.first_slice_depth = self.total, self.z_slices, self.first_slice_depth
+        c.far_z_mode = 0 if self.far_z_constant is None else 1
+        c.far_z_constant = 0.0 if self.far_z_constant is None else self.far_z_constant
+        c.dynamic_resizing = int(self.dynamic_resizing)
+        c.screen_w, c.screen_h = self.screen
+        c.view_cluster_bindings_max_indices = self.max_indices
+        return c
+
+    def oracle_kwargs(self):
+        return dict(screen=tuple(self.screen), config_kind=CONFIG_KINDS[self.kind], cfg_dims=tuple(self.dims), total=self.total,
+                    z_slices=self.z_slices, first_slice_depth=self.first_slice_depth,
+                    far_z_mode=0 if self.far_z_constant is None else 1,
+                    far_z_constant=0.0 if self.far_z_constant is None else self.far_z_constant,
+                    dynamic_resizing=self.dynamic_resizing, max_indices=self.max_indices)
+
+
+def clip_from_view(cam):
+    """The camera's projection on the oracle side: its explicit clip_from_view, else the oracle's perspective."""
+    if cam.clip_from_view is not None:
+        return np.ascontiguousarray(cam.clip_from_view, np.float32)
+    return orc.perspective(cam.fov, cam.aspect, cam.near)
 
 
 class OracleWorld:
@@ -17,6 +61,7 @@ class OracleWorld:
     def __init__(self, scene, static_opt=True, cluster_kwargs=None):
         self.scene = scene
         self.cluster_kwargs = cluster_kwargs or {}
+        self.fb_used = None            # the Clusters feedback each view's last frame() started from
         n = scene.n
         self.gt = np.tile(IDENTITY, (n, 1))
         self.vv = np.zeros(n, np.uint8)
@@ -62,12 +107,13 @@ class OracleWorld:
             vis = np.nonzero(self.vv[sc.light_row] & 1)[0]
             lights = np.concatenate([self.gt[sc.light_row[vis], 9:12], sc.light_range[vis, None]], 1).astype(np.float32)
             ll = None if sc.light_layers is None else np.ascontiguousarray(sc.light_layers[vis], np.uint64)
+            self.fb_used = [dict(f) for f in self.fb]
             for v, cam in enumerate(sc.cameras):
-                cfv = orc.perspective(cam.fov, cam.aspect, cam.near)
-                vin = orc.default_cluster_view_in(cam.gt, cfv, views_planes[v], screen=sc.screen,
+                kw = dict(screen=sc.screen)
+                kw.update(self.cluster_kwargs)
+                vin = orc.default_cluster_view_in(cam.gt, clip_from_view(cam), views_planes[v],
                                                   view_layers=1 if sc.view_layers is None else int(sc.view_layers[v]),
-                                                  last_farthest_z=self.fb[v]["far"], last_index_count=self.fb[v]["cnt"],
-                                                  **self.cluster_kwargs)
+                                                  last_farthest_z=self.fb[v]["far"], last_index_count=self.fb[v]["cnt"], **kw)
                 out, offsets, idx, _ = orc.assign_lights_to_clusters(vin, lights, ll)
                 self.fb[v]["far"] = out.farthest_z; self.fb[v]["cnt"] = out.total_index_count
                 clusters.append((out, offsets, vis[idx].astype(np.uint32)))
@@ -138,9 +184,13 @@ def compare_frame(pipe, world, frame_no, cluster=True, check_gt=True, run_device
     return stats
 
 
-def run_parity(scene, frames=3, static_opt=True, animate=True, cluster=True, visible_diff=False):
-    pipe = bb.VisibilityPipeline(scene, static_transform_optimizations=static_opt)
-    world = OracleWorld(scene, static_opt)
+def run_parity(scene, frames=3, static_opt=True, animate=True, cluster=True, visible_diff=False, cluster_spec=None,
+               before_frame=None, on_frame=None):
+    """`cluster_spec` (ClusterSpec) sets the cluster config of both sides; `before_frame(pipe, world, f)` may edit the scene
+    before frame f is set up, `on_frame(pipe, world, f)` runs after frame f matched."""
+    pipe = bb.VisibilityPipeline(scene, static_transform_optimizations=static_opt,
+                                 cluster_config=None if cluster_spec is None else cluster_spec.abi_config())
+    world = OracleWorld(scene, static_opt, cluster_kwargs=None if cluster_spec is None else cluster_spec.oracle_kwargs())
     if visible_diff:
         pipe.enable_visible_diff()
     try:
@@ -151,7 +201,11 @@ def run_parity(scene, frames=3, static_opt=True, animate=True, cluster=True, vis
                     rows, trs = scenes.mutate_roots(scene, f)
                     pipe.ctx.upload_transforms_scattered(rows, trs)
                     world.tchanged[rows] = 1
+            if before_frame is not None:
+                before_frame(pipe, world, f)
             pipe.update_views(clusters=cluster)
             compare_frame(pipe, world, f, cluster=cluster)
+            if on_frame is not None:
+                on_frame(pipe, world, f)
     finally:
         pipe.close()
