@@ -113,6 +113,10 @@ _SIGNATURES = {
     "b200vis_join": (C.c_int32, [_vp]),
     "b200vis_tail_stream": (C.c_int32, [_vp, _P(_vp)]),
     "b200vis_set_topology": (C.c_int32, [_vp, C.c_uint32, _vp, _vp]),
+    "b200vis_edit_topology": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp]),
+    "b200vis_topology_summary": (C.c_int32, [_vp, _P(C.c_uint32)]),
+    "b200vis_host_edit_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, C.c_uint32, _vp, C.c_uint32,
+                                           _P(C.c_uint32), _P(C.c_uint32), _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "b200vis_kernel_launch_count": (C.c_uint64, []),
     "b200vis_p2p_link": (C.c_int32, [_vp, C.c_uint32]),
     "b200vis_upload_render_layers_ext": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp]),
@@ -309,6 +313,53 @@ def host_warp_plan(parent, tile_rows=0):
     return desc, nonroot, sched, wtopo
 
 
+class EditedPlan:
+    """What b200vis_host_edit_plan returns: rc (0, or the error of the first failing step), n rows, tile_desc[T,17]
+    (columns 0-7 as host_tile_plan, 8 = chunks | contiguous bits << 8, 9-16 = nonroot), sched[T,256], topo[n], wtopo[n],
+    counters (tiles re-planned, rows re-planned by the last applied step, passes, steps applied)."""
+
+    def __init__(self, rc, n, desc, sched, topo, wtopo, counters):
+        self.rc, self.n, self.desc, self.sched, self.topo, self.wtopo, self.counters = rc, n, desc, sched, topo, wtopo, counters
+
+    def tile_desc(self):
+        """(tile_desc[T,8], topo) in the layout of host_tile_plan."""
+        return self.desc[:, :8].copy(), self.topo
+
+    def warp_plan(self):
+        """(tile_desc[T,4], nonroot[T,8], sched[T,256], wtopo) in the layout of host_warp_plan."""
+        d = self.desc[:, [0, 1, 8, 7]].copy()
+        return d, self.desc[:, 9:17].copy(), self.sched, self.wtopo
+
+
+def edit_script(steps):
+    """Encodes [(despawn_rows, reparent_rows, new_parent, spawn_parent), ...] for host_edit_plan."""
+    words = []
+    for despawn, reparent, new_parent, spawn_parent in steps:
+        despawn, reparent, new_parent, spawn_parent = (list(map(int, x)) for x in (despawn, reparent, new_parent, spawn_parent))
+        assert len(reparent) == len(new_parent)
+        words += [len(despawn), len(reparent), len(spawn_parent)] + despawn + reparent + new_parent + spawn_parent
+    return np.asarray(words, np.uint32)
+
+
+def host_edit_plan(parent, steps, max_rows=None, tile_rows=0):
+    """The plan after applying edit steps (see edit_script) to a fresh plan of `parent`, as b200vis_edit_topology keeps it."""
+    parent = _arr(parent, np.uint32)
+    script = edit_script(steps)
+    if max_rows is None:
+        max_rows = len(parent) + sum(len(s[3]) for s in steps)
+    lib = load_library()
+    n_out, nt, ctr = C.c_uint32(0), C.c_uint32(0), (C.c_uint32 * 4)()
+    rc = lib.b200vis_host_edit_plan(len(parent), _ptr(parent), tile_rows, max_rows, len(script), _ptr(script), 0,
+                                    C.byref(n_out), C.byref(nt), None, None, None, None, ctr)
+    T, n = nt.value, n_out.value
+    desc = np.zeros((T, 17), np.uint32); sched = np.zeros((T, 256), np.uint8)
+    topo = np.zeros(n, np.uint32); wtopo = np.zeros(n, np.uint32)
+    rc2 = lib.b200vis_host_edit_plan(len(parent), _ptr(parent), tile_rows, max_rows, len(script), _ptr(script), T,
+                                     C.byref(n_out), C.byref(nt), _ptr(desc), _ptr(topo), _ptr(wtopo), _ptr(sched), ctr)
+    assert rc2 == rc
+    return EditedPlan(rc, n, desc, sched, topo, wtopo, tuple(ctr))
+
+
 def p2p_link(contexts):
     """b200vis_p2p_link: contexts[r] was created with world_size=len(contexts), rank=r (one process, several devices)."""
     arr = (C.c_void_p * len(contexts))(*[c._h for c in contexts])
@@ -372,6 +423,20 @@ class Context:
         assert len(p) == len(e)
         self._check(self._lib.b200vis_set_topology(self._h, len(p), _ptr(p), _ptr(e)))
         self.n = len(p)
+
+    def edit_topology(self, despawn=(), reparent=(), new_parent=(), spawn_parent=(), spawn_entity_bits=()):
+        """One frame's despawns, reparents and spawns (b200vis_edit_topology); spawned rows are appended at self.n."""
+        d = _arr(despawn, np.uint32); r = _arr(reparent, np.uint32); npr = _arr(new_parent, np.uint32)
+        sp = _arr(spawn_parent, np.uint32); sb = _arr(spawn_entity_bits, np.uint64)
+        assert len(r) == len(npr) and len(sp) == len(sb)
+        self._check(self._lib.b200vis_edit_topology(self._h, len(d), _ptr(d), len(r), _ptr(r), _ptr(npr), len(sp), _ptr(sp), _ptr(sb)))
+        self.n = getattr(self, "n", 0) + len(sp)
+
+    def topology_summary(self):
+        """(rows incl. tombstones, live rows, tiles, passes)."""
+        out = (C.c_uint32 * 4)()
+        self._check(self._lib.b200vis_topology_summary(self._h, out))
+        return tuple(out)
 
     def upload_transforms(self, first_row, trs):
         t = _arr(trs, np.float32).reshape(-1, 10)

@@ -54,6 +54,9 @@ NcclApi g_nccl;
 constexpr int kNcclUint32 = 3;   // ncclUint32 in nccl.h's ncclDataType_t
 }
 
+struct Plan;
+static void free_plan(Plan *p);
+
 struct b200vis_ctx {
     b200vis_config cfg{};
     int device = 0;
@@ -95,6 +98,13 @@ struct b200vis_ctx {
     std::vector<uint32_t> pass_small;   // the first pass_small[p] tiles of pass p have <= 32 rows (B200VIS_SPLIT_DEEP_TILES)
     std::vector<uint8_t> pass_named;    // every tile of pass p is flat or walks with named level barriers (Tile::lvl_warps): the tile kernel may let a CTA's warps drift a tile apart
     int static_opt = 1;
+    // b200vis_edit_topology: the host plan kept between calls, the world's keys (Entity::to_bits()) in rank order -- on the
+    // host after set_topology, on the device from the first edit that needs a merge -- and the spare rank arrays a merge
+    // writes into (swapped in when the edit is committed)
+    Plan *hplan = nullptr;
+    std::vector<uint64_t> h_keys; bool keys_resident = false; uint64_t max_key = 0;
+    uint64_t *d_keys = nullptr, *d_keys2 = nullptr; uint32_t *d_rank2 = nullptr, *d_row_of_rank2 = nullptr;
+    uint8_t *h_edit = nullptr; size_t h_edit_bytes = 0; cudaEvent_t ev_edit = nullptr;   // pinned staging of an edit's uploads
 
     // per-frame constants
     // The "frame blob": FrameConsts followed by the packed per-view plane tables and z thresholds.
@@ -212,8 +222,11 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->bind.oc, ctx->bind.il, ctx->bind.count, ctx->d_bind_map,
                    ctx->d_range_se, ctx->d_range_ua, ctx->d_range_views, ctx->d_visibility, ctx->d_iv_changed,
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
-                   ctx->shadow.count, ctx->shadow.active};
+                   ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2};
     for (void *p : dev) if (p) cudaFree(p);
+    if (ctx->h_edit) cudaFreeHost(ctx->h_edit);
+    if (ctx->ev_edit) cudaEventDestroy(ctx->ev_edit);
+    free_plan(ctx->hplan);
     for (int i = 0; i < b200vis_ctx::kRing; ++i) {
         if (ctx->h_ring[i]) cudaFreeHost(ctx->h_ring[i]);
         if (ctx->ring_ev[i]) cudaEventDestroy(ctx->ring_ev[i]);
@@ -398,48 +411,30 @@ struct Plan {
     std::vector<uint32_t> pass_begin;    // tile index ranges per pass: [pass_begin[p], pass_begin[p+1])
     std::vector<uint32_t> pass_small;
     uint32_t n_ext = 0;                  // rows whose parent sits in another tile
+    // The same tiles in creation (= row) order, with what b200vis_edit_topology needs to re-plan some of them: the tile of
+    // every row, each tile's pass and the tiles of its out-of-tile parents, and the live children of every row.
+    // WarpTile::sched is the creation index, in both orders.
+    std::vector<Tile> tiles_c;
+    std::vector<WarpTile> wtiles_c;
+    std::vector<uint32_t> tile_of, level, n_children;
+    std::vector<std::vector<uint32_t>> ext;
+    uint32_t cap = kTileRows;            // tile size the rows were cut with
+    // edit state (b200vis_edit_topology): the parent array, which rows are alive
+    std::vector<uint32_t> parent;
+    std::vector<uint8_t> alive;
+    uint32_t n = 0, n_dead = 0;
 };
-static int32_t build_plan(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, uint32_t cap, Plan &plan) {
-    std::vector<uint32_t> &topo = plan.topo; std::vector<Tile> &tiles_sorted = plan.tiles;
-    std::vector<uint32_t> &pass_begin = plan.pass_begin; std::vector<uint32_t> *pass_small = &plan.pass_small;
-    if (cap < 32) cap = 32;
-    if (cap > (uint32_t)kTileRows) cap = kTileRows;
-    for (uint32_t r = 0; r < n; ++r) {
-        const uint32_t p = parent[r];
-        if (p == kNoParent || p == kDetached) continue;
-        if (p >= n) return fail(ctx, B200VIS_ERR_PARENT_OUT_OF_RANGE, "row %u: parent %u out of range (n=%u)", r, p, n);
-    }
-    {   // cycle check: every chain must end at a root / detached row
-        std::vector<uint8_t> color(n, 0);
-        std::vector<uint32_t> path;
-        for (uint32_t r = 0; r < n; ++r) {
-            if (color[r]) continue;
-            path.clear();
-            uint32_t c = r;
-            while (true) {
-                if (color[c] == 2) break;
-                if (color[c] == 1) return fail(ctx, B200VIS_ERR_HIERARCHY_CYCLE, "hierarchy cycle through row %u", c);
-                color[c] = 1; path.push_back(c);
-                const uint32_t p = parent[c];
-                if (p >= n) break;
-                c = p;
-            }
-            for (uint32_t x : path) color[x] = 2;
-        }
-    }
-    for (uint32_t r = 0; r < n; ++r)
-        if (parent[r] < n && parent[r] >= r)
-            return fail(ctx, B200VIS_ERR_UNSUPPORTED,
-                        "row %u has parent %u >= itself: rows must be in topological order (use b200vis_plan_row_order)", r,
-                        parent[r]);
-    // greedy tiling, cutting at the latest tree boundary inside a full tile
+
+static bool split_deep_tiles() {
     static int split_env = -1;
     if (split_env < 0) { const char *e = getenv("B200VIS_SPLIT_DEEP_TILES"); split_env = (e && atoi(e)) ? 1 : 0; }
-    const bool split_deep = split_env == 1;
-    std::vector<Tile> tiles;
-    std::vector<uint32_t> tile_of(n);
-    std::vector<uint8_t> marked(n, 0);
-    uint32_t start = 0;
+    return split_env == 1;
+}
+
+// Greedy tiling of rows [start, n), cutting at the latest tree boundary inside a full tile; appends to `tiles`.
+static void cut_tiles(uint32_t n, const uint32_t *parent, uint32_t start, uint32_t cap, std::vector<Tile> &tiles) {
+    const bool split_deep = split_deep_tiles();
+    std::vector<uint8_t> marked(n - start, 0);
     while (start < n) {
         uint32_t end = std::min<uint32_t>(n, start + cap);
         if (end < n && parent[end] < n) {          // the cut would split a tree: back up to a boundary
@@ -449,12 +444,13 @@ static int32_t build_plan(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, 
         }
         {   // k_tile_warp keeps the GlobalTransforms of the rows WITH in-tile children in kWarpParentSlots shared-memory
             // slots: cut the tile before the child that would need one more (only chains and unary-heavy trees get there)
+            const uint32_t s0 = (uint32_t)(n - marked.size());
             uint32_t parents = 0;
             for (uint32_t c = start; c < end; ++c) {
                 const uint32_t p = parent[c];
-                if (p < n && p >= start && !marked[p]) {
+                if (p < n && p >= start && !marked[p - s0]) {
                     if (parents == (uint32_t)kWarpParentSlots) { end = c; break; }
-                    marked[p] = 1; ++parents;
+                    marked[p - s0] = 1; ++parents;
                 }
             }
         }
@@ -486,148 +482,378 @@ static int32_t build_plan(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, 
         for (uint32_t part = 0; part < (cut ? 2u : 1u); ++part) {
             const uint32_t b = (part == 0) ? start : start + cut, e = (cut && part == 0) ? start + cut : end;
             Tile t; t.base = b; t.n_rows = (uint16_t)(e - b); t.n_levels = 1; t.warp_sync_mask = 0xFFFFFFFFu; t.top_levels = 0; t.lvl_warps = 0;
-            for (uint32_t r = b; r < e; ++r) tile_of[r] = (uint32_t)tiles.size();
             tiles.push_back(t);
         }
         start = end;
     }
-    // rows with children IN THEIR OWN TILE (a child in a later tile reads its parent from HBM, an earlier pass)
-    std::vector<uint8_t> has_children(n, 0), has_local_children(n, 0);
-    for (uint32_t r = 0; r < n; ++r)
-        if (parent[r] < n) { has_children[parent[r]] = 1; if (tile_of[parent[r]] == tile_of[r]) has_local_children[parent[r]] = 1; }
+}
+
+// Plans one tile (t.base, t.n_rows set): the topo / wtopo words of its rows, its level data, schedule and warp work item,
+// and the tiles of its out-of-tile parents (sorted, unique).  T_HAS_CHILDREN is "has a child anywhere" (n_children[r] > 0);
+// tile_of(p) gives the tile of a row before t.base.  Returns the rows with an out-of-tile parent, or -1 when the rows with
+// in-tile children exceed the warp kernel's kWarpParentSlots (only an edit can produce such a tile: the tiler cuts before).
+template <class TileOf>
+static int64_t plan_tile(const uint32_t *parent, const uint32_t *n_children, TileOf tile_of, Tile &t, WarpTile &w,
+                         uint32_t creation_index, uint8_t *sch, uint32_t *topo, uint32_t *wtopo, std::vector<uint32_t> &ext) {
+    const uint32_t b = t.base, nr = t.n_rows;
+    t.n_levels = 1; t.warp_sync_mask = 0xFFFFFFFFu; t.top_levels = 0; t.lvl_warps = 0;
+    uint32_t ldepth[kTileRows];
+    uint8_t local_kids[kTileRows] = {};   // rows with children IN THEIR OWN TILE (a child in a later tile reads its parent from HBM)
+    ext.clear();
+    int64_t n_ext = 0;
     // topo words, in-tile depth, tile levels
-    topo.assign(n, 0);
-    plan.n_ext = 0;
-    std::vector<uint32_t> ldepth(n, 0), tile_level(tiles.size(), 0);
-    for (uint32_t r = 0; r < n; ++r) {
-        const uint32_t p = parent[r], ti = tile_of[r];
-        uint32_t w = 0;
-        if (p == kNoParent) w |= T_ROOT;
-        else if (p == kDetached) w |= T_DETACHED;
-        else if (tile_of[p] == ti) {
-            ldepth[r] = ldepth[p] + 1;
-            w |= (p - tiles[ti].base) | (ldepth[r] << 9);
-            tiles[ti].n_levels = std::max<uint16_t>(tiles[ti].n_levels, (uint16_t)(ldepth[r] + 1));
+    for (uint32_t i = 0; i < nr; ++i) {
+        const uint32_t r = b + i, p = parent[r];
+        uint32_t wd = 0;
+        ldepth[i] = 0;
+        if (p == kNoParent) wd |= T_ROOT;
+        else if (p == kDetached) wd |= T_DETACHED;
+        else if (p >= b) {
+            ldepth[i] = ldepth[p - b] + 1;
+            local_kids[p - b] = 1;
+            wd |= (p - b) | (ldepth[i] << 9);
+            t.n_levels = std::max<uint16_t>(t.n_levels, (uint16_t)(ldepth[i] + 1));
             // a level keeps its warp-sync bit only while every parent->child edge into it stays inside one warp
-            if (ldepth[r] < 32 && ((p - tiles[ti].base) >> 5) != ((r - tiles[ti].base) >> 5))
-                tiles[ti].warp_sync_mask &= ~(1u << ldepth[r]);
+            if (ldepth[i] < 32 && ((p - b) >> 5) != (i >> 5)) t.warp_sync_mask &= ~(1u << ldepth[i]);
         } else {
-            w |= T_EXT_PARENT;
-            ++plan.n_ext;
-            tile_level[ti] = std::max(tile_level[ti], tile_level[tile_of[p]] + 1);
+            wd |= T_EXT_PARENT;
+            ++n_ext;
+            ext.push_back(tile_of(p));
         }
-        if (has_children[r]) w |= T_HAS_CHILDREN;
-        topo[r] = w;
+        if (n_children[r]) wd |= T_HAS_CHILDREN;
+        topo[i] = wd;
     }
+    std::sort(ext.begin(), ext.end());
+    ext.erase(std::unique(ext.begin(), ext.end()), ext.end());
     {   // top_levels: the leading depth levels whose rows all sit among the tile's first 32 rows
-        std::vector<uint32_t> max_local;
-        for (size_t ti = 0; ti < tiles.size(); ++ti) {
-            Tile &t = tiles[ti];
-            max_local.assign(t.n_levels, 0);
-            for (uint32_t r = t.base; r < t.base + t.n_rows; ++r) max_local[ldepth[r]] = std::max(max_local[ldepth[r]], r - t.base);
-            uint32_t K = 0;
-            while (K < t.n_levels && max_local[K] < 32u) ++K;
-            static int cap_env = -1;      // B200VIS_TOP_LEVELS_CAP: how many levels the scout may take (experiment knob)
-            if (cap_env < 0) { const char *e = getenv("B200VIS_TOP_LEVELS_CAP"); cap_env = e ? atoi(e) : 255; }
-            if (K > (uint32_t)cap_env) K = (uint32_t)cap_env;
-            t.top_levels = (t.n_levels > 1) ? K : 0u;       // flat tiles have nothing to walk ahead
-        }
+        uint32_t max_local[kTileRows] = {};
+        for (uint32_t i = 0; i < nr; ++i) max_local[ldepth[i]] = std::max(max_local[ldepth[i]], i);
+        uint32_t K = 0;
+        while (K < t.n_levels && max_local[K] < 32u) ++K;
+        static int cap_env = -1;      // B200VIS_TOP_LEVELS_CAP: how many levels the scout may take (experiment knob)
+        if (cap_env < 0) { const char *e = getenv("B200VIS_TOP_LEVELS_CAP"); cap_env = e ? atoi(e) : 255; }
+        if (K > (uint32_t)cap_env) K = (uint32_t)cap_env;
+        t.top_levels = (t.n_levels > 1) ? K : 0u;       // flat tiles have nothing to walk ahead
     }
     {   // lvl_warps: which warps meet at which level hand-over (named barriers, k_propagate_cull_tma)
         static int level_sync = -1;     // B200VIS_LEVEL_SYNC=cta: keep the CTA-wide level barriers (A/B switch)
         if (level_sync < 0) { const char *e = getenv("B200VIS_LEVEL_SYNC"); level_sync = (e && e[0] == 'c') ? 0 : 1; }
-        for (size_t ti = 0; level_sync && ti < tiles.size(); ++ti) {
-            Tile &t = tiles[ti];
-            if (t.n_levels < 2 || t.n_levels > 8) continue;      // seven barrier ids per tile parity (levels 1..7)
+        if (level_sync && t.n_levels >= 2 && t.n_levels <= 8) {      // seven barrier ids per tile parity (levels 1..7)
             uint32_t lv[kTileRows / 32] = {};          // per warp: bit l = the warp holds a row of in-tile depth l (a detached
-            for (uint32_t r = t.base; r < t.base + t.n_rows; ++r)      // row has depth 0: it publishes "not visited" to its children)
-                lv[(r - t.base) >> 5] |= 1u << ldepth[r];
+            for (uint32_t i = 0; i < nr; ++i)          // row has depth 0: it publishes "not visited" to its children)
+                lv[i >> 5] |= 1u << ldepth[i];
             unsigned long long packed = 0;
             for (uint32_t l = 1; l < t.n_levels; ++l) {
                 unsigned long long c = 0;
-                for (uint32_t w = 0; w < (uint32_t)kTileRows / 32u; ++w) c += ((lv[w] >> (l - 1)) & 3u) ? 1u : 0u;
+                for (uint32_t wi = 0; wi < (uint32_t)kTileRows / 32u; ++wi) c += ((lv[wi] >> (l - 1)) & 3u) ? 1u : 0u;
                 packed |= c << (4u * l);
             }
             t.lvl_warps = packed;
         }
     }
-    // ---- warp work items: schedule, parent slots, wtopo ------------------------------------------------------------
-    std::vector<WarpTile> wtiles(tiles.size());
-    std::vector<uint8_t> sched_all(tiles.size() * (size_t)kTileRows, 0xFF);
-    plan.wtopo.assign(n, 0);
-    {
-        std::vector<uint32_t> slot_of(n, 0);     // parent slot of the rows with in-tile children
-        std::vector<uint32_t> level_count, order;
-        for (size_t ti = 0; ti < tiles.size(); ++ti) {
-            const Tile &t = tiles[ti];
-            const uint32_t b = t.base, nr = t.n_rows;
-            // rows in (depth, row) order: counting sort by in-tile depth
-            level_count.assign((size_t)t.n_levels + 1, 0);
-            for (uint32_t r = b; r < b + nr; ++r) level_count[ldepth[r] + 1]++;
-            for (uint32_t l = 0; l < t.n_levels; ++l) level_count[l + 1] += level_count[l];
-            order.assign(nr, 0);
-            { std::vector<uint32_t> cur(level_count.begin(), level_count.end() - 1);
-              for (uint32_t r = b; r < b + nr; ++r) order[cur[ldepth[r]]++] = r - b; }
-            // slots: a level with >= 32 rows starts on a chunk boundary when the padding still fits into kTileRows slots
-            uint8_t *sch = sched_all.data() + ti * (size_t)kTileRows;
-            uint32_t pos = 0, next_slot = 0;
-            for (uint32_t l = 0; l < t.n_levels; ++l) {
-                const uint32_t lb = level_count[l], le = level_count[l + 1], cnt = le - lb;
-                if ((pos & 31u) && cnt >= 32u) {
-                    const uint32_t padded = (pos + 31u) & ~31u;
-                    if (padded + (nr - lb) <= (uint32_t)kTileRows) pos = padded;
-                }
-                for (uint32_t i = lb; i < le; ++i) {
-                    const uint32_t r = b + order[i];
-                    sch[pos++] = (uint8_t)order[i];
-                    if (has_local_children[r]) slot_of[r] = next_slot++;
-                }
-            }
-            WarpTile &w = wtiles[ti];
-            memset(&w, 0, sizeof w);
-            w.base = b; w.n_rows = (uint16_t)nr; w.n_chunks = (uint8_t)((pos + 31u) / 32u); w.sched = (uint32_t)ti;
-            for (uint32_t c = 0; c < w.n_chunks; ++c) {
-                bool contig = true; int64_t delta = 0; bool have = false;
-                for (uint32_t lane = 0; lane < 32; ++lane) {
-                    const uint8_t lr = sch[c * 32 + lane];
-                    if (lr == 0xFF && nr != (uint32_t)kTileRows) continue;   // padding (a full tile has none: 0xFF is row 255)
-                    const int64_t d = (int64_t)lr - (int64_t)lane;
-                    if (!have) { delta = d; have = true; } else if (d != delta) contig = false;
-                    if (ldepth[b + lr] > 0) w.nonroot[c] |= 1u << lane;
-                }
-                if (contig) w.contig |= (uint8_t)(1u << c);
-            }
+    // ---- warp work item: schedule, parent slots, wtopo -------------------------------------------------------------
+    // rows in (depth, row) order: counting sort by in-tile depth
+    uint32_t level_count[kTileRows + 1] = {}, order[kTileRows], slot_of[kTileRows] = {};
+    for (uint32_t i = 0; i < nr; ++i) level_count[ldepth[i] + 1]++;
+    for (uint32_t l = 0; l < t.n_levels; ++l) level_count[l + 1] += level_count[l];
+    { uint32_t cur[kTileRows];
+      for (uint32_t l = 0; l < t.n_levels; ++l) cur[l] = level_count[l];
+      for (uint32_t i = 0; i < nr; ++i) order[cur[ldepth[i]]++] = i; }
+    // slots: a level with >= 32 rows starts on a chunk boundary when the padding still fits into kTileRows slots
+    memset(sch, 0xFF, kTileRows);
+    uint32_t pos = 0, next_slot = 0;
+    for (uint32_t l = 0; l < t.n_levels; ++l) {
+        const uint32_t lb = level_count[l], le = level_count[l + 1], cnt = le - lb;
+        if ((pos & 31u) && cnt >= 32u) {
+            const uint32_t padded = (pos + 31u) & ~31u;
+            if (padded + (nr - lb) <= (uint32_t)kTileRows) pos = padded;
         }
-        for (uint32_t r = 0; r < n; ++r) {
-            uint32_t w = topo[r] & 0xF0000000u;      // T_HAS_CHILDREN stays the reference's "has a Children component"
-            if (has_local_children[r]) w |= W_HAS_SLOT | (slot_of[r] << 8);
-            w |= ldepth[r] & 0xFFu;
-            if (ldepth[r]) w |= slot_of[parent[r]] << 15;
-            plan.wtopo[r] = w;
+        for (uint32_t i = lb; i < le; ++i) {
+            sch[pos++] = (uint8_t)order[i];
+            if (local_kids[order[i]]) slot_of[order[i]] = next_slot++;
         }
     }
-    // NOTE: tile_level of tile t only depends on tiles with a smaller index (topological rows), and
-    // those are final by the time a row of t is visited, because rows are visited in ascending order.
-    const uint32_t n_pass = tiles.empty() ? 0 : *std::max_element(tile_level.begin(), tile_level.end()) + 1;
-    pass_begin.assign(n_pass + 1, 0);
-    for (uint32_t lv : tile_level) pass_begin[lv + 1]++;
-    for (uint32_t p = 0; p < n_pass; ++p) pass_begin[p + 1] += pass_begin[p];
-    tiles_sorted.resize(tiles.size());
-    plan.wtiles.resize(tiles.size());
-    std::vector<uint32_t> cursor(pass_begin.begin(), pass_begin.end() - (n_pass ? 1 : 0));
-    if (pass_small) pass_small->assign(n_pass, 0);
-    // within a pass: the small tiles (<= 32 rows, only produced by the split above) first, then the rest
-    for (int small = 1; small >= 0; --small)
-        for (size_t i = 0; i < tiles.size(); ++i) {
-            const bool is_small = split_deep && tiles[i].n_rows <= 32;
-            if ((int)is_small != small) continue;
-            const uint32_t at = cursor[tile_level[i]]++;
-            tiles_sorted[at] = tiles[i];
-            plan.wtiles[at] = wtiles[i];       // .sched keeps pointing at the tile's block in creation order
-            if (is_small && pass_small) (*pass_small)[tile_level[i]]++;
+    if (next_slot > (uint32_t)kWarpParentSlots) return -1;
+    memset(&w, 0, sizeof w);
+    w.base = b; w.n_rows = (uint16_t)nr; w.n_chunks = (uint8_t)((pos + 31u) / 32u); w.sched = creation_index;
+    for (uint32_t c = 0; c < w.n_chunks; ++c) {
+        bool contig = true; int64_t delta = 0; bool have = false;
+        for (uint32_t lane = 0; lane < 32; ++lane) {
+            const uint8_t lr = sch[c * 32 + lane];
+            if (lr == 0xFF && nr != (uint32_t)kTileRows) continue;   // padding (a full tile has none: 0xFF is row 255)
+            const int64_t d = (int64_t)lr - (int64_t)lane;
+            if (!have) { delta = d; have = true; } else if (d != delta) contig = false;
+            if (ldepth[lr] > 0) w.nonroot[c] |= 1u << lane;
         }
-    plan.sched.swap(sched_all);
+        if (contig) w.contig |= (uint8_t)(1u << c);
+    }
+    for (uint32_t i = 0; i < nr; ++i) {
+        uint32_t wd = topo[i] & 0xF0000000u;      // T_HAS_CHILDREN stays the reference's "has a Children component"
+        if (local_kids[i]) wd |= W_HAS_SLOT | (slot_of[i] << 8);
+        wd |= ldepth[i] & 0xFFu;
+        if (ldepth[i]) wd |= slot_of[parent[b + i] - b] << 15;
+        wtopo[i] = wd;
+    }
+    return n_ext;
+}
+
+// Passes from the tile graph (a tile runs one pass after the latest of its out-of-tile parents' tiles), then the tiles
+// sorted by pass.  O(tiles + external edges): a parent row precedes its children, so ext tiles have smaller indices.
+static void order_passes(Plan &plan) {
+    const size_t T = plan.tiles_c.size();
+    plan.level.assign(T, 0);
+    for (size_t ti = 0; ti < T; ++ti)
+        for (uint32_t e : plan.ext[ti]) plan.level[ti] = std::max(plan.level[ti], plan.level[e] + 1);
+    const uint32_t n_pass = T ? *std::max_element(plan.level.begin(), plan.level.end()) + 1 : 0;
+    plan.pass_begin.assign(n_pass + 1, 0);
+    for (uint32_t lv : plan.level) plan.pass_begin[lv + 1]++;
+    for (uint32_t p = 0; p < n_pass; ++p) plan.pass_begin[p + 1] += plan.pass_begin[p];
+    plan.tiles.resize(T);
+    plan.wtiles.resize(T);
+    std::vector<uint32_t> cursor(plan.pass_begin.begin(), plan.pass_begin.end() - (n_pass ? 1 : 0));
+    plan.pass_small.assign(n_pass, 0);
+    // within a pass: the small tiles (<= 32 rows, only produced by B200VIS_SPLIT_DEEP_TILES) first, then the rest
+    const bool split_deep = split_deep_tiles();
+    for (int small = 1; small >= 0; --small)
+        for (size_t i = 0; i < T; ++i) {
+            const bool is_small = split_deep && plan.tiles_c[i].n_rows <= 32;
+            if ((int)is_small != small) continue;
+            const uint32_t at = cursor[plan.level[i]]++;
+            plan.tiles[at] = plan.tiles_c[i];
+            plan.wtiles[at] = plan.wtiles_c[i];       // .sched keeps pointing at the tile's block in creation order
+            if (is_small) plan.pass_small[plan.level[i]]++;
+        }
+}
+
+// Validates the hierarchy (range, cycles), cuts the rows into tiles of <= kTileRows rows --
+// preferring cuts at tree boundaries so parents sit in the same tile as their children -- and
+// orders the tiles into passes so that a tile's out-of-tile parents are finished by an earlier
+// launch.  Forests of small trees need one pass; a tree larger than a tile needs a few.
+static int32_t build_plan(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, uint32_t cap, Plan &plan) {
+    if (cap < 32) cap = 32;
+    if (cap > (uint32_t)kTileRows) cap = kTileRows;
+    for (uint32_t r = 0; r < n; ++r) {
+        const uint32_t p = parent[r];
+        if (p == kNoParent || p == kDetached) continue;
+        if (p >= n) return fail(ctx, B200VIS_ERR_PARENT_OUT_OF_RANGE, "row %u: parent %u out of range (n=%u)", r, p, n);
+    }
+    {   // cycle check: every chain must end at a root / detached row
+        std::vector<uint8_t> color(n, 0);
+        std::vector<uint32_t> path;
+        for (uint32_t r = 0; r < n; ++r) {
+            if (color[r]) continue;
+            path.clear();
+            uint32_t c = r;
+            while (true) {
+                if (color[c] == 2) break;
+                if (color[c] == 1) return fail(ctx, B200VIS_ERR_HIERARCHY_CYCLE, "hierarchy cycle through row %u", c);
+                color[c] = 1; path.push_back(c);
+                const uint32_t p = parent[c];
+                if (p >= n) break;
+                c = p;
+            }
+            for (uint32_t x : path) color[x] = 2;
+        }
+    }
+    for (uint32_t r = 0; r < n; ++r)
+        if (parent[r] < n && parent[r] >= r)
+            return fail(ctx, B200VIS_ERR_UNSUPPORTED,
+                        "row %u has parent %u >= itself: rows must be in topological order (use b200vis_plan_row_order)", r,
+                        parent[r]);
+    plan.cap = cap; plan.n = n; plan.n_dead = 0;
+    plan.tiles_c.clear();
+    cut_tiles(n, parent, 0, cap, plan.tiles_c);
+    const size_t T = plan.tiles_c.size();
+    plan.tile_of.resize(n);
+    for (size_t ti = 0; ti < T; ++ti)
+        for (uint32_t r = plan.tiles_c[ti].base; r < plan.tiles_c[ti].base + plan.tiles_c[ti].n_rows; ++r) plan.tile_of[r] = (uint32_t)ti;
+    plan.n_children.assign(n, 0);
+    for (uint32_t r = 0; r < n; ++r) if (parent[r] < n) plan.n_children[parent[r]]++;
+    plan.topo.resize(n); plan.wtopo.resize(n);
+    plan.wtiles_c.resize(T);
+    plan.sched.assign(T * (size_t)kTileRows, 0xFF);
+    plan.ext.assign(T, {});
+    plan.n_ext = 0;
+    const uint32_t *tile_of = plan.tile_of.data();
+    for (size_t ti = 0; ti < T; ++ti) {
+        const uint32_t b = plan.tiles_c[ti].base;
+        plan.n_ext += (uint32_t)plan_tile(parent, plan.n_children.data(), [tile_of](uint32_t p) { return tile_of[p]; }, plan.tiles_c[ti],
+                                          plan.wtiles_c[ti], (uint32_t)ti, plan.sched.data() + ti * (size_t)kTileRows,
+                                          plan.topo.data() + b, plan.wtopo.data() + b, plan.ext[ti]);
+    }
+    order_passes(plan);
     return B200VIS_OK;
+}
+
+// ---- incremental re-planning (b200vis_edit_topology) ----------------------------------------------------------------
+struct TopologyEdit {
+    uint32_t n_despawn; const uint32_t *despawn;
+    uint32_t n_reparent; const uint32_t *reparent; const uint32_t *new_parent;
+    uint32_t n_spawn; const uint32_t *spawn_parent;
+};
+struct EditResult {
+    std::vector<uint32_t> tiles;                           // re-planned tiles (creation index), ascending
+    std::vector<std::pair<uint32_t, uint32_t>> ranges;     // their row ranges [first, end), ascending and disjoint
+    uint32_t rows = 0;                                     // rows re-planned
+};
+
+// Applies one frame's despawns, reparents and spawns to the plan, re-planning only the tiles they touch: the tiles
+// holding a despawned or reparented row, the tiles of parents that gain their first or lose their last child, and for
+// spawns the last tile (if not full) together with the appended rows, cut by the same greedy tiler.  Host work is
+// O(edited rows + re-planned tiles x kTileRows + tiles).  All or nothing: on error `hp` is unchanged.
+static int32_t edit_plan(b200vis_ctx *ctx, Plan &hp, uint32_t max_rows, const TopologyEdit &ed, EditResult &res) {
+    const uint32_t n = hp.n, n2 = n + ed.n_spawn;
+    if ((uint64_t)n + ed.n_spawn > max_rows)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "edit_topology: %u + %u rows exceed max_entities %u", n, ed.n_spawn, max_rows);
+    if (split_deep_tiles()) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "edit_topology: not with B200VIS_SPLIT_DEEP_TILES");
+    // ---- validation (nothing is touched) ----
+    std::vector<uint32_t> ds(ed.despawn, ed.despawn + ed.n_despawn);
+    std::sort(ds.begin(), ds.end());
+    auto despawned = [&](uint32_t r) { return std::binary_search(ds.begin(), ds.end(), r); };
+    for (size_t i = 0; i < ds.size(); ++i) {
+        if (ds[i] >= n || !hp.alive[ds[i]]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: despawned row %u is out of range or dead", ds[i]);
+        if (i && ds[i] == ds[i - 1]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: row %u is despawned twice", ds[i]);
+    }
+    {   // despawn is recursive: every live child of a despawned row is despawned in the same call
+        std::vector<uint32_t> kids(ds.size(), 0);
+        for (uint32_t d : ds) {
+            const uint32_t p = hp.parent[d];
+            if (p < n && despawned(p)) kids[std::lower_bound(ds.begin(), ds.end(), p) - ds.begin()]++;
+        }
+        for (size_t i = 0; i < ds.size(); ++i)
+            if (kids[i] != hp.n_children[ds[i]])
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: despawned row %u keeps %u live children (despawn them too, or reparent them first)",
+                            ds[i], hp.n_children[ds[i]] - kids[i]);
+    }
+    {
+        std::vector<uint32_t> rp(ed.reparent, ed.reparent + ed.n_reparent);
+        std::sort(rp.begin(), rp.end());
+        for (size_t i = 1; i < rp.size(); ++i)
+            if (rp[i] == rp[i - 1]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: row %u is reparented twice", rp[i]);
+    }
+    for (uint32_t j = 0; j < ed.n_reparent; ++j) {
+        const uint32_t r = ed.reparent[j], p = ed.new_parent[j];
+        if (r >= n || !hp.alive[r] || despawned(r)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: reparented row %u is out of range or dead", r);
+        if (p == kNoParent || p == kDetached) continue;
+        if (p >= n) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: new parent %u of row %u is out of range", p, r);
+        if (p >= r) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "edit_topology: new parent %u of row %u breaks the row order (compact with set_topology)", p, r);
+        if (!hp.alive[p] || despawned(p)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: new parent %u of row %u is dead", p, r);
+    }
+    for (uint32_t k = 0; k < ed.n_spawn; ++k) {
+        const uint32_t r = n + k, p = ed.spawn_parent[k];
+        if (p == kNoParent || p == kDetached) continue;
+        if (p >= n2) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: parent %u of spawned row %u is out of range", p, r);
+        if (p >= r) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "edit_topology: parent %u of spawned row %u is a later row of the batch", p, r);
+        if (p < n && (!hp.alive[p] || despawned(p))) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: parent %u of spawned row %u is dead", p, r);
+    }
+    // ---- apply to the hierarchy (undone if a re-planned tile turns out unplannable) ----
+    std::vector<std::pair<uint32_t, uint32_t>> old_parent;          // (row, parent before the edit)
+    std::vector<uint32_t> dirty;
+    auto touch_parent = [&](uint32_t p, int delta) {                 // a parent gains / loses a child
+        if (p >= n2) return;
+        const uint32_t before = hp.n_children[p];
+        hp.n_children[p] = before + delta;
+        if (p < n && ((before == 0) != (hp.n_children[p] == 0))) dirty.push_back(hp.tile_of[p]);   // T_HAS_CHILDREN flips
+    };
+    hp.parent.resize(n2); hp.alive.resize(n2, 1); hp.n_children.resize(n2, 0);
+    for (uint32_t d : ds) {
+        old_parent.emplace_back(d, hp.parent[d]);
+        touch_parent(hp.parent[d], -1);
+        hp.parent[d] = kDetached; hp.alive[d] = 0;
+        dirty.push_back(hp.tile_of[d]);
+    }
+    for (uint32_t j = 0; j < ed.n_reparent; ++j) {
+        const uint32_t r = ed.reparent[j];
+        old_parent.emplace_back(r, hp.parent[r]);
+        touch_parent(hp.parent[r], -1);
+        hp.parent[r] = ed.new_parent[j];
+        touch_parent(hp.parent[r], +1);
+        dirty.push_back(hp.tile_of[r]);
+    }
+    for (uint32_t k = 0; k < ed.n_spawn; ++k) {
+        hp.parent[n + k] = ed.spawn_parent[k];
+        touch_parent(ed.spawn_parent[k], +1);
+    }
+    auto undo = [&]() {
+        for (size_t i = old_parent.size(); i-- > 0;) {
+            const uint32_t r = old_parent[i].first;
+            touch_parent(hp.parent[r], -1);
+            hp.parent[r] = old_parent[i].second;
+            touch_parent(hp.parent[r], +1);
+            hp.alive[r] = 1;
+        }
+        for (uint32_t k = 0; k < ed.n_spawn; ++k) touch_parent(ed.spawn_parent[k], -1);
+        hp.parent.resize(n); hp.alive.resize(n); hp.n_children.resize(n);
+    };
+    // ---- re-plan ----
+    const uint32_t T = (uint32_t)hp.tiles_c.size();
+    uint32_t sfx_tile = T, s = n;            // spawns: tiles [sfx_tile, ...) are cut again from row s
+    if (ed.n_spawn && T && hp.tiles_c[T - 1].n_rows < hp.cap) { sfx_tile = T - 1; s = hp.tiles_c[T - 1].base; }
+    std::sort(dirty.begin(), dirty.end());
+    dirty.erase(std::unique(dirty.begin(), dirty.end()), dirty.end());
+    while (!dirty.empty() && dirty.back() >= sfx_tile) dirty.pop_back();
+    std::vector<Tile> sfx;
+    if (ed.n_spawn) cut_tiles(n2, hp.parent.data(), s, hp.cap, sfx);
+    std::vector<uint32_t> sfx_tile_of(n2 - s);
+    for (size_t i = 0; i < sfx.size(); ++i)
+        for (uint32_t r = sfx[i].base; r < sfx[i].base + sfx[i].n_rows; ++r) sfx_tile_of[r - s] = sfx_tile + (uint32_t)i;
+    const uint32_t *tile_of = hp.tile_of.data(), *sto = sfx_tile_of.data();
+    auto tile_of_row = [tile_of, sto, s](uint32_t p) { return p >= s ? sto[p - s] : tile_of[p]; };
+    const size_t n_new = dirty.size() + sfx.size();
+    std::vector<Tile> nt(n_new);
+    std::vector<WarpTile> nw(n_new);
+    std::vector<std::vector<uint32_t>> next(n_new);
+    std::vector<uint8_t> nsched(n_new * (size_t)kTileRows);
+    std::vector<uint32_t> ntopo, nwtopo;
+    uint32_t rows = 0;
+    for (size_t i = 0; i < n_new; ++i) rows += i < dirty.size() ? hp.tiles_c[dirty[i]].n_rows : sfx[i - dirty.size()].n_rows;
+    ntopo.resize(rows); nwtopo.resize(rows);
+    for (size_t i = 0, at = 0; i < n_new; ++i) {
+        const bool d = i < dirty.size();
+        nt[i] = d ? hp.tiles_c[dirty[i]] : sfx[i - dirty.size()];
+        const uint32_t ci = d ? dirty[i] : sfx_tile + (uint32_t)(i - dirty.size());
+        if (plan_tile(hp.parent.data(), hp.n_children.data(), tile_of_row, nt[i], nw[i], ci, nsched.data() + i * (size_t)kTileRows,
+                      ntopo.data() + at, nwtopo.data() + at, next[i]) < 0) {
+            undo();
+            return fail(ctx, B200VIS_ERR_UNSUPPORTED, "edit_topology: tile at row %u would need more than %d parent slots (compact with set_topology)",
+                        nt[i].base, kWarpParentSlots);
+        }
+        at += nt[i].n_rows;
+    }
+    // ---- commit ----
+    hp.tiles_c.resize(sfx_tile + sfx.size()); hp.wtiles_c.resize(sfx_tile + sfx.size()); hp.ext.resize(sfx_tile + sfx.size());
+    hp.sched.resize(hp.tiles_c.size() * (size_t)kTileRows);
+    hp.topo.resize(n2); hp.wtopo.resize(n2); hp.tile_of.resize(n2);
+    for (uint32_t r = s; r < n2; ++r) hp.tile_of[r] = sfx_tile_of[r - s];
+    res.tiles.clear(); res.ranges.clear(); res.rows = rows;
+    for (size_t i = 0, at = 0; i < n_new; ++i) {
+        const uint32_t ci = i < dirty.size() ? dirty[i] : sfx_tile + (uint32_t)(i - dirty.size());
+        hp.tiles_c[ci] = nt[i]; hp.wtiles_c[ci] = nw[i]; hp.ext[ci].swap(next[i]);
+        memcpy(hp.sched.data() + (size_t)ci * kTileRows, nsched.data() + i * (size_t)kTileRows, kTileRows);
+        memcpy(hp.topo.data() + nt[i].base, ntopo.data() + at, nt[i].n_rows * 4u);
+        memcpy(hp.wtopo.data() + nt[i].base, nwtopo.data() + at, nt[i].n_rows * 4u);
+        at += nt[i].n_rows;
+        res.tiles.push_back(ci);
+        if (!res.ranges.empty() && res.ranges.back().second == nt[i].base) res.ranges.back().second += nt[i].n_rows;
+        else res.ranges.emplace_back(nt[i].base, nt[i].base + nt[i].n_rows);
+    }
+    hp.n = n2; hp.n_dead += (uint32_t)ds.size();
+    hp.n_ext = 0;     // not tracked across edits (only set_topology's choice of tile size reads it)
+    order_passes(hp);
+    return B200VIS_OK;
+}
+
+static void free_plan(Plan *p) { delete p; }
+
+// the pass ranges of a plan, and which passes may run the named-barrier schedule
+static void install_passes(b200vis_ctx *ctx, const Plan &plan) {
+    const std::vector<uint32_t> &pass_begin = plan.pass_begin;
+    ctx->pass_begin = pass_begin;
+    ctx->pass_small = plan.pass_small;
+    ctx->pass_named.assign(pass_begin.empty() ? 0 : pass_begin.size() - 1, 1);
+    for (size_t pi = 0; pi + 1 < pass_begin.size(); ++pi)
+        for (uint32_t ti = pass_begin[pi]; ti < pass_begin[pi + 1]; ++ti)
+            if (plan.tiles[ti].n_levels > 1 && plan.tiles[ti].lvl_warps == 0ull) { ctx->pass_named[pi] = 0; break; }
 }
 
 extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, const uint64_t *entity_bits) {
@@ -651,7 +877,6 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         }
     }
     std::vector<uint32_t> &topo = plan.topo; std::vector<Tile> &tiles = plan.tiles;
-    std::vector<uint32_t> &pass_begin = plan.pass_begin, &pass_small = plan.pass_small;
     if (tiles.size() > ctx->tiles_cap) {
         void *old[] = {ctx->d_tiles, ctx->d_wtiles, ctx->d_sched};
         for (void *q : old) if (q) cudaFree(q);
@@ -682,12 +907,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         CU(cudaMemcpy(ctx->d_rank, rank.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
         CU(cudaMemcpy(ctx->d_row_of_rank, order.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
     }
-    ctx->pass_begin = pass_begin;
-    ctx->pass_small = pass_small;
-    ctx->pass_named.assign(pass_begin.empty() ? 0 : pass_begin.size() - 1, 1);
-    for (size_t pi = 0; pi + 1 < pass_begin.size(); ++pi)
-        for (uint32_t ti = pass_begin[pi]; ti < pass_begin[pi + 1]; ++ti)
-            if (tiles[ti].n_levels > 1 && tiles[ti].lvl_warps == 0ull) { ctx->pass_named[pi] = 0; break; }
+    install_passes(ctx, plan);
     ctx->rank_identity = sorted;
     ctx->n = n;
     ctx->rows.n = n;
@@ -701,7 +921,233 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
     if (ctx->diff.prev) CU(cudaMemset(ctx->diff.prev, 0, (size_t)ctx->vis.words_stride * ctx->cfg.max_views * 4));   // ranks changed: old list = empty
     ctx->topology_set = true;
     ctx->gt_aos_valid = false;
+    {   // what b200vis_edit_topology starts from: the plan, and the keys in rank order (uploaded by the first merge)
+        if (!ctx->hplan) ctx->hplan = new Plan();
+        plan.parent.assign(parent, parent + n); plan.alive.assign(n, 1);
+        *ctx->hplan = std::move(plan);
+        ctx->h_keys.resize(n);
+        for (uint32_t i = 0; i < n; ++i) ctx->h_keys[i] = entity_bits[sorted ? i : order[i]];
+        ctx->keys_resident = false;
+        ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
+    }
     return B200VIS_OK;
+}
+
+static int32_t grow_edit_staging(b200vis_ctx *ctx, size_t bytes) {
+    if (bytes <= ctx->h_edit_bytes) return B200VIS_OK;
+    if (ctx->h_edit) cudaFreeHost(ctx->h_edit);
+    ctx->h_edit = nullptr; ctx->h_edit_bytes = 0;
+    bytes = std::max<size_t>(bytes, (size_t)1 << 20);
+    CU(cudaMallocHost(&ctx->h_edit, bytes));
+    ctx->h_edit_bytes = bytes;
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, const uint32_t *despawn_rows,
+                                         uint32_t n_reparent, const uint32_t *reparent_rows, const uint32_t *new_parent,
+                                         uint32_t n_spawn, const uint32_t *spawn_parent, const uint64_t *spawn_entity_bits) {
+    CHECK_CTX_JOIN();   // the tail of the frame in flight reads the rank arrays and the visible sets
+    if (!ctx->topology_set || !ctx->hplan) return fail(ctx, B200VIS_ERR_NOT_READY, "edit_topology: b200vis_set_topology has not been called");
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "edit_topology: world_size > 1 (use set_topology)");
+    if ((n_despawn && !despawn_rows) || (n_reparent && (!reparent_rows || !new_parent)) || (n_spawn && (!spawn_parent || !spawn_entity_bits)))
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: null array");
+    Plan &hp = *ctx->hplan;
+    const uint32_t n = ctx->n, n2 = n + n_spawn;
+    if ((uint64_t)n + n_spawn > ctx->cfg.max_entities)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "edit_topology: %u + %u rows exceed max_entities %u", n, n_spawn, ctx->cfg.max_entities);
+    cudaStream_t st = ctx->stream;
+    if (ctx->ev_edit) CU(cudaEventSynchronize(ctx->ev_edit));   // the last edit's staging copies have been read
+    else CU(cudaEventCreateWithFlags(&ctx->ev_edit, cudaEventDisableTiming));
+    // ---- ranks of the new keys: appended (rank == row stays true) or merged on the device ----
+    std::vector<uint32_t> ord(n_spawn);
+    std::iota(ord.begin(), ord.end(), 0u);
+    std::sort(ord.begin(), ord.end(), [&](uint32_t a, uint32_t b) { return spawn_entity_bits[a] < spawn_entity_bits[b]; });
+    for (uint32_t i = 1; i < n_spawn; ++i)
+        if (spawn_entity_bits[ord[i]] == spawn_entity_bits[ord[i - 1]])
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: entity bits %llx spawned twice", (unsigned long long)spawn_entity_bits[ord[i]]);
+    bool append = ctx->rank_identity;
+    for (uint32_t k = 0; k < n_spawn && append; ++k)
+        append = k ? spawn_entity_bits[k] > spawn_entity_bits[k - 1] : (n == 0 || spawn_entity_bits[0] > ctx->max_key);
+    const bool merge = n_spawn && !append;
+    const size_t keys_off = 0, rows_off = (size_t)n_spawn * 8, dup_off = rows_off + (((size_t)n_spawn * 4 + 15) & ~(size_t)15);
+    if (merge) {
+        const size_t N = ctx->cfg.max_entities;
+        if (!ctx->d_keys) CU(dalloc(&ctx->d_keys, N));
+        if (!ctx->d_keys2) { CU(dalloc(&ctx->d_keys2, N)); CU(dalloc(&ctx->d_rank2, N)); CU(dalloc(&ctx->d_row_of_rank2, N)); }
+        if (!ctx->keys_resident) {
+            CU(cudaStreamSynchronize(st));
+            CU(cudaMemcpy(ctx->d_keys, ctx->h_keys.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
+            ctx->keys_resident = true;
+            std::vector<uint64_t>().swap(ctx->h_keys);
+        }
+        int32_t rc = grow_edit_staging(ctx, dup_off + 16); if (rc) return rc;
+        uint64_t *hk = reinterpret_cast<uint64_t *>(ctx->h_edit + keys_off);
+        uint32_t *hr = reinterpret_cast<uint32_t *>(ctx->h_edit + rows_off);
+        uint32_t *hd = reinterpret_cast<uint32_t *>(ctx->h_edit + dup_off);
+        for (uint32_t j = 0; j < n_spawn; ++j) { hk[j] = spawn_entity_bits[ord[j]]; hr[j] = n + ord[j]; }
+        hd[0] = 0;
+        if (dup_off + 4 > ctx->stage_bytes) return fail(ctx, B200VIS_ERR_CAPACITY, "staging buffer too small");
+        CU(cudaMemcpyAsync(ctx->d_stage, ctx->h_edit, dup_off + 4, cudaMemcpyHostToDevice, st));
+        uint32_t *d_dup = reinterpret_cast<uint32_t *>(ctx->d_stage + dup_off);
+        launch_rank_merge(st, ctx->d_keys, ctx->rank_identity ? nullptr : ctx->d_row_of_rank, n,
+                          reinterpret_cast<const uint64_t *>(ctx->d_stage + keys_off), reinterpret_cast<const uint32_t *>(ctx->d_stage + rows_off),
+                          n_spawn, ctx->d_keys2, ctx->d_row_of_rank2, ctx->d_rank2, d_dup);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(hd, d_dup, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        if (hd[0]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: a spawned entity's bits equal those of an existing (live or dead) row");
+    }
+    if (n_despawn && (ctx->lights.n || !ctx->h_shadow.empty())) {   // a dead row must not go on being clustered or shadowed
+        std::vector<uint32_t> ds(despawn_rows, despawn_rows + n_despawn);
+        std::sort(ds.begin(), ds.end());
+        for (uint32_t i = 0; i < ctx->lights.n; ++i)
+            if (std::binary_search(ds.begin(), ds.end(), ctx->h_light_row[i]))
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: row %u is light %u: remove it with b200vis_set_lights first", ctx->h_light_row[i], i);
+        for (size_t i = 0; i < ctx->h_shadow.size(); ++i)
+            if (ctx->h_shadow[i].kind != B200VIS_SHADOW_DIRECTIONAL_CASCADE && std::binary_search(ds.begin(), ds.end(), ctx->h_shadow[i].row))
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: row %u is shadow item %zu: replace the shadow items first", ctx->h_shadow[i].row, i);
+    }
+    // ---- host plan ----
+    if (hp.tiles_c.size() + n_spawn > ctx->tiles_cap) {
+        // at most one new tile per spawned row.  Grown before the edit is validated, so the current plan is copied whole:
+        // if the edit then fails, the next frame runs the unchanged plan from the new buffers
+        const uint32_t cap = (uint32_t)std::max<size_t>(2 * (size_t)ctx->tiles_cap, hp.tiles_c.size() + n_spawn + 1024);
+        Tile *t = nullptr; WarpTile *w = nullptr; uint8_t *s = nullptr;
+        CU(dalloc(&t, cap)); CU(dalloc(&w, cap)); CU(dalloc(&s, (size_t)cap * kTileRows));
+        CU(cudaMemcpyAsync(t, ctx->d_tiles, hp.tiles.size() * sizeof(Tile), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(w, ctx->d_wtiles, hp.wtiles.size() * sizeof(WarpTile), cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemcpyAsync(s, ctx->d_sched, hp.tiles_c.size() * (size_t)kTileRows, cudaMemcpyDeviceToDevice, st));
+        CU(cudaStreamSynchronize(st));
+        cudaFree(ctx->d_tiles); cudaFree(ctx->d_wtiles); cudaFree(ctx->d_sched);
+        ctx->d_tiles = t; ctx->d_wtiles = w; ctx->d_sched = s; ctx->tiles_cap = cap;
+    }
+    const TopologyEdit ed{n_despawn, despawn_rows, n_reparent, reparent_rows, new_parent, n_spawn, spawn_parent};
+    EditResult er;
+    int32_t rc = edit_plan(ctx, hp, ctx->cfg.max_entities, ed, er);
+    if (rc) return rc;
+    // ---- commit: one pinned staging packet, async copies of the descriptors, the re-planned rows and schedule blocks ----
+    const size_t T = hp.tiles.size();
+    size_t bytes = T * (sizeof(Tile) + sizeof(WarpTile)) + (size_t)er.rows * 12 + er.tiles.size() * (size_t)kTileRows +
+                   ((size_t)n_despawn + n_reparent) * 4 + (append ? (size_t)n_spawn * 8 : 0) + 64;
+    rc = grow_edit_staging(ctx, bytes); if (rc) return rc;
+    uint8_t *h = ctx->h_edit;
+    size_t off = 0;
+    auto put = [&](void *dst, const void *src, size_t nb) -> int32_t {
+        if (!nb) return B200VIS_OK;
+        memcpy(h + off, src, nb);
+        CU(cudaMemcpyAsync(dst, h + off, nb, cudaMemcpyHostToDevice, st));
+        off += (nb + 15) & ~(size_t)15;
+        return B200VIS_OK;
+    };
+    if ((rc = put(ctx->d_tiles, hp.tiles.data(), T * sizeof(Tile)))) return rc;
+    if ((rc = put(ctx->d_wtiles, hp.wtiles.data(), T * sizeof(WarpTile)))) return rc;
+    for (const auto &rg : er.ranges) {
+        const size_t a = rg.first, c = (size_t)(rg.second - rg.first) * 4;
+        if ((rc = put(ctx->rows.topo + a, hp.topo.data() + a, c))) return rc;
+        if ((rc = put(ctx->d_wtopo + a, hp.wtopo.data() + a, c))) return rc;
+        if ((rc = put(ctx->d_parent + a, hp.parent.data() + a, c))) return rc;
+    }
+    for (uint32_t ci : er.tiles)
+        if ((rc = put(ctx->d_sched + (size_t)ci * kTileRows, hp.sched.data() + (size_t)ci * kTileRows, kTileRows))) return rc;
+    // row lists of the column kernel: through the device staging buffer (stream-ordered after the merge that used it)
+    const size_t lists = ((size_t)n_despawn + n_reparent) * 4;
+    if (lists > ctx->stage_bytes) return fail(ctx, B200VIS_ERR_CAPACITY, "staging buffer too small");
+    if ((rc = put(ctx->d_stage, despawn_rows, (size_t)n_despawn * 4))) return rc;
+    if ((rc = put(ctx->d_stage + (size_t)n_despawn * 4, reparent_rows, (size_t)n_reparent * 4))) return rc;
+    CU(cudaEventRecord(ctx->ev_edit, st));
+    RowEdit re{};
+    re.dead = reinterpret_cast<const uint32_t *>(ctx->d_stage); re.n_dead = n_despawn;
+    re.moved = reinterpret_cast<const uint32_t *>(ctx->d_stage + (size_t)n_despawn * 4); re.n_moved = n_reparent;
+    re.first_new = n; re.n_new = n_spawn;
+    re.cls = ctx->d_cls; re.caster = ctx->d_caster; re.visibility = ctx->d_visibility; re.vv_shadow = ctx->d_vv_shadow;
+    re.layers = ctx->have_layers ? ctx->d_layers : nullptr; re.layers_ext = ctx->d_layers_ext;
+    re.range = ctx->have_range ? ctx->d_range : nullptr; re.range_se = ctx->d_range_se; re.range_ua = ctx->d_range_ua;
+    Rows R = ctx->rows;
+    launch_edit_rows(st, R, re);
+    CU(cudaGetLastError());
+    // ---- ranks ----
+    if (merge) {
+        const uint32_t *old_rank = ctx->rank_identity ? nullptr : ctx->d_rank;
+        std::swap(ctx->d_keys, ctx->d_keys2); std::swap(ctx->d_rank, ctx->d_rank2); std::swap(ctx->d_row_of_rank, ctx->d_row_of_rank2);
+        if (ctx->diff.prev) {   // last frame's visible sets, bit = rank: to the new ranks (diff.words is free between frames)
+            const size_t words = (size_t)ctx->vis.words_stride * ctx->cfg.max_views;
+            CU(cudaMemcpyAsync(ctx->diff.words, ctx->diff.prev, words * 4, cudaMemcpyDeviceToDevice, st));
+            launch_remap_rank_sets(st, ctx->diff.words, ctx->diff.prev, ctx->vis.words_stride, ctx->cfg.max_views, (n2 + 31) / 32, n2, n,
+                                   ctx->d_row_of_rank, old_rank);
+            CU(cudaGetLastError());
+        }
+        ctx->rank_identity = false;
+    } else if (n_spawn) {
+        if (ctx->keys_resident) { if ((rc = put(ctx->d_keys + n, spawn_entity_bits, (size_t)n_spawn * 8))) return rc; CU(cudaEventRecord(ctx->ev_edit, st)); }
+        else ctx->h_keys.insert(ctx->h_keys.end(), spawn_entity_bits, spawn_entity_bits + n_spawn);
+    }
+    if (n_spawn) ctx->max_key = std::max(ctx->max_key, spawn_entity_bits[ord[n_spawn - 1]]);
+    install_passes(ctx, hp);
+    ctx->n = n2;
+    ctx->rows.n = n2;
+    ctx->vis.n_words = (n2 + 31) / 32;
+    // the visible masks are empty between frames and the chunk counters past the old row count were never written: growing
+    // n_words / n_chunks needs no clearing
+    ctx->vis.n_chunks = (ctx->vis.n_words + kChunkWords - 1) / kChunkWords;
+    ctx->gt_aos_valid = false;
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_topology_summary(const b200vis_ctx *ctx, uint32_t out[4]) {
+    if (!ctx || !out) return B200VIS_ERR_INVALID_ARG;
+    const Plan *hp = ctx->hplan;
+    out[0] = ctx->n;
+    out[1] = hp ? ctx->n - hp->n_dead : ctx->n;
+    out[2] = hp ? (uint32_t)hp->tiles.size() : 0u;
+    out[3] = ctx->pass_begin.empty() ? 0u : (uint32_t)ctx->pass_begin.size() - 1;
+    return B200VIS_OK;
+}
+
+// True when `row` is a despawned row (b200vis_edit_topology) that no compaction has dropped yet.
+static bool row_is_dead(const b200vis_ctx *ctx, uint32_t row) {
+    return ctx->hplan && row < ctx->hplan->n && !ctx->hplan->alive[row];
+}
+
+extern "C" int32_t b200vis_host_edit_plan(uint32_t n, const uint32_t *parent, uint32_t tile_rows, uint32_t max_rows, uint32_t script_words,
+                                          const uint32_t *script, uint32_t tiles_capacity, uint32_t *n_rows_out, uint32_t *n_tiles,
+                                          uint32_t *tile_desc, uint32_t *topo, uint32_t *wtopo, uint8_t *sched, uint32_t counters[4]) {
+    if ((n && !parent) || (script_words && !script) || !n_rows_out || !n_tiles || !counters) return B200VIS_ERR_INVALID_ARG;
+    Plan plan;
+    int32_t rc = build_plan(nullptr, n, parent, tile_rows ? tile_rows : kTileRows, plan);
+    if (rc) return rc;
+    plan.parent.assign(parent, parent + n); plan.alive.assign(n, 1);
+    counters[0] = counters[1] = counters[3] = 0;
+    for (uint32_t at = 0; at < script_words;) {
+        if (script_words - at < 3) { rc = fail(nullptr, B200VIS_ERR_INVALID_ARG, "host_edit_plan: truncated step header"); break; }
+        const uint32_t nd = script[at], nr = script[at + 1], ns = script[at + 2];
+        const uint64_t len = 3ull + nd + 2ull * nr + ns;
+        if (len > script_words - at) { rc = fail(nullptr, B200VIS_ERR_INVALID_ARG, "host_edit_plan: truncated step"); break; }
+        const uint32_t *a = script + at + 3;
+        const TopologyEdit ed{nd, a, nr, a + nd, a + nd + nr, ns, a + nd + 2 * nr};
+        EditResult er;
+        rc = edit_plan(nullptr, plan, max_rows, ed, er);
+        if (rc) break;
+        counters[0] = (uint32_t)er.tiles.size(); counters[1] = er.rows; counters[3]++;
+        at += (uint32_t)len;
+    }
+    counters[2] = plan.pass_begin.empty() ? 0u : (uint32_t)plan.pass_begin.size() - 1;
+    *n_rows_out = plan.n;
+    *n_tiles = (uint32_t)plan.tiles.size();
+    if (!tile_desc) return rc;
+    if (plan.tiles.size() > tiles_capacity || (plan.n && (!topo || !wtopo)) || !sched) return B200VIS_ERR_CAPACITY;
+    for (size_t p = 0; p + 1 < plan.pass_begin.size(); ++p)
+        for (uint32_t i = plan.pass_begin[p]; i < plan.pass_begin[p + 1]; ++i) {
+            const Tile &t = plan.tiles[i];
+            const WarpTile &w = plan.wtiles[i];
+            uint32_t *d = tile_desc + (size_t)i * 17;
+            d[0] = t.base; d[1] = t.n_rows; d[2] = t.n_levels; d[3] = t.warp_sync_mask; d[4] = t.top_levels;
+            d[5] = (uint32_t)t.lvl_warps; d[6] = (uint32_t)(t.lvl_warps >> 32); d[7] = (uint32_t)p;
+            d[8] = w.n_chunks | ((uint32_t)w.contig << 8);
+            memcpy(d + 9, w.nonroot, sizeof w.nonroot);
+            memcpy(sched + (size_t)i * kTileRows, plan.sched.data() + (size_t)w.sched * kTileRows, kTileRows);
+        }
+    if (plan.n) { memcpy(topo, plan.topo.data(), (size_t)plan.n * 4); memcpy(wtopo, plan.wtopo.data(), (size_t)plan.n * 4); }
+    return rc;
 }
 
 extern "C" int32_t b200vis_host_plan_summary(uint32_t n, const uint32_t *parent, uint32_t out[4]) {
@@ -975,7 +1421,8 @@ extern "C" int32_t b200vis_set_lights(b200vis_ctx *ctx, uint32_t n_lights, const
     if (n_lights > ctx->cfg.max_lights) return fail(ctx, B200VIS_ERR_CAPACITY, "set_lights: %u > max_lights %u", n_lights, ctx->cfg.max_lights);
     if (n_lights && (!light_row || !range)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_lights: null");
     for (uint32_t i = 0; i < n_lights; ++i)
-        if (light_row[i] >= ctx->cfg.max_entities) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_lights: light %u row %u out of range", i, light_row[i]);
+        if (light_row[i] >= ctx->cfg.max_entities || row_is_dead(ctx, light_row[i]))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_lights: light %u row %u out of range or despawned", i, light_row[i]);
     CU(cudaMemcpyAsync(ctx->d_light_row, light_row, (size_t)n_lights * 4, cudaMemcpyHostToDevice, ctx->stream));
     CU(cudaMemcpyAsync(ctx->d_light_range, range, (size_t)n_lights * 4, cudaMemcpyHostToDevice, ctx->stream));
     if (layer_mask) CU(cudaMemcpyAsync(ctx->d_light_layers, layer_mask, (size_t)n_lights * 8, cudaMemcpyHostToDevice, ctx->stream));
@@ -1671,8 +2118,8 @@ extern "C" int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, 
     for (uint32_t i = 0; i < n_items; ++i) {
         const b200vis_shadow_item &it = items[i];
         if (it.kind > B200VIS_SHADOW_DIRECTIONAL_CASCADE) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items: item %u has kind %u", i, it.kind);
-        if (it.kind != B200VIS_SHADOW_DIRECTIONAL_CASCADE && it.light_row >= ctx->n)
-            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items: item %u: light row %u out of range", i, it.light_row);
+        if (it.kind != B200VIS_SHADOW_DIRECTIONAL_CASCADE && (it.light_row >= ctx->n || row_is_dead(ctx, it.light_row)))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items: item %u: light row %u out of range or despawned", i, it.light_row);
         ShadowLight &s = ctx->h_shadow[i];
         memset(&s, 0, sizeof s);
         memcpy(s.planes, it.frusta, sizeof s.planes);

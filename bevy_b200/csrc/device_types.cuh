@@ -239,4 +239,15 @@ struct BindingBufs {
     uint32_t *count;         // [V][2] n_offsets, n_indices
 };
 
+// b200vis_edit_topology: the rows whose columns an edit rewrites (k_edit_rows); optional columns are nullptr when absent
+struct RowEdit {
+    const uint32_t *dead; uint32_t n_dead;      // despawned rows
+    const uint32_t *moved; uint32_t n_moved;    // reparented rows
+    uint32_t first_new, n_new;                  // spawned rows [first_new, first_new + n_new)
+    uint8_t *cls, *caster, *visibility, *vv_shadow, *range_ua;
+    uint64_t *layers, *layers_ext;
+    uint32_t *range;
+    float2 *range_se;
+};
+
 }  // namespace b200vis

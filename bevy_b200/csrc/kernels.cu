@@ -4208,6 +4208,113 @@ void launch_pack_state(cudaStream_t st, const Rows &R, uint32_t first, uint32_t 
     if (count) { ++g_launches; k_pack_state<<<cdiv(count, 256), 256, 0, st>>>(R, first, count, out, changed_bit); }
 }
 
+// ------------------------------------------------------------------------------------------
+// Topology edits (b200vis_edit_topology): the state of the device world carried over to the edited one.  None of these
+// runs per frame; each is one pass over device-resident arrays instead of a host round trip.
+// ------------------------------------------------------------------------------------------
+__device__ __forceinline__ uint32_t lower_bound_u64(const uint64_t *a, uint32_t n, uint64_t key) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < key) lo = mid + 1; else hi = mid; }
+    return lo;
+}
+constexpr uint32_t kMergeSmemKeys = 6144;   // new keys staged in shared memory (48 KB) up to this many
+// Rank merge: the world's keys in rank order (Entity::to_bits(), 8 B per row, dead rows included) and the batch's new keys
+// (sorted on the host) into one order.  Old rank i moves to i + |new keys below it|, new key j lands at j + |old keys below
+// it|, so every thread finds its place with one binary search.  Writes the merged keys, row_of_rank and rank; a key present
+// on both sides sets *dup (the host then rejects the edit before anything is committed).  old_row_of_rank == nullptr: rank == row.
+__global__ void __launch_bounds__(256)
+k_rank_merge(const uint64_t *__restrict__ old_keys, const uint32_t *__restrict__ old_row_of_rank, uint32_t n_old,
+             const uint64_t *__restrict__ new_keys, const uint32_t *__restrict__ new_rows, uint32_t n_new,
+             uint64_t *__restrict__ keys, uint32_t *__restrict__ row_of_rank, uint32_t *__restrict__ rank, uint32_t *__restrict__ dup) {
+    extern __shared__ uint64_t s_new_keys[];
+    const bool staged = n_new <= kMergeSmemKeys;
+    if (staged) for (uint32_t j = threadIdx.x; j < n_new; j += blockDim.x) s_new_keys[j] = new_keys[j];
+    __syncthreads();
+    const uint64_t *nk = staged ? s_new_keys : new_keys;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_old) {
+        const uint64_t key = old_keys[i];
+        const uint32_t lb = lower_bound_u64(nk, n_new, key);
+        if (lb < n_new && nk[lb] == key) atomicOr(dup, 1u);
+        const uint32_t pos = i + lb, row = old_row_of_rank ? old_row_of_rank[i] : i;
+        keys[pos] = key; row_of_rank[pos] = row; rank[row] = pos;
+    } else if (i < n_old + n_new) {
+        const uint32_t j = i - n_old;
+        const uint64_t key = nk[j];
+        const uint32_t pos = j + lower_bound_u64(old_keys, n_old, key), row = new_rows[j];
+        keys[pos] = key; row_of_rank[pos] = row; rank[row] = pos;
+    }
+}
+// A rank-ordered bit set (one per view, `stride` words apart) rebuilt for the new ranks: bit rk of the new set is the
+// old set's bit at the old rank of row_of_rank[rk]; rows appended by the edit start cleared.
+__global__ void __launch_bounds__(256)
+k_remap_rank_sets(const uint32_t *__restrict__ old_sets, uint32_t *__restrict__ sets, uint32_t stride, uint32_t n_words,
+                  uint32_t n_rows, uint32_t n_old_rows, const uint32_t *__restrict__ row_of_rank, const uint32_t *__restrict__ old_rank) {
+    const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x, v = blockIdx.y;
+    if (w >= n_words) return;
+    const uint32_t *old = old_sets + (size_t)v * stride;
+    uint32_t out = 0;
+    for (uint32_t b = 0; b < 32; ++b) {
+        const uint32_t rk = w * 32u + b;
+        if (rk >= n_rows) break;
+        const uint32_t row = row_of_rank[rk];
+        if (row >= n_old_rows) continue;
+        const uint32_t ork = old_rank ? old_rank[row] : row;
+        out |= ((old[ork >> 5] >> (ork & 31u)) & 1u) << b;
+    }
+    sets[(size_t)v * stride + w] = out;
+}
+// Column values of despawned rows (out of every query: no cull, no class, ViewVisibility 0, no shadow caster, no
+// Visibility components), reparented rows (marked changed) and spawned rows (what b200vis_create leaves, marked changed).
+__global__ void __launch_bounds__(256) k_edit_rows(Rows R, RowEdit e) {
+    uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < e.n_dead) {
+        const uint32_t row = e.dead[i];
+        R.flags[row] = (uint8_t)F_NO_CPU_CULL;
+        R.state[row] = 0;
+        if (e.cls) e.cls[row] = 0;
+        if (e.caster) e.caster[row] = 0;
+        if (e.visibility) e.visibility[row] = (uint8_t)V_NO_COMPONENTS;
+        return;
+    }
+    i -= e.n_dead;
+    if (i < e.n_moved) { const uint32_t row = e.moved[i]; R.flags[row] = (uint8_t)(R.flags[row] | F_TCHANGED); return; }
+    i -= e.n_moved;
+    if (i >= e.n_new) return;
+    const uint32_t row = e.first_new + i;
+    const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    R.trsA[row] = z4; R.trsB[row] = z4; R.trsC[row] = make_float2(0.f, 0.f);
+    R.gt0[row] = z4; R.gt1[row] = z4; R.gt2[row] = z4;
+    R.bndA[row] = z4; R.bndB[row] = make_float2(0.f, 0.f);
+    R.flags[row] = (uint8_t)F_TCHANGED;
+    R.state[row] = 0;
+    if (e.cls) e.cls[row] = 0;
+    if (e.caster) e.caster[row] = 0;
+    if (e.visibility) e.visibility[row] = 0;          // Visibility::Inherited
+    if (e.vv_shadow) e.vv_shadow[row] = 0xFF;         // the host column's value is unknown: the first write-back sends it
+    if (e.layers) e.layers[row] = 1u;                 // RenderLayers::default()
+    if (e.layers_ext) { e.layers_ext[(size_t)row * 3] = 0; e.layers_ext[(size_t)row * 3 + 1] = 0; e.layers_ext[(size_t)row * 3 + 2] = 0; }
+    if (e.range) e.range[row] = 0;
+    if (e.range_se) e.range_se[row] = make_float2(0.f, 0.f);
+    if (e.range_ua) e.range_ua[row] = 0;
+}
+void launch_rank_merge(cudaStream_t st, const uint64_t *old_keys, const uint32_t *old_row_of_rank, uint32_t n_old, const uint64_t *new_keys,
+                       const uint32_t *new_rows, uint32_t n_new, uint64_t *keys, uint32_t *row_of_rank, uint32_t *rank, uint32_t *dup) {
+    const uint32_t total = n_old + n_new;
+    if (!total) return;
+    const size_t smem = n_new <= kMergeSmemKeys ? (size_t)n_new * 8 : 0;
+    ++g_launches; k_rank_merge<<<cdiv(total, 256), 256, smem, st>>>(old_keys, old_row_of_rank, n_old, new_keys, new_rows, n_new, keys, row_of_rank, rank, dup);
+}
+void launch_remap_rank_sets(cudaStream_t st, const uint32_t *old_sets, uint32_t *sets, uint32_t stride, uint32_t n_sets, uint32_t n_words,
+                            uint32_t n_rows, uint32_t n_old_rows, const uint32_t *row_of_rank, const uint32_t *old_rank) {
+    if (!n_words || !n_sets) return;
+    ++g_launches; k_remap_rank_sets<<<dim3(cdiv(n_words, 256), n_sets), 256, 0, st>>>(old_sets, sets, stride, n_words, n_rows, n_old_rows, row_of_rank, old_rank);
+}
+void launch_edit_rows(cudaStream_t st, const Rows &R, const RowEdit &e) {
+    const uint32_t total = e.n_dead + e.n_moved + e.n_new;
+    if (total) { ++g_launches; k_edit_rows<<<cdiv(total, 256), 256, 0, st>>>(R, e); }
+}
+
 }  // namespace b200vis
 
 #ifdef B200VIS_TILE_TIMING

@@ -52,4 +52,10 @@ void launch_pack_inherited(cudaStream_t st, const Rows &R, uint32_t first, uint3
 void launch_pack_ranges(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, uint32_t *out);
 void launch_unpack_range_params(cudaStream_t st, float2 *se, uint8_t *ua, uint32_t first, uint32_t count, const float *src_se, const uint8_t *src_ua);
 void launch_pack_state(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, uint8_t *out, uint32_t changed_bit);
+// b200vis_edit_topology
+void launch_rank_merge(cudaStream_t st, const uint64_t *old_keys, const uint32_t *old_row_of_rank, uint32_t n_old, const uint64_t *new_keys,
+                       const uint32_t *new_rows, uint32_t n_new, uint64_t *keys, uint32_t *row_of_rank, uint32_t *rank, uint32_t *dup);
+void launch_remap_rank_sets(cudaStream_t st, const uint32_t *old_sets, uint32_t *sets, uint32_t stride, uint32_t n_sets, uint32_t n_words,
+                            uint32_t n_rows, uint32_t n_old_rows, const uint32_t *row_of_rank, const uint32_t *old_rank);
+void launch_edit_rows(cudaStream_t st, const Rows &R, const RowEdit &e);
 }

@@ -13,10 +13,11 @@ from . import abi
 
 class VisibilityPipeline:
     def __init__(self, scene, device=0, static_transform_optimizations=True, max_cluster_indices=0,
-                 world_size=1, rank=0, cluster_config=None, max_lights=None):
+                 world_size=1, rank=0, cluster_config=None, max_lights=None, max_entities=None):
+        """max_entities: row capacity of the context (default: the scene's rows), room for rows spawned by edit_topology."""
         self.scene = scene
         n, L, V = scene.n, len(scene.light_row), max(len(scene.cameras), 1)
-        self.ctx = abi.Context(n, max_lights=max(L, 1) if max_lights is None else max(max_lights, L, 1), max_views=V, device=device,
+        self.ctx = abi.Context(max(n, max_entities or 0), max_lights=max(L, 1) if max_lights is None else max(max_lights, L, 1), max_views=V, device=device,
                                max_cluster_indices=max_cluster_indices, world_size=world_size, rank=rank)
         c = self.ctx
         c.set_static_transform_optimizations(static_transform_optimizations)

@@ -180,7 +180,9 @@ B200VIS_API int32_t b200vis_join(b200vis_ctx *ctx);
 B200VIS_API int32_t b200vis_tail_stream(b200vis_ctx *ctx, void **cuda_stream);
 
 /* ---- mirroring the ECS columns --------------------------------------------- */
-/* Hierarchy + identity; call on spawn/despawn/Changed<ChildOf> only.
+/* Hierarchy + identity: the whole world, planned from scratch, with fresh frame state (every visible entity is
+ * reported added by the next visible diff).  Per-frame spawns, despawns and ChildOf changes go through
+ * b200vis_edit_topology instead; this call is its fallback and the compaction that drops despawned rows.
  * Replaces the Children/ChildOf walks of propagate_descendants_unchecked
  * (systems.rs:679-748) with a cached execution plan.  entity_bits = Entity::to_bits()
  * (crates/bevy_ecs/src/entity/mod.rs:468-476), which fixes the order of every
@@ -188,6 +190,33 @@ B200VIS_API int32_t b200vis_tail_stream(b200vis_ctx *ctx, void **cuda_stream);
  * (parent_row[r] < r); b200vis_plan_row_order produces such an order. */
 B200VIS_API int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n_rows, const uint32_t *parent_row,
                              const uint64_t *entity_bits);
+/* One call per frame with every structural change of that frame, applied in this order:
+ *   1. despawn   despawn_rows[n_despawn]: the rows leave every query and become tombstones (the other rows keep their
+ *                numbers).  Despawn is recursive: a despawned row's live children must be despawned in the same call.
+ *   2. reparent  reparent_rows[n_reparent] -> new_parent[] (B200VIS_NO_PARENT, B200VIS_DETACHED or a live row < the row):
+ *                Changed<ChildOf> / RemovedComponents<ChildOf>; the rows are marked as b200vis_mark_transforms_changed does.
+ *   3. spawn     n_spawn rows appended at [n, n + n_spawn): spawn_parent[] (sentinel, live row, or an earlier row of this
+ *                batch), spawn_entity_bits[] = Entity::to_bits(); Added<GlobalTransform> (marked changed).
+ * All or nothing: on any error nothing has changed.  Errors: CAPACITY (more than max_entities rows, tombstones included);
+ * INVALID_ARG (a row out of range or dead, entity bits equal to those of any row, live or dead, a despawned row with live
+ * children, a despawned row that is still in the b200vis_set_lights list or a point / spot shadow item: remove it there
+ * first); UNSUPPORTED (a parent at or after its child's row, a tile that would need more than 128 rows with in-tile
+ * children, world_size > 1).  On UNSUPPORTED or CAPACITY, fall back to b200vis_set_topology.
+ * Dead rows: parent B200VIS_DETACHED, flags B200VIS_F_NO_CPU_CULLING only, ViewVisibility 0, no VisibilityClass, not a
+ * shadow caster.  They are in no visible, shadow or cluster list; a dead row that was visible is reported removed by
+ * the next visible diff; its Changed flags never fire (the write-back mirrors its ViewVisibility 0 once).
+ * b200vis_set_lights and b200vis_set_shadow_items reject dead rows.
+ * Spawned rows start as b200vis_create leaves a row: Transform, GlobalTransform and bounds all zero, flags 0 (no
+ * InheritedVisibility), no class, RenderLayers layer 0, no VisibilityRange, Visibility::Inherited, not a shadow caster.
+ * Upload their columns with the usual calls before the next run.
+ * Frame history carries over: frame counter, statistics, the visible-diff sets (which b200vis_run_shadow_culling reads),
+ * Clusters feedback, recorded frame constants and the result / column sinks. */
+B200VIS_API int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, const uint32_t *despawn_rows,
+                                          uint32_t n_reparent, const uint32_t *reparent_rows, const uint32_t *new_parent,
+                                          uint32_t n_spawn, const uint32_t *spawn_parent, const uint64_t *spawn_entity_bits);
+/* out = { rows (tombstones included), live rows, tiles, passes }: what a caller weighs before compacting with
+ * b200vis_set_topology. */
+B200VIS_API int32_t b200vis_topology_summary(const b200vis_ctx *ctx, uint32_t out[4]);
 /* Helper for the shim: a permutation (new_row -> old_row) that is topological and
  * keeps every tree contiguous in BFS order (the layout the tile kernel likes). */
 B200VIS_API int32_t b200vis_plan_row_order(uint32_t n_rows, const uint32_t *parent_row, uint32_t *new_to_old);
@@ -208,6 +237,18 @@ B200VIS_API int32_t b200vis_host_tile_plan(uint32_t n_rows, const uint32_t *pare
  * tile_rows = 0 means the default tile size (256).  With tile_desc == NULL only *n_tiles is written. */
 B200VIS_API int32_t b200vis_host_warp_plan(uint32_t n_rows, const uint32_t *parent_row, uint32_t tile_rows, uint32_t tiles_capacity,
                                            uint32_t *n_tiles, uint32_t *tile_desc, uint32_t *nonroot, uint8_t *sched, uint32_t *wtopo);
+/* The plan b200vis_edit_topology keeps, after an edit script (no GPU needed; for tests and tools).  The script is a
+ * sequence of steps, each { n_despawn, n_reparent, n_spawn, despawn_rows[n_despawn], reparent_rows[n_reparent],
+ * new_parent[n_reparent], spawn_parent[n_spawn] }, applied like b200vis_edit_topology calls with at most max_rows rows.
+ * Returns the first failing step's error (the outputs then hold the plan before that step).  *n_rows = rows after
+ * the script; tile_desc[i][17] = { the 8 words of b200vis_host_tile_plan, chunks | contiguous-chunk bits << 8,
+ * nonroot[8] of b200vis_host_warp_plan }, sched[i][256], topo[row], wtopo[row] as there; counters = { tiles re-planned
+ * and rows re-planned by the last applied step, passes, steps applied }.  With tile_desc == NULL only *n_rows, *n_tiles
+ * and counters are written. */
+B200VIS_API int32_t b200vis_host_edit_plan(uint32_t n_rows, const uint32_t *parent_row, uint32_t tile_rows, uint32_t max_rows,
+                                           uint32_t script_words, const uint32_t *script, uint32_t tiles_capacity, uint32_t *n_rows_out,
+                                           uint32_t *n_tiles, uint32_t *tile_desc, uint32_t *topo, uint32_t *wtopo, uint8_t *sched,
+                                           uint32_t counters[4]);
 
 /* Transform column, dirty ranges: trs[count][10] = translation.xyz, rotation.xyzw, scale.xyz
  * (components/transform.rs:86-105).  Marks the rows Changed<Transform>. */
