@@ -121,6 +121,7 @@ struct b200vis_ctx {
     uint8_t *d_blob = nullptr;          // the one the current frame uses
     FrameConsts *d_consts = nullptr;    // == d_blob
     bool consts_dirty = true;
+    const uint8_t *blob_flushed = nullptr;   // the device blob the last flush wrote (the only one known to be current)
     size_t blob_used = 0;               // bytes of the last packed blob
     struct Recorded { FrameConsts host; uint8_t *dev; size_t bytes; };
     std::vector<Recorded> recorded;     // b200vis_record_frame_constants
@@ -1500,6 +1501,7 @@ static int32_t flush_consts(b200vis_ctx *ctx) {
     CU(cudaEventRecord(ctx->ring_ev[slot], ctx->stream));
     ctx->blob_used = off;
     ctx->consts_dirty = false;
+    ctx->blob_flushed = ctx->d_blob;
     return B200VIS_OK;
 }
 
@@ -1763,7 +1765,9 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     } else {
         ctx->d_blob = ctx->d_blob2[cslot];          // the side stream may still read the other two copies
         ctx->d_consts = reinterpret_cast<FrameConsts *>(ctx->d_blob);
-        ctx->consts_dirty = ctx->consts_dirty || pipelined;   // each copy must be current
+        // each copy must be current: a pipelined frame rewrites its slot, and so does any run whose slot is not the one last
+        // flushed (CULL advances the frame, so a CLUSTER run right behind it reads the next slot)
+        ctx->consts_dirty = ctx->consts_dirty || pipelined || ctx->blob_flushed != ctx->d_blob;
         const int32_t rc = flush_consts(ctx); if (rc) return rc;
         fc = ctx->d_consts;
     }

@@ -3464,11 +3464,16 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
                 const float reach = (sl.range + e1) * 1.001f + 1e-3f;      // d <= r + rr/d <= r + E1 where the exact test passes
                 skip = (dx * dx + dy * dy) + dz * dz > reach * reach;
             } else if (!skip) {
+                const float ax = fmaxf(fabsf(bx0), fabsf(bx1)), ay = fmaxf(fabsf(by0), fabsf(by1)), az = fmaxf(fabsf(bz0), fabsf(bz1));
                 for (int k = 0; k < 6 && !skip; ++k) {               // a half space no point of the box reaches, even grown by E1
                     if (k == 4) continue;
                     const float4 n = sl.planes[0][k];
                     const float m = ((fmaxf(n.x * bx0, n.x * bx1) + fmaxf(n.y * by0, n.y * by1)) + fmaxf(n.z * bz0, n.z * bz1)) + n.w;
-                    skip = m + (e1 * 1.001f + 1e-3f) * ((fabsf(n.x) + fabsf(n.y)) + fabsf(n.z)) < 0.0f;
+                    const float reach = e1 * ((fabsf(n.x) + fabsf(n.y)) + fabsf(n.z));
+                    // the margin scales with the operands (as in warp_view_reject): m sums ((x + y) + z) + w, the exact test
+                    // (x + z) + (y + w), and far from the origin the two differ by more than any absolute margin
+                    const float mag = ((fabsf(n.x) * ax + fabsf(n.y) * ay) + fabsf(n.z) * az) + (fabsf(n.w) + reach);
+                    skip = (m + reach) + (1e-5f * mag + 1e-6f) < 0.0f;
                 }
             }
             live = !skip;

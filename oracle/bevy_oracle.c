@@ -1151,7 +1151,7 @@ ORC_API int orc_check_spot_light_mesh_visibility(uint32_t n, const float *gt, co
  * view, concatenated in `frusta`), the light's RenderLayers and the view's bit in the VisibleEntityRanges masks
  * (-1 = the view is not in the map => entity_is_in_range_of_view is false).  The near plane is NOT tested (a caster may
  * lie before it, :455-458).  Out: per cascade (in item order) rows ascending by entity bits; set_visible is applied
- * (the reference defers it to a command, same result).  (Device side: not built yet.) */
+ * (the reference defers it to a command, same result).  Device side: cascade items of b200vis_set_shadow_items (k_shadow_cull). */
 ORC_API int orc_check_dir_light_mesh_visibility(uint32_t n, const float *gt, const float *bounds, const uint8_t *flags,
                                                 const uint8_t *caster, const uint64_t *layer_mask, const uint32_t *range_mask,
                                                 const uint64_t *entity_bits, uint8_t *vv, uint8_t *vv_changed, uint32_t n_items,

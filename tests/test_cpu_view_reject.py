@@ -7,6 +7,8 @@ import numpy as np
 import pytest
 
 f32 = np.float32
+OFFSET_DIR = np.array([0.6, -0.48, 0.64])           # unit length: world offsets go along this direction
+OFFSETS = (0.0, 1e4, 1e5, 1e6)                       # the scaled margin must hold far from the origin too
 
 
 def exact_rejects(planes, c, r):
@@ -45,10 +47,11 @@ def box_rejects(planes, c, r):
     return False
 
 
-def random_frustum(rng, normalised=True):
-    """Five half spaces (normal, d) of a perspective-like frustum at a random pose; optionally with un-normalised normals."""
+def random_frustum(rng, normalised=True, offset=0.0):
+    """Five half spaces (normal, d) of a perspective-like frustum at a random pose `offset` from the origin (along a fixed
+    diagonal); optionally with un-normalised normals."""
     q = rng.normal(size=(3, 3)); q, _ = np.linalg.qr(q)
-    eye = rng.uniform(-300, 300, 3)
+    eye = rng.uniform(-300, 300, 3) + offset * OFFSET_DIR
     a, b = np.tan(rng.uniform(0.2, 0.7)), np.tan(rng.uniform(0.15, 0.5))
     local = [(1, 0, -a), (-1, 0, -a), (0, 1, -b), (0, -1, -b), (0, 0, -1)]      # L R B T near (looking down -z)
     planes = []
@@ -62,13 +65,18 @@ def random_frustum(rng, normalised=True):
 
 @pytest.mark.parametrize("normalised", [True, False])
 def test_warp_shortcuts_never_reject_a_view_the_exact_test_keeps(normalised):
-    rng = np.random.default_rng(7 if normalised else 8)
+    """Near the origin and far from it (world offsets up to 1e6), where the margin must grow with the coordinates."""
+    for k, offset in enumerate(OFFSETS):
+        _warp_shortcuts_at(np.random.default_rng((7 if normalised else 8) + 100 * k), normalised, offset)
+
+
+def _warp_shortcuts_at(rng, normalised, offset):
     hits = {"sphere": 0, "box": 0}
     trials = 0
     for _ in range(400):
-        planes = random_frustum(rng, normalised)
+        planes = random_frustum(rng, normalised, offset)
         for spread in (0.5, 4.0, 40.0, 400.0):
-            centre = rng.uniform(-500, 500, 3)
+            centre = rng.uniform(-500, 500, 3) + offset * OFFSET_DIR
             c = (centre + rng.normal(scale=spread, size=(32, 3))).astype(f32)
             r = rng.uniform(0.0, 1.5, 32).astype(f32)
             if rng.random() < 0.1:
@@ -78,22 +86,35 @@ def test_warp_shortcuts_never_reject_a_view_the_exact_test_keeps(normalised):
             for name, fn in (("sphere", sphere_rejects), ("box", box_rejects)):
                 if fn(planes, c, r):
                     hits[name] += 1
-                    assert ex.all(), f"{name} bound rejected a warp with a row the exact test keeps"
+                    assert ex.all(), f"{name} bound rejected a warp with a row the exact test keeps (world offset {offset:g})"
     # the shortcut has to fire for most far-away warps, or it is worthless
-    assert hits["sphere"] > trials // 3 and hits["box"] > trials // 3
+    assert hits["sphere"] > trials // 3 and hits["box"] > trials // 3, (offset, hits, trials)
 
 
 def test_rows_just_inside_a_plane_are_never_rejected():
-    rng = np.random.default_rng(11)
+    for k, offset in enumerate(OFFSETS):
+        _rows_just_inside_at(np.random.default_rng(11 + 100 * k), offset)
+
+
+def _rows_just_inside_at(rng, offset):
+    kept = 0
     for _ in range(300):
-        planes = random_frustum(rng)
+        planes = random_frustum(rng, True, offset)
         n = planes[rng.integers(5)].astype(np.float64)
-        # a tight warp whose first row touches the plane from outside by less than its radius: the exact test keeps it
-        p0 = rng.uniform(-200, 200, 3)
+        # a tight warp whose first row touches the plane from outside by less than its radius: the exact test keeps it.  The
+        # warp starts from a point inside the frustum (on its axis, in front of the apex the four side planes share) moved onto
+        # the plane, so that the other four planes keep it
+        side = np.array(planes[:4], np.float64)
+        eye = np.linalg.lstsq(side[:, :3], -side[:, 3], rcond=None)[0]
+        p0 = eye + np.asarray(planes[4][:3], np.float64) * rng.uniform(1.0, 100.0)
         p0 -= n[:3] * ((n[:3] @ p0 + n[3]) / (n[:3] @ n[:3]))          # onto the plane
-        r = np.full(32, 0.5, f32)
-        c = (p0 - n[:3] * 0.4999 + rng.normal(scale=1e-3, size=(32, 3))).astype(f32)
+        # far from the origin the float32 grid is coarser than the 1e-4 / 1e-3 steps used near it: scale them with it
+        sp = float(np.spacing(f32(np.abs(p0).max())))
+        r = np.full(32, max(0.5, 16 * sp), f32)
+        c = (p0 - n[:3] * (r[0] - max(1e-4, 8 * sp)) + rng.normal(scale=max(1e-3, sp), size=(32, 3))).astype(f32)
         ex = exact_rejects([planes[k] for k in range(5)], c, r)
         if not ex.all():
-            assert not sphere_rejects(planes, c, r)
-            assert not box_rejects(planes, c, r)
+            kept += 1
+            assert not sphere_rejects(planes, c, r), f"world offset {offset:g}"
+            assert not box_rejects(planes, c, r), f"world offset {offset:g}"
+    assert kept > 200, (offset, kept)          # most warps do keep a row: the check is not vacuous at any offset
