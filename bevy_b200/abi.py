@@ -114,6 +114,7 @@ _SIGNATURES = {
     "b200vis_tail_stream": (C.c_int32, [_vp, _P(_vp)]),
     "b200vis_set_topology": (C.c_int32, [_vp, C.c_uint32, _vp, _vp]),
     "b200vis_edit_topology": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _vp, _vp, C.c_uint32, _vp, _vp]),
+    "b200vis_compact_topology": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, _vp]),
     "b200vis_topology_summary": (C.c_int32, [_vp, _P(C.c_uint32)]),
     "b200vis_host_edit_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, C.c_uint32, _vp, C.c_uint32,
                                            _P(C.c_uint32), _P(C.c_uint32), _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
@@ -331,22 +332,35 @@ class EditedPlan:
         return d, self.desc[:, 9:17].copy(), self.sched, self.wtopo
 
 
+class Compaction:
+    """A compaction step of an edit script: b200vis_compact_topology with these reparents, where held results still
+    name the dead rows `held`."""
+
+    def __init__(self, reparent=(), new_parent=(), held=()):
+        self.reparent, self.new_parent, self.held = list(map(int, reparent)), list(map(int, new_parent)), list(map(int, held))
+        assert len(self.reparent) == len(self.new_parent)
+
+
 def edit_script(steps):
-    """Encodes [(despawn_rows, reparent_rows, new_parent, spawn_parent), ...] for host_edit_plan."""
+    """Encodes [(despawn_rows, reparent_rows, new_parent, spawn_parent) or Compaction, ...] for host_edit_plan."""
     words = []
-    for despawn, reparent, new_parent, spawn_parent in steps:
-        despawn, reparent, new_parent, spawn_parent = (list(map(int, x)) for x in (despawn, reparent, new_parent, spawn_parent))
+    for step in steps:
+        if isinstance(step, Compaction):
+            words += [0xFFFFFFFF, len(step.reparent), len(step.held)] + step.reparent + step.new_parent + step.held
+            continue
+        despawn, reparent, new_parent, spawn_parent = (list(map(int, x)) for x in step)
         assert len(reparent) == len(new_parent)
         words += [len(despawn), len(reparent), len(spawn_parent)] + despawn + reparent + new_parent + spawn_parent
     return np.asarray(words, np.uint32)
 
 
 def host_edit_plan(parent, steps, max_rows=None, tile_rows=0):
-    """The plan after applying edit steps (see edit_script) to a fresh plan of `parent`, as b200vis_edit_topology keeps it."""
+    """The plan after applying edit steps (see edit_script) to a fresh plan of `parent`, as b200vis_edit_topology and
+    b200vis_compact_topology keep it."""
     parent = _arr(parent, np.uint32)
     script = edit_script(steps)
     if max_rows is None:
-        max_rows = len(parent) + sum(len(s[3]) for s in steps)
+        max_rows = len(parent) + sum(len(s[3]) for s in steps if not isinstance(s, Compaction))
     lib = load_library()
     n_out, nt, ctr = C.c_uint32(0), C.c_uint32(0), (C.c_uint32 * 4)()
     rc = lib.b200vis_host_edit_plan(len(parent), _ptr(parent), tile_rows, max_rows, len(script), _ptr(script), 0,
@@ -431,6 +445,16 @@ class Context:
         assert len(r) == len(npr) and len(sp) == len(sb)
         self._check(self._lib.b200vis_edit_topology(self._h, len(d), _ptr(d), len(r), _ptr(r), _ptr(npr), len(sp), _ptr(sp), _ptr(sb)))
         self.n = getattr(self, "n", 0) + len(sp)
+
+    def compact_topology(self, reparent=(), new_parent=()):
+        """Drops the tombstones no held result names and applies reparents that need not keep row order
+        (b200vis_compact_topology).  Returns old_to_new: the new row of every old row, 0xFFFFFFFF if it was dropped."""
+        r = _arr(reparent, np.uint32); npr = _arr(new_parent, np.uint32)
+        assert len(r) == len(npr)
+        o2n = np.zeros(self.topology_summary()[0], np.uint32)
+        self._check(self._lib.b200vis_compact_topology(self._h, len(r), _ptr(r), _ptr(npr), _ptr(o2n)))
+        self.n = int((o2n != 0xFFFFFFFF).sum())
+        return o2n
 
     def topology_summary(self):
         """(rows incl. tombstones, live rows, tiles, passes)."""

@@ -844,6 +844,58 @@ static int32_t edit_plan(b200vis_ctx *ctx, Plan &hp, uint32_t max_rows, const To
     return B200VIS_OK;
 }
 
+static int32_t plan_world(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, Plan &plan);
+
+// The host half of b200vis_compact_topology: the survivors (live rows, and the dead rows in `held` that results still
+// name), the reparents applied, the survivors renumbered in b200vis_plan_row_order's order of their current order, and
+// the plan set_topology builds for the new parent array (cap == 0: with its tile-size search).  Writes the new plan to
+// `out`; `hp` is only read.
+static int32_t compact_plan(b200vis_ctx *ctx, const Plan &hp, uint32_t n_reparent, const uint32_t *reparent, const uint32_t *new_parent,
+                            const std::vector<uint32_t> &held, uint32_t cap, Plan &out, std::vector<uint32_t> &old_to_new,
+                            std::vector<uint32_t> &new_to_old) {
+    const uint32_t n = hp.n;
+    std::vector<uint32_t> par(hp.parent);
+    std::vector<uint8_t> keep(hp.alive);
+    for (uint32_t r : held) {
+        if (r >= n || hp.alive[r]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: held row %u is out of range or live", r);
+        keep[r] = 1;
+    }
+    {
+        std::vector<uint32_t> rp(reparent, reparent + n_reparent);
+        std::sort(rp.begin(), rp.end());
+        for (size_t i = 1; i < rp.size(); ++i)
+            if (rp[i] == rp[i - 1]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: row %u is reparented twice", rp[i]);
+    }
+    for (uint32_t j = 0; j < n_reparent; ++j) {
+        const uint32_t r = reparent[j], p = new_parent[j];
+        if (r >= n || !hp.alive[r]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: reparented row %u is out of range or dead", r);
+        if (p != kNoParent && p != kDetached && (p >= n || !hp.alive[p]))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: new parent %u of row %u is out of range or dead", p, r);
+        par[r] = p;
+    }
+    // survivors in their current order; a live row's parent is live (despawns are recursive), a dead row is detached
+    std::vector<uint32_t> surv, s_of(n, kNoParent);
+    for (uint32_t r = 0; r < n; ++r)
+        if (keep[r]) { s_of[r] = (uint32_t)surv.size(); surv.push_back(r); }
+    const uint32_t ns = (uint32_t)surv.size();
+    std::vector<uint32_t> ps(ns), ord(ns);
+    for (uint32_t i = 0; i < ns; ++i) { const uint32_t p = par[surv[i]]; ps[i] = p < n ? s_of[p] : p; }
+    if (b200vis_plan_row_order(ns, ps.data(), ord.data()) != B200VIS_OK)
+        return fail(ctx, B200VIS_ERR_HIERARCHY_CYCLE, "compact_topology: the reparents make a hierarchy cycle");
+    old_to_new.assign(n, kNoParent);
+    new_to_old.resize(ns);
+    for (uint32_t i = 0; i < ns; ++i) { new_to_old[i] = surv[ord[i]]; old_to_new[new_to_old[i]] = i; }
+    std::vector<uint32_t> pn(ns);
+    for (uint32_t i = 0; i < ns; ++i) { const uint32_t p = par[new_to_old[i]]; pn[i] = p < n ? old_to_new[p] : p; }
+    const int32_t rc = cap ? build_plan(ctx, ns, pn.data(), cap, out) : plan_world(ctx, ns, pn.data(), out);
+    if (rc) return rc;
+    out.parent = std::move(pn);
+    out.alive.resize(ns);
+    out.n_dead = 0;
+    for (uint32_t i = 0; i < ns; ++i) { out.alive[i] = hp.alive[new_to_old[i]]; out.n_dead += out.alive[i] ? 0u : 1u; }
+    return B200VIS_OK;
+}
+
 static void free_plan(Plan *p) { delete p; }
 
 // the pass ranges of a plan, and which passes may run the named-barrier schedule
@@ -857,26 +909,31 @@ static void install_passes(b200vis_ctx *ctx, const Plan &plan) {
             if (plan.tiles[ti].n_levels > 1 && plan.tiles[ti].lvl_warps == 0ull) { ctx->pass_named[pi] = 0; break; }
 }
 
+// The plan of a whole world, as set_topology and the compaction install it.  Tile size: a tile is one WARP's work item, and
+// the machine has ~4700 resident warps: small scenes get smaller tiles (more warps busy) as long as that does not split
+// trees across tiles (more passes / parents read from HBM).
+static int32_t plan_world(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, Plan &plan) {
+    int32_t rc = build_plan(ctx, n, parent, kTileRows, plan);
+    if (rc != B200VIS_OK) return rc;
+    static int cap_env = -1;
+    if (cap_env < 0) { const char *e = getenv("B200VIS_TILE_ROWS"); cap_env = e ? atoi(e) : 0; }
+    uint32_t target = cap_env > 0 ? (uint32_t)cap_env : (uint32_t)std::min<uint64_t>(kTileRows, (((uint64_t)n / 9472u) + 31u) / 32u * 32u);
+    if (target < 32) target = 32;
+    for (uint32_t cap = target; cap < (uint32_t)kTileRows; cap *= 2) {
+        Plan q;
+        if (build_plan(ctx, n, parent, cap, q) != B200VIS_OK) break;
+        if (q.pass_begin.size() <= plan.pass_begin.size() && q.n_ext <= plan.n_ext) { plan = std::move(q); break; }
+    }
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, const uint64_t *entity_bits) {
     CHECK_CTX_JOIN();
     if (n && (!parent || !entity_bits)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_topology: null array");
     if (n > ctx->cfg.max_entities) return fail(ctx, B200VIS_ERR_CAPACITY, "set_topology: %u rows > max_entities %u", n, ctx->cfg.max_entities);
-    // Tile size: a tile is one WARP's work item, and the machine has ~4700 resident warps: small scenes get smaller tiles
-    // (more warps busy) as long as that does not split trees across tiles (more passes / parents read from HBM).
     Plan plan;
-    int32_t rc = build_plan(ctx, n, parent, kTileRows, plan);
+    int32_t rc = plan_world(ctx, n, parent, plan);
     if (rc != B200VIS_OK) return rc;
-    {
-        static int cap_env = -1;
-        if (cap_env < 0) { const char *e = getenv("B200VIS_TILE_ROWS"); cap_env = e ? atoi(e) : 0; }
-        uint32_t target = cap_env > 0 ? (uint32_t)cap_env : (uint32_t)std::min<uint64_t>(kTileRows, (((uint64_t)n / 9472u) + 31u) / 32u * 32u);
-        if (target < 32) target = 32;
-        for (uint32_t cap = target; cap < (uint32_t)kTileRows; cap *= 2) {
-            Plan q;
-            if (build_plan(ctx, n, parent, cap, q) != B200VIS_OK) break;
-            if (q.pass_begin.size() <= plan.pass_begin.size() && q.n_ext <= plan.n_ext) { plan = std::move(q); break; }
-        }
-    }
     std::vector<uint32_t> &topo = plan.topo; std::vector<Tile> &tiles = plan.tiles;
     if (tiles.size() > ctx->tiles_cap) {
         void *old[] = {ctx->d_tiles, ctx->d_wtiles, ctx->d_sched};
@@ -944,6 +1001,27 @@ static int32_t grow_edit_staging(b200vis_ctx *ctx, size_t bytes) {
     return B200VIS_OK;
 }
 
+// The spare rank arrays an edit's rank merge and a compaction write into (swapped in when the call commits): each is
+// allocated once, on first need, and assigned only when every array asked for was allocated, so a failed allocation
+// leaves none of them half set up.  keys: also the spare of the resident keys.
+static int32_t alloc_rank_spares(b200vis_ctx *ctx, bool keys) {
+    const size_t N = ctx->cfg.max_entities;
+    uint64_t *k = nullptr; uint32_t *r = nullptr, *rr = nullptr;
+    cudaError_t e = cudaSuccess;
+    if (keys && !ctx->d_keys2) e = dalloc(&k, N);
+    if (e == cudaSuccess && !ctx->d_rank2) e = dalloc(&r, N);
+    if (e == cudaSuccess && !ctx->d_row_of_rank2) e = dalloc(&rr, N);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        cudaFree(k); cudaFree(r); cudaFree(rr);
+        return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA, "spare rank arrays: %s", cudaGetErrorString(e));
+    }
+    if (k) ctx->d_keys2 = k;
+    if (r) ctx->d_rank2 = r;
+    if (rr) ctx->d_row_of_rank2 = rr;
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, const uint32_t *despawn_rows,
                                          uint32_t n_reparent, const uint32_t *reparent_rows, const uint32_t *new_parent,
                                          uint32_t n_spawn, const uint32_t *spawn_parent, const uint64_t *spawn_entity_bits) {
@@ -974,7 +1052,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
     if (merge) {
         const size_t N = ctx->cfg.max_entities;
         if (!ctx->d_keys) CU(dalloc(&ctx->d_keys, N));
-        if (!ctx->d_keys2) { CU(dalloc(&ctx->d_keys2, N)); CU(dalloc(&ctx->d_rank2, N)); CU(dalloc(&ctx->d_row_of_rank2, N)); }
+        { const int32_t arc = alloc_rank_spares(ctx, true); if (arc) return arc; }
         if (!ctx->keys_resident) {
             CU(cudaStreamSynchronize(st));
             CU(cudaMemcpy(ctx->d_keys, ctx->h_keys.data(), (size_t)n * 8, cudaMemcpyHostToDevice));
@@ -1094,6 +1172,263 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
     return B200VIS_OK;
 }
 
+extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparent, const uint32_t *reparent_rows,
+                                            const uint32_t *new_parent, uint32_t *old_to_new_out) {
+    CHECK_CTX_JOIN();   // the tail of the frame in flight writes the lists and reads the rank arrays
+    if (!ctx->topology_set || !ctx->hplan) return fail(ctx, B200VIS_ERR_NOT_READY, "compact_topology: b200vis_set_topology has not been called");
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "compact_topology: world_size > 1 (use set_topology)");
+    if (n_reparent && (!reparent_rows || !new_parent)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: null array");
+    Plan &hp = *ctx->hplan;
+    const uint32_t n = ctx->n, V = ctx->cfg.max_views;
+    cudaStream_t st = ctx->stream;
+    if (ctx->ev_edit) CU(cudaEventSynchronize(ctx->ev_edit));   // the last edit's staging copies have been read
+    else CU(cudaEventCreateWithFlags(&ctx->ev_edit, cudaEventDisableTiming));
+    // ---- the row-valued results the context holds: every view slot's visible list (an inactive view keeps its last
+    // one), the visible diff, the shadow lists.  A dead row they name survives this compaction as a tombstone ----
+    // the visible-diff state exists once the diff was ever enabled, and stays what the shadow stage reads and what a
+    // download returns even while the diff is switched off: it is carried over whenever it exists, as the edit does
+    const bool diff = ctx->diff.prev != nullptr;
+    const uint32_t LS = ctx->vis.list_stride;
+    RowLists lists[4]; uint32_t n_lists = 0;
+    lists[n_lists++] = RowLists{ctx->vis.lists, LS, V, 1, reinterpret_cast<const uint32_t *>(ctx->d_stats)};   // DevStats::visible_count
+    if (diff) {
+        lists[n_lists++] = RowLists{ctx->diff.lists, LS, V, 2, ctx->diff.count};                        // added
+        lists[n_lists++] = RowLists{ctx->diff.lists + (size_t)V * LS, LS, V, 2, ctx->diff.count + 1};   // removed
+    }
+    if (ctx->shadow.n_lights) lists[n_lists++] = RowLists{ctx->shadow.lists, ctx->shadow.list_cap, ctx->shadow.n_lights * 6, 1, ctx->shadow.count};
+    // what the call allocates for itself only (scratch for small worlds, trace events): released on every return
+    struct CallScratch {
+        uint8_t *tmp = nullptr; cudaEvent_t ev[3] = {nullptr, nullptr, nullptr};
+        ~CallScratch() { if (tmp) cudaFree(tmp); for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e); }
+    } own;
+    std::vector<uint32_t> held;
+    if (hp.n_dead) {
+        CU(cudaMemsetAsync(ctx->d_dirty, 0, n, st));
+        for (uint32_t i = 0; i < n_lists; ++i) launch_mark_listed_rows(st, lists[i], n, ctx->d_dirty, n);
+        if (diff)   // last frame's visible sets: a row in them is reported removed by the next diff
+            launch_mark_set_rows(st, ctx->diff.prev, ctx->vis.words_stride, V, (n + 31) / 32, ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->d_dirty);
+        CU(cudaGetLastError());
+        CU(cudaMemcpyAsync(ctx->h_stage, ctx->d_dirty, n, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        for (uint32_t r = 0; r < n; ++r) if (!hp.alive[r] && ctx->h_stage[r]) held.push_back(r);
+    }
+    // ---- host plan (validates everything; nothing is changed before it succeeds) ----
+    // B200VIS_COMPACT_TRACE: host clock around the planning, events around the device work, one line on stderr per call
+    static int trace = -1;
+    if (trace < 0) trace = getenv("B200VIS_COMPACT_TRACE") ? 1 : 0;
+    using clk = std::chrono::steady_clock;
+    const auto t_plan0 = clk::now();
+    Plan q;
+    std::vector<uint32_t> o2n, n2o;
+    int32_t rc = compact_plan(ctx, hp, n_reparent, reparent_rows, new_parent, held, 0, q, o2n, n2o);
+    if (rc) return rc;
+    const double plan_ms = std::chrono::duration<double, std::milli>(clk::now() - t_plan0).count();
+    cudaEvent_t *tev = own.ev;
+    float gather_ms = 0.f, copy_ms = 0.f;
+    size_t row_bytes = 0;
+    if (trace) for (int i = 0; i < 3; ++i) CU(cudaEventCreate(&tev[i]));
+    const uint32_t n2 = (uint32_t)n2o.size(), T = (uint32_t)q.tiles.size();
+    std::vector<uint32_t> dropped;
+    for (uint32_t r = 0; r < n; ++r) if (o2n[r] == kNoParent) dropped.push_back(r);
+    const uint32_t nd = (uint32_t)dropped.size();
+    // ---- the resident per-row columns the permutation moves (columns never uploaded are absent) ----
+    struct Column { void *p; uint32_t elem, per_row; unsigned long long fill; };   // fill: value of the rows past the new count
+    std::vector<Column> cols;
+    {
+        auto add = [&](void *p, uint32_t elem, uint32_t per_row, unsigned long long fill) { if (p) cols.push_back(Column{p, elem, per_row, fill}); };
+        const Rows &R = ctx->rows;
+        for (void *p : {(void *)R.trsA, (void *)R.trsB, (void *)R.gt0, (void *)R.gt1, (void *)R.gt2, (void *)R.bndA}) add(p, 16, 1, 0);
+        add(R.trsC, 8, 1, 0); add(R.bndB, 8, 1, 0);
+        add(ctx->d_layers_ext, 8, 3, 0);                                   // RenderLayers blocks 1..3
+        if (ctx->have_layers) add(ctx->d_layers, 8, 1, 1);                 // block 0; RenderLayers::default()
+        add(ctx->d_range_se, 8, 1, 0);
+        if (ctx->have_range) add(ctx->d_range, 4, 1, 0);
+        add(ctx->d_light_ord, 4, 1, 0xFFFFFFFFull);                        // not a light
+        for (void *p : {(void *)R.flags, (void *)R.state, (void *)ctx->d_cls, (void *)ctx->d_range_ua, (void *)ctx->d_visibility,
+                        (void *)ctx->d_iv_changed, (void *)ctx->d_caster}) add(p, 1, 1, 0);
+        add(ctx->d_vv_shadow, 1, 1, 0xFF);                                 // the host's value unknown
+    }
+    // ---- device scratch: the maps, then the permuted columns (a group at a time) and the reparented rows ----
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t o_o2n = 0, o_n2o = al((size_t)n * 4), o_drow = o_n2o + al((size_t)n2 * 4), o_drk = o_drow + al((size_t)nd * 4),
+                 o_src = o_drk + al((size_t)nd * 4), o_flag = o_src + al((size_t)n2 * 4), o_cols = o_flag + 256;
+    size_t max_col = al((size_t)n_reparent * 4), all_cols = max_col;
+    for (const Column &c : cols) { const size_t nb = al((size_t)n * c.elem * c.per_row); max_col = std::max(max_col, nb); all_cols += nb; }
+    // ---- buffers, all before the first device write (a failed allocation leaves the world as it was) ----
+    if ((rc = alloc_rank_spares(ctx, ctx->keys_resident))) return rc;
+    const uint32_t n_items = ctx->shadow.n_lights;
+    const size_t bytes = ((size_t)n + 2 * n2 + 2 * nd + ctx->lights.n + n_reparent) * 4 + (size_t)n_items * sizeof(ShadowLight) + (size_t)n2 * 12 +
+                         (size_t)T * (sizeof(Tile) + sizeof(WarpTile) + kTileRows) + 16 * 16 + 64;
+    if ((rc = grow_edit_staging(ctx, bytes))) return rc;
+    uint8_t *scratch = ctx->d_stage;
+    size_t scratch_bytes = ctx->stage_bytes;
+    if (o_cols + max_col > scratch_bytes) {
+        // a small world: its 64 B/row staging buffer cannot hold the maps' aligned regions next to the widest column.  A
+        // scratch buffer of its own for this call, large enough for every column in one group
+        scratch_bytes = o_cols + all_cols;
+        const cudaError_t e = cudaMalloc(reinterpret_cast<void **>(&own.tmp), scratch_bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError(); own.tmp = nullptr;
+            return fail(ctx, B200VIS_ERR_OUT_OF_MEMORY, "compact_topology: %zu bytes of scratch: %s", scratch_bytes, cudaGetErrorString(e));
+        }
+        scratch = own.tmp;
+    }
+    if (T > ctx->tiles_cap) {
+        const uint32_t cap = T + 1024;
+        Tile *t = nullptr; WarpTile *w = nullptr; uint8_t *s = nullptr;
+        if (dalloc(&t, cap) != cudaSuccess || dalloc(&w, cap) != cudaSuccess || dalloc(&s, (size_t)cap * kTileRows) != cudaSuccess) {
+            cudaGetLastError();
+            if (t) cudaFree(t); if (w) cudaFree(w); if (s) cudaFree(s);
+            return fail(ctx, B200VIS_ERR_OUT_OF_MEMORY, "compact_topology: tile descriptors for %u tiles", T);
+        }
+        CU(cudaStreamSynchronize(st));
+        cudaFree(ctx->d_tiles); cudaFree(ctx->d_wtiles); cudaFree(ctx->d_sched);
+        ctx->d_tiles = t; ctx->d_wtiles = w; ctx->d_sched = s; ctx->tiles_cap = cap;
+    }
+    uint32_t *d_o2n = reinterpret_cast<uint32_t *>(scratch + o_o2n), *d_n2o = reinterpret_cast<uint32_t *>(scratch + o_n2o);
+    uint32_t *d_drow = reinterpret_cast<uint32_t *>(scratch + o_drow), *d_drk = reinterpret_cast<uint32_t *>(scratch + o_drk);
+    uint32_t *d_src = reinterpret_cast<uint32_t *>(scratch + o_src), *d_flag = reinterpret_cast<uint32_t *>(scratch + o_flag);
+    uint8_t *h = ctx->h_edit;
+    size_t off = 0;
+    auto put = [&](void *dst, const void *src, size_t nb) -> int32_t {
+        if (!nb) return B200VIS_OK;
+        memcpy(h + off, src, nb);
+        CU(cudaMemcpyAsync(dst, h + off, nb, cudaMemcpyHostToDevice, st));
+        off += (nb + 15) & ~(size_t)15;
+        return B200VIS_OK;
+    };
+    const auto t_dev0 = clk::now();
+    if ((rc = put(d_o2n, o2n.data(), (size_t)n * 4))) return rc;
+    if ((rc = put(d_n2o, n2o.data(), (size_t)n2 * 4))) return rc;
+    // ---- ranks: the dropped rows' keys go, every other rank moves down by the dropped ranks below it ----
+    std::vector<uint32_t> drk;
+    if (ctx->rank_identity) drk = dropped;
+    else if (nd) {
+        if ((rc = put(d_drow, dropped.data(), (size_t)nd * 4))) return rc;
+        launch_gather_u32(st, ctx->d_rank, d_drow, nd, d_drk);
+        CU(cudaGetLastError());
+        drk.resize(nd);
+        CU(cudaMemcpyAsync(ctx->h_stage, d_drk, (size_t)nd * 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        memcpy(drk.data(), ctx->h_stage, (size_t)nd * 4);
+        std::sort(drk.begin(), drk.end());
+    }
+    if ((rc = put(d_drk, drk.data(), (size_t)nd * 4))) return rc;
+    CU(cudaMemsetAsync(d_flag, 0, 4, st));
+    launch_compact_ranks(st, ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->keys_resident ? ctx->d_keys : nullptr, n, d_drk, nd, d_o2n,
+                         ctx->d_row_of_rank2, ctx->d_rank2, ctx->keys_resident ? ctx->d_keys2 : nullptr, d_src, d_flag);
+    CU(cudaGetLastError());
+    // last frame's visible sets (bit = rank) to the new ranks, through diff.words (free between frames); words past the new
+    // end cleared
+    if (diff) {
+        const size_t words = (size_t)ctx->vis.words_stride * V;
+        CU(cudaMemcpyAsync(ctx->diff.words, ctx->diff.prev, words * 4, cudaMemcpyDeviceToDevice, st));
+        CU(cudaMemsetAsync(ctx->diff.prev, 0, words * 4, st));
+        launch_remap_rank_sets(st, ctx->diff.words, ctx->diff.prev, ctx->vis.words_stride, V, (n2 + 31) / 32, n2, n, d_src, nullptr);
+        CU(cudaGetLastError());
+    }
+    // ---- the lists results hold, renumbered in place (survivors keep their rank order, so every list stays sorted) ----
+    for (uint32_t i = 0; i < n_lists; ++i) launch_renumber_listed_rows(st, lists[i], n, d_o2n, n);
+    CU(cudaGetLastError());
+    // ---- the row permutation of every resident per-row column, in groups that fit the staging buffer ----
+    {
+        RowPermute pm{};
+        pm.new_to_old = d_n2o; pm.n_new = n2; pm.n_old = n;
+        void *home[kPermuteCols];
+        const size_t avail = scratch_bytes - o_cols;   // >= the widest column (checked before the first write)
+        size_t used = 0;
+        auto flush = [&]() -> int32_t {
+            if (!pm.n_cols) return B200VIS_OK;
+            if (trace) CU(cudaEventRecord(tev[0], st));
+            launch_permute_rows(st, pm);
+            CU(cudaGetLastError());
+            if (trace) CU(cudaEventRecord(tev[1], st));
+            for (uint32_t c = 0; c < pm.n_cols; ++c) {
+                CU(cudaMemcpyAsync(home[c], pm.col[c].dst, (size_t)n * pm.col[c].elem * pm.col[c].per_row, cudaMemcpyDeviceToDevice, st));
+                row_bytes += (size_t)pm.col[c].elem * pm.col[c].per_row;
+            }
+            if (trace) {
+                float a = 0.f, b = 0.f;
+                CU(cudaEventRecord(tev[2], st));
+                CU(cudaEventSynchronize(tev[2]));
+                CU(cudaEventElapsedTime(&a, tev[0], tev[1])); CU(cudaEventElapsedTime(&b, tev[1], tev[2]));
+                gather_ms += a; copy_ms += b;
+            }
+            pm.n_cols = 0; used = 0;
+            return B200VIS_OK;
+        };
+        for (const Column &c : cols) {
+            const size_t nb = al((size_t)n * c.elem * c.per_row);
+            if (used + nb > avail || pm.n_cols == (uint32_t)kPermuteCols) { if ((rc = flush())) return rc; }
+            home[pm.n_cols] = c.p;
+            pm.col[pm.n_cols++] = PermuteColumn{c.p, scratch + o_cols + used, c.elem, c.per_row, c.fill};
+            used += nb;
+        }
+        if ((rc = flush())) return rc;
+    }
+    if (n_reparent) {   // Changed<ChildOf> / RemovedComponents<ChildOf>: marked as the reparent step of edit_topology marks them
+        std::vector<uint32_t> moved(n_reparent);
+        for (uint32_t j = 0; j < n_reparent; ++j) moved[j] = o2n[reparent_rows[j]];
+        uint32_t *d_moved = reinterpret_cast<uint32_t *>(scratch + o_cols);
+        if ((rc = put(d_moved, moved.data(), (size_t)n_reparent * 4))) return rc;
+        RowEdit re{};
+        re.moved = d_moved; re.n_moved = n_reparent;
+        launch_edit_rows(st, ctx->rows, re);
+        CU(cudaGetLastError());
+    }
+    // ---- light and shadow-item rows (ordinals and item order unchanged), the plan, the state past the new end ----
+    for (uint32_t &r : ctx->h_light_row) if (r < n) r = o2n[r];   // a light is never a dead row
+    if ((rc = put(ctx->d_light_row, ctx->h_light_row.data(), (size_t)ctx->lights.n * 4))) return rc;
+    for (ShadowLight &s : ctx->h_shadow) if (s.kind != B200VIS_SHADOW_DIRECTIONAL_CASCADE) s.row = o2n[s.row];
+    if ((rc = put(ctx->d_shadow_lights, ctx->h_shadow.data(), (size_t)n_items * sizeof(ShadowLight)))) return rc;
+    if ((rc = put(ctx->rows.topo, q.topo.data(), (size_t)n2 * 4))) return rc;
+    if ((rc = put(ctx->d_wtopo, q.wtopo.data(), (size_t)n2 * 4))) return rc;
+    if ((rc = put(ctx->d_parent, q.parent.data(), (size_t)n2 * 4))) return rc;
+    if ((rc = put(ctx->d_tiles, q.tiles.data(), (size_t)T * sizeof(Tile)))) return rc;
+    if ((rc = put(ctx->d_wtiles, q.wtiles.data(), (size_t)T * sizeof(WarpTile)))) return rc;
+    if ((rc = put(ctx->d_sched, q.sched.data(), q.sched.size()))) return rc;
+    CU(cudaEventRecord(ctx->ev_edit, st));
+    const uint32_t nw2 = (n2 + 31) / 32, nc2 = (nw2 + kChunkWords - 1) / kChunkWords;
+    {   // growing the row count later relies on every mask word and chunk counter past the count being zero
+        const VisibleBufs &vb = ctx->vis;
+        if (vb.words_stride > nw2) CU(cudaMemset2DAsync(vb.mask + nw2, (size_t)vb.words_stride * 4, 0, (size_t)(vb.words_stride - nw2) * 4, 2 * V, st));
+        if (vb.chunks_stride > nc2) {
+            CU(cudaMemset2DAsync(vb.chunk_count + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4, 3 * kMaxViews, st));
+            if (ctx->diff.chunk) CU(cudaMemset2DAsync(ctx->diff.chunk + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4, V, st));
+            if (ctx->shadow.chunk_count)
+                CU(cudaMemset2DAsync(ctx->shadow.chunk_count + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4,
+                                     (size_t)ctx->shadow_cap_lights * 6, st));
+        }
+    }
+    uint32_t *h_flag = reinterpret_cast<uint32_t *>(h + off);
+    CU(cudaMemcpyAsync(h_flag, d_flag, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    // ---- commit ----
+    std::swap(ctx->d_rank, ctx->d_rank2); std::swap(ctx->d_row_of_rank, ctx->d_row_of_rank2);
+    if (ctx->keys_resident) std::swap(ctx->d_keys, ctx->d_keys2);
+    else {
+        std::vector<uint64_t> keys; keys.reserve(n2);
+        for (uint32_t rk = 0, j = 0; rk < n; ++rk) { if (j < nd && drk[j] == rk) { ++j; continue; } keys.push_back(ctx->h_keys[rk]); }
+        ctx->h_keys.swap(keys);
+    }
+    ctx->rank_identity = *h_flag == 0;
+    *ctx->hplan = std::move(q);
+    install_passes(ctx, *ctx->hplan);
+    ctx->n = n2;
+    ctx->rows.n = n2;
+    ctx->vis.n_words = nw2;
+    ctx->vis.n_chunks = nc2;
+    ctx->gt_aos_valid = false;
+    if (old_to_new_out) memcpy(old_to_new_out, o2n.data(), (size_t)n * 4);
+    if (trace) {
+        const double dev_ms = std::chrono::duration<double, std::milli>(clk::now() - t_dev0).count();
+        fprintf(stderr, "[b200vis_compact] rows %u -> %u (held %zu)  host plan %.3f ms  device part %.3f ms (host clock)  "
+                "permute: %zu B/row, gather %.3f ms, copy-back %.3f ms\n",
+                n, n2, held.size(), plan_ms, dev_ms, row_bytes, gather_ms, copy_ms);
+    }
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_topology_summary(const b200vis_ctx *ctx, uint32_t out[4]) {
     if (!ctx || !out) return B200VIS_ERR_INVALID_ARG;
     const Plan *hp = ctx->hplan;
@@ -1120,6 +1455,21 @@ extern "C" int32_t b200vis_host_edit_plan(uint32_t n, const uint32_t *parent, ui
     counters[0] = counters[1] = counters[3] = 0;
     for (uint32_t at = 0; at < script_words;) {
         if (script_words - at < 3) { rc = fail(nullptr, B200VIS_ERR_INVALID_ARG, "host_edit_plan: truncated step header"); break; }
+        if (script[at] == 0xFFFFFFFFu) {   // compaction step
+            const uint32_t nr = script[at + 1], nh = script[at + 2];
+            const uint64_t len = 3ull + 2ull * nr + nh;
+            if (len > script_words - at) { rc = fail(nullptr, B200VIS_ERR_INVALID_ARG, "host_edit_plan: truncated step"); break; }
+            const uint32_t *a = script + at + 3;
+            const std::vector<uint32_t> held(a + 2 * nr, a + 2 * nr + nh);
+            Plan q;
+            std::vector<uint32_t> o2n, n2o;
+            rc = compact_plan(nullptr, plan, nr, a, a + nr, held, tile_rows, q, o2n, n2o);
+            if (rc) break;
+            plan = std::move(q);
+            counters[0] = (uint32_t)plan.tiles.size(); counters[1] = plan.n; counters[3]++;
+            at += (uint32_t)len;
+            continue;
+        }
         const uint32_t nd = script[at], nr = script[at + 1], ns = script[at + 2];
         const uint64_t len = 3ull + nd + 2ull * nr + ns;
         if (len > script_words - at) { rc = fail(nullptr, B200VIS_ERR_INVALID_ARG, "host_edit_plan: truncated step"); break; }

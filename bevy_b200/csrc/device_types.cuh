@@ -250,4 +250,24 @@ struct RowEdit {
     float2 *range_se;
 };
 
+// b200vis_compact_topology: row-valued lists (list l = rows[l * stride .. + count[l * count_step]))
+struct RowLists {
+    uint32_t *rows;
+    uint32_t stride, n_lists, count_step;
+    const uint32_t *count;
+};
+// ... and the columns one k_permute_rows launch moves (elem = 1, 4, 8 or 16 bytes, per_row elements per row)
+constexpr int kPermuteCols = 16;
+struct PermuteColumn {
+    const void *src; void *dst;
+    uint32_t elem, per_row;
+    unsigned long long fill;    // value of the rows past the new row count
+};
+struct RowPermute {
+    PermuteColumn col[kPermuteCols];
+    uint32_t n_cols;
+    const uint32_t *new_to_old;
+    uint32_t n_new, n_old;
+};
+
 }  // namespace b200vis

@@ -4320,6 +4320,112 @@ void launch_edit_rows(cudaStream_t st, const Rows &R, const RowEdit &e) {
     if (total) { ++g_launches; k_edit_rows<<<cdiv(total, 256), 256, 0, st>>>(R, e); }
 }
 
+// ------------------------------------------------------------------------------------------
+// Compaction (b200vis_compact_topology): the world renumbered on the device.  Run only at compaction time.
+// ------------------------------------------------------------------------------------------
+// Rows named by held results: mark[row] = 1 for every entry of the lists (the first count[l * count_step] rows of list l).
+__global__ void __launch_bounds__(256) k_mark_listed_rows(RowLists L, uint8_t *__restrict__ mark, uint32_t n_rows) {
+    const uint32_t l = blockIdx.y, c = L.count[(size_t)l * L.count_step];
+    const uint32_t *rows = L.rows + (size_t)l * L.stride;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < c; i += gridDim.x * blockDim.x) {
+        const uint32_t r = rows[i];
+        if (r < n_rows) mark[r] = 1;
+    }
+}
+// ... and every row whose rank bit is set in one of the rank-ordered sets
+__global__ void __launch_bounds__(256) k_mark_set_rows(const uint32_t *__restrict__ sets, uint32_t stride, uint32_t n_words,
+                                                       const uint32_t *__restrict__ row_of_rank, uint8_t *__restrict__ mark) {
+    const uint32_t w = blockIdx.x * blockDim.x + threadIdx.x;
+    if (w >= n_words) return;
+    uint32_t bits = sets[(size_t)blockIdx.y * stride + w];
+    while (bits) {
+        const uint32_t b = __ffs(bits) - 1; bits &= bits - 1;
+        const uint32_t rk = w * 32u + b;
+        mark[row_of_rank ? row_of_rank[rk] : rk] = 1;
+    }
+}
+// The lists' rows renumbered in place (a listed row is never dropped: the host keeps every row the lists name).
+__global__ void __launch_bounds__(256) k_renumber_listed_rows(RowLists L, const uint32_t *__restrict__ old_to_new, uint32_t n_old) {
+    const uint32_t l = blockIdx.y, c = L.count[(size_t)l * L.count_step];
+    uint32_t *rows = L.rows + (size_t)l * L.stride;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < c; i += gridDim.x * blockDim.x) {
+        const uint32_t r = rows[i];
+        if (r < n_old) rows[i] = old_to_new[r];
+    }
+}
+__global__ void __launch_bounds__(256) k_gather_u32(const uint32_t *__restrict__ src, const uint32_t *__restrict__ idx, uint32_t n,
+                                                    uint32_t *__restrict__ dst) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dst[i] = src[idx[i]];
+}
+// Ranks after dropping rows: old rank r (kept) moves down by the number of dropped ranks below it (`dropped` is sorted), its
+// row is renumbered through old_to_new.  Writes the new row_of_rank and rank, the keys when they are resident, src_rank
+// (new rank -> old rank, for k_remap_rank_sets) and sets *not_identity when some new rank differs from its row.
+__global__ void __launch_bounds__(256)
+k_compact_ranks(const uint32_t *__restrict__ old_row_of_rank, const uint64_t *__restrict__ old_keys, uint32_t n_old,
+                const uint32_t *__restrict__ dropped, uint32_t n_drop, const uint32_t *__restrict__ old_to_new,
+                uint32_t *__restrict__ row_of_rank, uint32_t *__restrict__ rank, uint64_t *__restrict__ keys,
+                uint32_t *__restrict__ src_rank, uint32_t *__restrict__ not_identity) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_old) return;
+    const uint32_t row = old_to_new[old_row_of_rank ? old_row_of_rank[r] : r];
+    if (row == 0xFFFFFFFFu) return;
+    uint32_t lo = 0, hi = n_drop;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (dropped[mid] < r) lo = mid + 1; else hi = mid; }
+    const uint32_t nr = r - lo;
+    row_of_rank[nr] = row; rank[row] = nr; src_rank[nr] = r;
+    if (keys) keys[nr] = old_keys[r];
+    if (nr != row) atomicOr(not_identity, 1u);
+}
+// The row permutation of the per-row columns: one thread per (new row, element); rows [n_new, n_old) get the column's
+// default.  The destination is a scratch buffer (a gather cannot run in place); the host copies it back.
+__global__ void __launch_bounds__(256) k_permute_rows(const __grid_constant__ RowPermute p) {
+    const PermuteColumn &c = p.col[blockIdx.y];
+    const uint32_t k = c.per_row;
+    const size_t total = (size_t)p.n_old * k;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const uint32_t r = (uint32_t)(i / k), j = (uint32_t)(i - (size_t)r * k);
+        const bool keep = r < p.n_new;
+        const size_t s = keep ? (size_t)p.new_to_old[r] * k + j : 0;
+        switch (c.elem) {
+        case 1: static_cast<uint8_t *>(c.dst)[i] = keep ? static_cast<const uint8_t *>(c.src)[s] : (uint8_t)c.fill; break;
+        case 4: static_cast<uint32_t *>(c.dst)[i] = keep ? static_cast<const uint32_t *>(c.src)[s] : (uint32_t)c.fill; break;
+        case 8: static_cast<unsigned long long *>(c.dst)[i] = keep ? static_cast<const unsigned long long *>(c.src)[s] : c.fill; break;
+        default: static_cast<uint4 *>(c.dst)[i] = keep ? static_cast<const uint4 *>(c.src)[s] : make_uint4(0u, 0u, 0u, 0u); break;
+        }
+    }
+}
+static uint32_t list_grid(uint32_t max_count) { return std::max<uint32_t>(1u, std::min<uint32_t>(cdiv(max_count, 256), 1024u)); }
+void launch_mark_listed_rows(cudaStream_t st, const RowLists &L, uint32_t max_count, uint8_t *mark, uint32_t n_rows) {
+    if (!L.n_lists || !max_count) return;
+    ++g_launches; k_mark_listed_rows<<<dim3(list_grid(max_count), L.n_lists), 256, 0, st>>>(L, mark, n_rows);
+}
+void launch_mark_set_rows(cudaStream_t st, const uint32_t *sets, uint32_t stride, uint32_t n_sets, uint32_t n_words,
+                          const uint32_t *row_of_rank, uint8_t *mark) {
+    if (!n_sets || !n_words) return;
+    ++g_launches; k_mark_set_rows<<<dim3(cdiv(n_words, 256), n_sets), 256, 0, st>>>(sets, stride, n_words, row_of_rank, mark);
+}
+void launch_renumber_listed_rows(cudaStream_t st, const RowLists &L, uint32_t max_count, const uint32_t *old_to_new, uint32_t n_old) {
+    if (!L.n_lists || !max_count) return;
+    ++g_launches; k_renumber_listed_rows<<<dim3(list_grid(max_count), L.n_lists), 256, 0, st>>>(L, old_to_new, n_old);
+}
+void launch_gather_u32(cudaStream_t st, const uint32_t *src, const uint32_t *idx, uint32_t n, uint32_t *dst) {
+    if (n) { ++g_launches; k_gather_u32<<<cdiv(n, 256), 256, 0, st>>>(src, idx, n, dst); }
+}
+void launch_compact_ranks(cudaStream_t st, const uint32_t *old_row_of_rank, const uint64_t *old_keys, uint32_t n_old, const uint32_t *dropped,
+                          uint32_t n_drop, const uint32_t *old_to_new, uint32_t *row_of_rank, uint32_t *rank, uint64_t *keys,
+                          uint32_t *src_rank, uint32_t *not_identity) {
+    if (n_old) { ++g_launches; k_compact_ranks<<<cdiv(n_old, 256), 256, 0, st>>>(old_row_of_rank, old_keys, n_old, dropped, n_drop, old_to_new,
+                                                                                  row_of_rank, rank, keys, src_rank, not_identity); }
+}
+void launch_permute_rows(cudaStream_t st, const RowPermute &p) {
+    if (!p.n_cols || !p.n_old) return;
+    uint32_t k = 1;
+    for (uint32_t c = 0; c < p.n_cols; ++c) k = std::max(k, p.col[c].per_row);
+    const uint32_t blocks = (uint32_t)std::min<size_t>(((size_t)p.n_old * k + 255) / 256, 8192);
+    ++g_launches; k_permute_rows<<<dim3(blocks, p.n_cols), 256, 0, st>>>(p);
+}
+
 }  // namespace b200vis
 
 #ifdef B200VIS_TILE_TIMING

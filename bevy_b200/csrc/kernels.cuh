@@ -58,4 +58,14 @@ void launch_rank_merge(cudaStream_t st, const uint64_t *old_keys, const uint32_t
 void launch_remap_rank_sets(cudaStream_t st, const uint32_t *old_sets, uint32_t *sets, uint32_t stride, uint32_t n_sets, uint32_t n_words,
                             uint32_t n_rows, uint32_t n_old_rows, const uint32_t *row_of_rank, const uint32_t *old_rank);
 void launch_edit_rows(cudaStream_t st, const Rows &R, const RowEdit &e);
+// b200vis_compact_topology
+void launch_mark_listed_rows(cudaStream_t st, const RowLists &L, uint32_t max_count, uint8_t *mark, uint32_t n_rows);
+void launch_mark_set_rows(cudaStream_t st, const uint32_t *sets, uint32_t stride, uint32_t n_sets, uint32_t n_words,
+                          const uint32_t *row_of_rank, uint8_t *mark);
+void launch_renumber_listed_rows(cudaStream_t st, const RowLists &L, uint32_t max_count, const uint32_t *old_to_new, uint32_t n_old);
+void launch_gather_u32(cudaStream_t st, const uint32_t *src, const uint32_t *idx, uint32_t n, uint32_t *dst);
+void launch_compact_ranks(cudaStream_t st, const uint32_t *old_row_of_rank, const uint64_t *old_keys, uint32_t n_old, const uint32_t *dropped,
+                          uint32_t n_drop, const uint32_t *old_to_new, uint32_t *row_of_rank, uint32_t *rank, uint64_t *keys,
+                          uint32_t *src_rank, uint32_t *not_identity);
+void launch_permute_rows(cudaStream_t st, const RowPermute &p);
 }

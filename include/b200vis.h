@@ -182,7 +182,8 @@ B200VIS_API int32_t b200vis_tail_stream(b200vis_ctx *ctx, void **cuda_stream);
 /* ---- mirroring the ECS columns --------------------------------------------- */
 /* Hierarchy + identity: the whole world, planned from scratch, with fresh frame state (every visible entity is
  * reported added by the next visible diff).  Per-frame spawns, despawns and ChildOf changes go through
- * b200vis_edit_topology instead; this call is its fallback and the compaction that drops despawned rows.
+ * b200vis_edit_topology instead, and b200vis_compact_topology drops the tombstones they leave; this call is for the
+ * first upload and for world_size > 1.
  * Replaces the Children/ChildOf walks of propagate_descendants_unchecked
  * (systems.rs:679-748) with a cached execution plan.  entity_bits = Entity::to_bits()
  * (crates/bevy_ecs/src/entity/mod.rs:468-476), which fixes the order of every
@@ -201,7 +202,8 @@ B200VIS_API int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n_rows, cons
  * INVALID_ARG (a row out of range or dead, entity bits equal to those of any row, live or dead, a despawned row with live
  * children, a despawned row that is still in the b200vis_set_lights list or a point / spot shadow item: remove it there
  * first); UNSUPPORTED (a parent at or after its child's row, a tile that would need more than 128 rows with in-tile
- * children, world_size > 1).  On UNSUPPORTED or CAPACITY, fall back to b200vis_set_topology.
+ * children, world_size > 1).  On UNSUPPORTED or CAPACITY, compact with b200vis_compact_topology (which also takes the
+ * reparents that break the row order) and repeat the rest of the edit.
  * Dead rows: parent B200VIS_DETACHED, flags B200VIS_F_NO_CPU_CULLING only, ViewVisibility 0, no VisibilityClass, not a
  * shadow caster.  They are in no visible, shadow or cluster list; a dead row that was visible is reported removed by
  * the next visible diff; its Changed flags never fire (the write-back mirrors its ViewVisibility 0 once).
@@ -214,8 +216,25 @@ B200VIS_API int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n_rows, cons
 B200VIS_API int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, const uint32_t *despawn_rows,
                                           uint32_t n_reparent, const uint32_t *reparent_rows, const uint32_t *new_parent,
                                           uint32_t n_spawn, const uint32_t *spawn_parent, const uint64_t *spawn_entity_bits);
-/* out = { rows (tombstones included), live rows, tiles, passes }: what a caller weighs before compacting with
- * b200vis_set_topology. */
+/* Renumber the world on the device: drop the tombstones b200vis_edit_topology left, apply reparents that need not keep
+ * row order, and re-plan -- keeping every column and the frame history resident.
+ * reparent_rows[n_reparent] -> new_parent[] use the current row numbers; a new parent is a live row anywhere in the world,
+ * B200VIS_NO_PARENT or B200VIS_DETACHED.  The rows are marked changed as the reparent step of b200vis_edit_topology marks
+ * them.  New row order: b200vis_plan_row_order over the surviving rows in their current order, reparents applied; the
+ * plan is the one b200vis_set_topology builds for that hierarchy.  old_to_new[r] (nullable, one entry per row before the
+ * call) = the new number of row r, or 0xFFFFFFFF if it was dropped: renumber the entity <-> row maps, the host mirror
+ * columns and the memory given to b200vis_set_column_sinks with it before the next write-back.
+ * A dead row that a held result still names -- any view slot's visible list (an inactive view keeps its list), the
+ * visible diff and the visible sets it compares against, a shadow list -- survives as a tombstone and goes at a later
+ * compaction.  Every output after the call (GlobalTransform, change flags, ViewVisibility, visible lists and classes,
+ * visible diff, shadow lists, clusters, statistics, sinks) equals what the uncompacted world gives, renumbered through
+ * old_to_new; the compaction itself sets no Changed flag.  Light ordinals and shadow-item order are kept.
+ * All or nothing.  Errors: INVALID_ARG (a reparented row out of range or dead or listed twice, a new parent out of range
+ * or dead), HIERARCHY_CYCLE, UNSUPPORTED (world_size > 1), NOT_READY (no b200vis_set_topology yet). */
+B200VIS_API int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparent, const uint32_t *reparent_rows,
+                                             const uint32_t *new_parent, uint32_t *old_to_new /* [rows before], nullable */);
+/* out = { rows (tombstones included), live rows, tiles, passes }: what a caller weighs before calling
+ * b200vis_compact_topology. */
 B200VIS_API int32_t b200vis_topology_summary(const b200vis_ctx *ctx, uint32_t out[4]);
 /* Helper for the shim: a permutation (new_row -> old_row) that is topological and
  * keeps every tree contiguous in BFS order (the layout the tile kernel likes). */
@@ -240,6 +259,9 @@ B200VIS_API int32_t b200vis_host_warp_plan(uint32_t n_rows, const uint32_t *pare
 /* The plan b200vis_edit_topology keeps, after an edit script (no GPU needed; for tests and tools).  The script is a
  * sequence of steps, each { n_despawn, n_reparent, n_spawn, despawn_rows[n_despawn], reparent_rows[n_reparent],
  * new_parent[n_reparent], spawn_parent[n_spawn] }, applied like b200vis_edit_topology calls with at most max_rows rows.
+ * A step { 0xFFFFFFFF, n_reparent, n_held, reparent_rows[n_reparent], new_parent[n_reparent], held_rows[n_held] } is
+ * a b200vis_compact_topology call whose held results name the dead rows held_rows[] (tile_rows != 0: the new plan is cut
+ * with that tile size instead of b200vis_set_topology's search).
  * Returns the first failing step's error (the outputs then hold the plan before that step).  *n_rows = rows after
  * the script; tile_desc[i][17] = { the 8 words of b200vis_host_tile_plan, chunks | contiguous-chunk bits << 8,
  * nonroot[8] of b200vis_host_warp_plan }, sched[i][256], topo[row], wtopo[row] as there; counters = { tiles re-planned
