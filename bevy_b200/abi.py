@@ -136,6 +136,7 @@ _SIGNATURES = {
     "b200vis_upload_transforms_scattered": (C.c_int32, [_vp, C.c_uint32, _vp, _vp]),
     "b200vis_mark_transforms_changed": (C.c_int32, [_vp, C.c_uint32, C.c_uint32]),
     "b200vis_upload_global_transforms": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp]),
+    "b200vis_write_global_transforms_scattered": (C.c_int32, [_vp, C.c_uint32, _vp, _vp]),
     "b200vis_upload_bounds": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
     "b200vis_upload_view_visibility": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp]),
     "b200vis_set_static_transform_optimizations": (C.c_int32, [_vp, C.c_int32]),
@@ -484,6 +485,13 @@ class Context:
     def upload_global_transforms(self, first_row, gt):
         g = _arr(gt, np.float32).reshape(-1, 12)
         self._check(self._lib.b200vis_upload_global_transforms(self._h, first_row, len(g), _ptr(g)))
+
+    def write_global_transforms_scattered(self, rows, gt):
+        """GlobalTransforms another system wrote since the last PROPAGATE (b200vis_write_global_transforms_scattered):
+        sets the rows' values and marks them changed for the next propagate pass."""
+        r = _arr(rows, np.uint32); g = _arr(gt, np.float32).reshape(-1, 12)
+        assert len(r) == len(g)
+        self._check(self._lib.b200vis_write_global_transforms_scattered(self._h, len(r), _ptr(r), _ptr(g)))
 
     def upload_bounds(self, first_row, bounds, flags, class_mask, layer_mask=None, range_mask=None):
         b = _arr(bounds, np.float32).reshape(-1, 6); f = _arr(flags, np.uint8); c = _arr(class_mask, np.uint8)

@@ -12,7 +12,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libb200vis.so")
 SOURCES = ["kernels.cu", "api.cu", "host_view.cpp"]
-HEADERS = ["device_types.cuh", "kernels.cuh", "host_view.hpp", os.path.join("..", "..", "include", "b200vis.h")]
+HEADERS = ["device_types.cuh", "kernels.cuh", "tile_kernel_1b.cuh","host_view.hpp", os.path.join("..", "..", "include", "b200vis.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",

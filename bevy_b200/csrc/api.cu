@@ -98,6 +98,9 @@ struct b200vis_ctx {
     std::vector<uint32_t> pass_small;   // the first pass_small[p] tiles of pass p have <= 32 rows (B200VIS_SPLIT_DEEP_TILES)
     std::vector<uint8_t> pass_named;    // every tile of pass p is flat or walks with named level barriers (Tile::lvl_warps): the tile kernel may let a CTA's warps drift a tile apart
     int static_opt = 1;
+    // b200vis_write_global_transforms_scattered left S_GT_EXT marks that no run with PROPAGATE has consumed yet (rows the
+    // edit despawned since may have lost theirs): the next propagate pass runs kernel 1b's marked instantiation
+    bool gt_ext_pending = false;
     // b200vis_edit_topology: the host plan kept between calls, the world's keys (Entity::to_bits()) in rank order -- on the
     // host after set_topology, on the device from the first edit that needs a merge -- and the spare rank arrays a merge
     // writes into (swapped in when the edit is committed)
@@ -954,6 +957,11 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         for (uint32_t i = 0; i < n; ++i) rank[order[i]] = i;
     }
     cudaStream_t st = ctx->stream;
+    if (ctx->gt_ext_pending) {     // a new world: GlobalTransforms written into the old one are no longer pending
+        launch_clear_gt_ext(st, ctx->rows, ctx->n);
+        CU(cudaGetLastError());
+        ctx->gt_ext_pending = false;
+    }
     CU(cudaStreamSynchronize(st));   // the vectors below are pageable and short-lived: copy synchronously
     CU(cudaMemcpy(ctx->rows.topo, topo.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice));
@@ -1649,6 +1657,37 @@ extern "C" int32_t b200vis_upload_global_transforms(b200vis_ctx *ctx, uint32_t f
     CU(cudaGetLastError());
     return B200VIS_OK;
 }
+extern "C" int32_t b200vis_write_global_transforms_scattered(b200vis_ctx *ctx, uint32_t count, const uint32_t *rows, const float *gt) {
+    CHECK_CTX();
+    if (!ctx->topology_set) return fail(ctx, B200VIS_ERR_NOT_READY, "write_global_transforms_scattered: b200vis_set_topology has not been called");
+    if (count && (!rows || !gt)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "write_global_transforms_scattered: null array");
+    for (uint32_t i = 0; i < count; ++i)
+        if (rows[i] >= ctx->n || row_is_dead(ctx, rows[i]))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "write_global_transforms_scattered: row %u (entry %u) out of range or despawned", rows[i], i);
+    if (!count) return B200VIS_OK;
+    // a row listed twice takes its last value: keep the last entry of every row, so that the scatter kernel's rows are distinct
+    std::vector<uint64_t> key(count);
+    for (uint32_t i = 0; i < count; ++i) key[i] = (uint64_t)rows[i] << 32 | i;
+    std::sort(key.begin(), key.end());
+    std::vector<uint32_t> urows; std::vector<float> ugt;
+    urows.reserve(count); ugt.reserve((size_t)count * 12);
+    for (uint32_t k = 0; k < count; ++k) {
+        if (k + 1 < count && (key[k + 1] >> 32) == (key[k] >> 32)) continue;
+        const uint32_t i = (uint32_t)key[k];
+        urows.push_back(rows[i]);
+        ugt.insert(ugt.end(), gt + (size_t)i * 12, gt + (size_t)i * 12 + 12);
+    }
+    const uint32_t m = (uint32_t)urows.size();
+    const size_t off_rows = ((size_t)m * 48 + 15) & ~(size_t)15;
+    int32_t rc = stage_in(ctx, ugt.data(), (size_t)m * 48, 0); if (rc) return rc;
+    rc = stage_in(ctx, urows.data(), (size_t)m * 4, off_rows); if (rc) return rc;
+    launch_write_gt_scattered(ctx->stream, ctx->rows, m, reinterpret_cast<const uint32_t *>(ctx->d_stage + off_rows),
+                              reinterpret_cast<const float *>(ctx->d_stage));
+    CU(cudaGetLastError());
+    ctx->gt_ext_pending = true;
+    ctx->gt_aos_valid = false;     // the dense write-back's copy of the column no longer holds what the host holds
+    return B200VIS_OK;
+}
 extern "C" int32_t b200vis_upload_bounds(b200vis_ctx *ctx, uint32_t first, uint32_t count, const float *bounds,
                                          const uint8_t *flags, const uint8_t *class_mask, const uint64_t *layer_mask,
                                          const uint32_t *range_mask) {
@@ -2076,6 +2115,13 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     cudaStream_t st = ctx->stream;
     const bool do_prop = stages & B200VIS_STAGE_PROPAGATE, do_cull = stages & B200VIS_STAGE_CULL;
     const bool has_assign = stages & B200VIS_STAGE_CLUSTER_ASSIGN, has_lists = stages & B200VIS_STAGE_CLUSTER_LISTS;
+    // pending external GlobalTransform writes: only kernel 1b has the marked instantiation
+    const bool gt_ext = do_prop && ctx->gt_ext_pending;
+    if (gt_ext && !tile_kernel_is_default()) {
+        const char *e = getenv("B200VIS_TILE_KERNEL");
+        return fail(ctx, B200VIS_ERR_UNSUPPORTED, "run: GlobalTransforms written by b200vis_write_global_transforms_scattered are pending, "
+                    "and B200VIS_TILE_KERNEL=%s selects a tile kernel that does not read them (unset it, or set it to tma)", e ? e : "");
+    }
     // ---- continuation of an open tail: CLUSTER_LISTS after the host's all-gather, still on the side stream --------
     if (ctx->pipeline && ctx->tail_open && stages == B200VIS_STAGE_CLUSTER_LISTS) {
         ClusterBufs cl = ctx->cl;
@@ -2169,7 +2215,14 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     if (do_prop || do_cull) {
         const uint32_t tile_stages = (do_prop ? 1u : 0u) | (do_cull ? 2u : 0u);
         if (do_prop) {
-            for (uint32_t p = 0; p < n_pass; ++p) {
+            for (uint32_t p = 0; p < n_pass && gt_ext; ++p) {
+                // the whole pass, small tiles (B200VIS_SPLIT_DEEP_TILES) included, through kernel 1b's marked instantiation
+                const uint32_t b = ctx->pass_begin[p];
+                launch_propagate_cull_ext(st, R, ctx->d_tiles + b, ctx->pass_begin[p + 1] - b, cvw, vb, ctx->d_stats, tile_stages,
+                                          (uint32_t)ctx->static_opt, cslot, ctx->d_tile_ticket, &ctx->tile_ticket_base);
+            }
+            if (gt_ext) ctx->gt_ext_pending = false;
+            for (uint32_t p = 0; p < n_pass && !gt_ext; ++p) {
                 const uint32_t ns = p < ctx->pass_small.size() ? ctx->pass_small[p] : 0u, b = ctx->pass_begin[p];
                 if (ns) launch_propagate_cull_small(st, R, ctx->d_tiles + b, ns, cvw, vb, ctx->d_stats, tile_stages, (uint32_t)ctx->static_opt, cslot);
                 if (tile_kernel_is_warp())

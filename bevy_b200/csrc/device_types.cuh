@@ -15,8 +15,12 @@ constexpr uint32_t kDetached = 0xFFFFFFFEu;
 // row flag byte (include/b200vis.h)
 constexpr uint32_t F_INHERITED = 0x01, F_AABB = 0x02, F_SPHERE = 0x04, F_NO_FRUSTUM = 0x08, F_RANGE = 0x10,
                    F_NO_CPU_CULL = 0x20, F_SPHERE_GT = 0x40, F_TCHANGED = 0x80;
-// per-row device state byte: bits 0-1 ViewVisibility, 4 gt_changed, 5 vv_changed, 6 visited, 7 has_class
+// per-row device state byte: bits 0-1 ViewVisibility, 2 gt_ext, 3 gt_handed, 4 gt_changed, 5 vv_changed, 6 visited, 7 has_class
 constexpr uint32_t S_VV = 0x03, S_GT_CHANGED = 0x10, S_VV_CHANGED = 0x20, S_VISITED = 0x40, S_HAS_CLASS = 0x80;
+// b200vis_write_global_transforms_scattered: S_GT_EXT marks a GlobalTransform another system wrote since the last PROPAGATE
+// (set by k_write_gt_scattered, consumed by the next propagate pass); S_GT_HANDED is what a row the propagate pass visited hands
+// its children in other tiles, changed || (visited && S_GT_EXT) (only the marked instantiation of kernel 1b writes and reads it)
+constexpr uint32_t S_GT_EXT = 0x04, S_GT_HANDED = 0x08;
 // topo word: parent_local[0:9) local_depth[9:18) | flags
 constexpr uint32_t T_ROOT = 1u << 28, T_HAS_CHILDREN = 1u << 29, T_EXT_PARENT = 1u << 30, T_DETACHED = 1u << 31;
 

@@ -477,301 +477,17 @@ __device__ unsigned long long g_tile_timing[8192 * 16];
 #define TT(slot) do { } while (0)
 #define TTW(slot) do { } while (0)
 #endif
-template <bool PROP, bool CULL, bool SIMPLE>
-__global__ void __launch_bounds__(kTileRows, 4)
-k_propagate_cull_tma(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const __grid_constant__ CullViews cvw,
-                     VisibleBufs vb, DevStats *__restrict__ stats, uint32_t static_opt, uint32_t parity,
-                     uint32_t *__restrict__ ticket, uint32_t ticket_base) {
-    extern __shared__ __align__(128) uint8_t smem_raw[];
-    TmaSmem &s = *reinterpret_cast<TmaSmem *>(smem_raw);
-    const uint32_t lr = threadIdx.x;
-    if (lr == 0) {
-        mbar_init(&s.bar[0], 1); mbar_init(&s.bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    // launched with programmatic stream serialization: everything above overlapped the previous kernel's tail
-    TT(0);
-    asm volatile("griddepcontrol.wait;" ::: "memory");
-    TT(1);
-    uint32_t t = blockIdx.x;
-    if (lr == 0 && t < n_tiles) issue_tile_loads<PROP, CULL>(R, tiles[t], s.st[0], &s.bar[0]);
-    uint32_t n_gt_total = 0, n_vv_total = 0;
-    // Tile hand-out: a CTA starts on tile blockIdx.x and then takes the tiles the grid has not started yet in ticket order
-    // (one atomic per tile, drawn by thread 0 when it prefetches, i.e. one tile ahead).  A fixed stride would leave a CTA with
-    // ceil(n/g) tiles running next to finished neighbours with floor(n/g) -- a fifth of the pass at 3.3 tiles per CTA.  The
-    // ticket counter is never reset: every launch draws exactly n_tiles tickets, and the host passes the running base.
-    for (uint32_t it = 0; t < n_tiles; ++it) {
-        const uint32_t sidx = it & 1u;
-        const Tile tile = tiles[t];
-        mbar_wait(&s.bar[sidx], (it >> 1) & 1u);
-        if (it == 1) { TT(2); }
-        TileStage &S = s.st[sidx];
-        const uint32_t off = tile.base & 15u;
-        const uint32_t li = off + lr;                 // index into the staged window
-        const bool active = lr < tile.n_rows;
-        const uint32_t row = tile.base + lr;
-        const uint32_t f = active ? S.flags[li] : 0u;
-        const uint32_t st8 = active ? S.state[li] : 0u;
-        // bounds are only needed after the hierarchy walk: plain coalesced loads issued now, consumed in phase 3
-        // (keeping them out of the staged window lets a fourth CTA fit in shared memory)
-        float4 bA = make_float4(0, 0, 0, 0); float2 bB = make_float2(0, 0);
-        if (CULL && active) { bA = R.bndA[row]; bB = R.bndB[row]; }
-
-        bool visited = false, changed = false;
-        if (PROP) {
-            const uint32_t topo = active ? S.topo[li] : T_DETACHED;
-            const uint32_t depth = (topo >> 9) & 0x1FFu, plocal = topo & 0x1FFu;
-            const bool tchanged = f & F_TCHANGED;
-            const bool has_children = topo & T_HAS_CHILDREN;
-            bool dirty = tchanged;
-            if (static_opt && R.dirty != nullptr) {
-                dirty = active && R.dirty[row];
-            } else if (static_opt && tile.n_levels > 1 && __syncthreads_or(tchanged && depth > 0)) {
-                // only when a non-root row of the tile changed does anything have to climb: otherwise every row's
-                // TransformTreeChanged bit equals its own Changed<Transform> bit (one barrier instead of two + a climb)
-                s.parent[lr] = (uint16_t)((depth > 0) ? plocal : 0xFFFFu);
-                s.dirty[lr] = 0;
-                __syncthreads();
-                if (active && tchanged) {
-                    uint32_t c = lr;
-                    while (!s.dirty[c]) {
-                        s.dirty[c] = 1;
-                        const uint32_t p = s.parent[c];
-                        if (p == 0xFFFFu) break;
-                        c = p;
-                    }
-                }
-                __syncthreads();
-                dirty = s.dirty[lr];
-            }
-            if (it == 1) { TT(3); }    // dirty phase done
-            const Aff l = affine_from_trs(S.trsA[li], S.trsB[li], S.trsC[li]);
-            const uint32_t my_level = (active && !(topo & T_DETACHED)) ? depth : 0xFFFFFFFFu;
-            if (active && (topo & T_DETACHED) && has_children) s.pst[lr] = 0;
-            if (my_level == 0) {
-                Aff n = l;
-                if (topo & T_ROOT) {
-                    visited = has_children ? (!static_opt || dirty) : tchanged;
-                    changed = visited;
-                } else {
-                    const uint32_t pr = R.parent[row];
-                    const uint32_t ps = R.state[pr];
-                    visited = (ps & S_VISITED) && !(static_opt && !dirty && !(ps & S_GT_CHANGED));
-                    if (visited) {
-                        n.r0 = affine_mul_row(R.gt0[pr], l); n.r1 = affine_mul_row(R.gt1[pr], l); n.r2 = affine_mul_row(R.gt2[pr], l);
-                        changed = row_neq(n.r0, S.gt0[li]) | row_neq(n.r1, S.gt1[li]) | row_neq(n.r2, S.gt2[li]);
-                    }
-                }
-                if (changed) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
-                if (has_children) s.pst[lr] = (uint8_t)((visited ? 1u : 0u) | (changed ? 2u : 0u));
-            }
-            if (it == 1) { TT(4); }    // local affine + level 0 done
-            // one level of the walk for this thread's row: the parent's rows are the tile's own (in-place) GlobalTransform entries
-            auto walk_row = [&]() {
-                const uint32_t pst = s.pst[plocal];
-                const uint32_t pi = off + plocal;
-                visited = (pst & 1u) && !(static_opt && !dirty && !(pst & 2u));
-                if (visited) {
-                    Aff n;
-                    n.r0 = affine_mul_row(S.gt0[pi], l); n.r1 = affine_mul_row(S.gt1[pi], l); n.r2 = affine_mul_row(S.gt2[pi], l);
-                    changed = row_neq(n.r0, S.gt0[li]) | row_neq(n.r1, S.gt1[li]) | row_neq(n.r2, S.gt2[li]);   // set_if_neq
-                    if (changed) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
-                }
-                if (has_children) s.pst[lr] = (uint8_t)((visited ? 1u : 0u) | (changed ? 2u : 0u));
-            };
-            if (tile.lvl_warps != 0ull) {
-                // Per-warp level schedule (2..8 levels).  A warp only takes part in the hand-over of the levels its own rows
-                // produce (level l-1) or consume (level l), through hardware named barrier l with exactly the warps the planner
-                // counted (Tile::lvl_warps): consumers bar.sync, pure producers bar.arrive and go on; a leaf warp waits once
-                // instead of once per level, and nobody pays the loop for levels that are not theirs.  (The tile still ends in a
-                // CTA-wide barrier, so one set of barrier ids is enough here.)
-                // (a detached row takes no part in the walk but publishes pst = 0 for its children: it counts as a level-0 row)
-                const uint32_t lmask = __reduce_or_sync(0xFFFFFFFFu, active ? (1u << (depth & 15u)) : 0u);
-                uint32_t need = (lmask | (lmask << 1)) & ((1u << tile.n_levels) - 2u);
-                while (need) {
-                    const uint32_t lvl = (uint32_t)__ffs((int)need) - 1u;
-                    need &= need - 1u;
-                    const bool consumer = (lmask >> lvl) & 1u;
-                    if ((tile.warp_sync_mask >> lvl) & 1u) {       // every edge into this level stays inside a warp
-                        if (!consumer) continue;
-                        __syncwarp();
-                    } else {
-                        const uint32_t cnt = ((uint32_t)(tile.lvl_warps >> (4u * lvl)) & 15u) * 32u;
-                        if (!consumer) {
-                            __threadfence_block();
-                            asm volatile("bar.arrive %0, %1;" ::"r"(lvl), "r"(cnt) : "memory");
-                            continue;
-                        }
-                        asm volatile("bar.sync %0, %1;" ::"r"(lvl), "r"(cnt) : "memory");
-                    }
-                    if (my_level == lvl) walk_row();
-                }
-            } else {
-                for (uint32_t lvl = 1; lvl < tile.n_levels; ++lvl) {
-                    if (lvl < 32u && ((tile.warp_sync_mask >> lvl) & 1u)) __syncwarp(); else __syncthreads();
-                    if (my_level == lvl) walk_row();
-                    if (it == 1 && lvl <= 7) { TT(4 + lvl); }   // thread 0 after the level's barrier and (for level-lvl rows) work
-                }
-            }
-            if (active && tchanged) R.flags[row] = (uint8_t)(f & ~F_TCHANGED);
-        }
-        if (it == 1) { TT(12); }   // walk done
-        // Prefetch the NEXT tile into the other stage.  That stage was last read by the previous tile's bulk store,
-        // issued most of an iteration ago, so the wait below is (almost always) already satisfied: putting the
-        // prefetch here instead of at the top of the loop keeps the store drain off every warp's critical path.
-        if (lr == 0) {
-            const uint32_t tn = ticket ? gridDim.x + (atomicAdd(ticket, 1u) - ticket_base) : t + gridDim.x;
-            if (tn < n_tiles) {
-                asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-                issue_tile_loads<PROP, CULL>(R, tiles[tn], s.st[sidx ^ 1u], &s.bar[sidx ^ 1u]);
-            }
-            s.next_tile[sidx] = tn;      // read by everybody behind the tile's closing barrier
-        }
-        uint32_t out = st8 & (S_VV | S_HAS_CLASS);
-        if (PROP) out |= (changed ? S_GT_CHANGED : 0u) | (visited ? S_VISITED : 0u);
-        else out |= st8 & (S_GT_CHANGED | S_VISITED);
-
-        bool vv_changed = false;
-        if (CULL) {
-            Aff g; g.r0 = S.gt0[li]; g.r1 = S.gt1[li]; g.r2 = S.gt2[li];   // own row: written by this thread or untouched
-            const bool in_query = active && !(f & F_NO_CPU_CULL);
-            const bool base = in_query && (f & F_INHERITED);
-        const bool rej_base = base;
-            const uint32_t prev = st8 & 1u;
-            const uint32_t lane = lr & 31u;
-            const bool has_aabb = f & F_AABB;
-            const bool do_test = (f & (F_AABB | F_SPHERE)) && !(f & F_NO_FRUSTUM);
-            float cx, cy, cz, radius;
-            const float hx = bA.w, hy = bB.x, hz = bB.y;
-            if (has_aabb) {
-                cx = ((g.r0.x * bA.x + g.r0.y * bA.y) + g.r0.z * bA.z) + g.r0.w;
-                cy = ((g.r1.x * bA.x + g.r1.y * bA.y) + g.r1.z * bA.z) + g.r1.w;
-                cz = ((g.r2.x * bA.x + g.r2.y * bA.y) + g.r2.z * bA.z) + g.r2.w;
-                const float vx = (g.r0.x * hx + g.r0.y * hy) + g.r0.z * hz;
-                const float vy = (g.r1.x * hx + g.r1.y * hy) + g.r1.z * hz;
-                const float vz = (g.r2.x * hx + g.r2.y * hy) + g.r2.z * hz;
-                radius = sqrtf((vx * vx + vy * vy) + vz * vz);
-            } else {
-                const bool from_gt = f & F_SPHERE_GT;
-                cx = from_gt ? g.r0.w : bA.x; cy = from_gt ? g.r1.w : bA.y; cz = from_gt ? g.r2.w : bA.z;
-                radius = bA.w;
-            }
-            unsigned long long elayers = 1ull; uint32_t erange = 0xFFFFFFFFu, rnk = row;
-            if (!SIMPLE && active) {
-                if (R.layers != nullptr) elayers = R.layers[row];
-                if ((f & F_RANGE) && R.range != nullptr) erange = range_mask_of(R, row, has_aabb, cx, cy, cz, g);
-                if (R.rank != nullptr) rnk = R.rank[row];
-            }
-            // warp-level shortcut: views whose frustum the whole warp's rows are outside of (see warp_view_reject)
-            const uint32_t rejmask = warp_view_reject(cvw, rej_base && do_test, rej_base && !do_test, cx, cy, cz, radius);
-            bool any = false;
-            uint32_t my_ballot = 0;
-#pragma unroll
-            for (uint32_t v = 0; v < kMaxViews; ++v) {
-                if (v >= cvw.n_views) break;
-                const uint32_t von = cvw.on[v];
-                if (!(von & 1u)) continue;
-                if (SIMPLE && !(von & 4u)) continue;   // bit2: the view includes the default layer
-                if (((rejmask >> v) & 1u) && !(von & 2u)) continue;         // every row of this warp is outside this view's frustum
-                bool vis = base;
-                if (!SIMPLE) {
-                    vis = vis && layers_intersect(R, cvw, row, v, elayers);
-                    if ((f & F_RANGE) && R.range != nullptr) {
-                        const int32_t ri = cvw.range_index[v];
-                        vis = vis && ri >= 0 && ((erange >> ri) & 1u);
-                    }
-                }
-                if (do_test && !(von & 2u)) {
-                    const float d0 = plane_dot_point(cvw.planes[v][0], cx, cy, cz), d1 = plane_dot_point(cvw.planes[v][1], cx, cy, cz);
-                    const float d2 = plane_dot_point(cvw.planes[v][2], cx, cy, cz), d3 = plane_dot_point(cvw.planes[v][3], cx, cy, cz);
-                    const float d4 = plane_dot_point(cvw.planes[v][4], cx, cy, cz);
-                    const bool out_s = (d0 + radius <= 0.0f) | (d1 + radius <= 0.0f) | (d2 + radius <= 0.0f) |
-                                       (d3 + radius <= 0.0f) | (d4 + radius <= 0.0f);
-                    vis = vis && !out_s;
-                    if (vis && has_aabb) {
-                        const float d[5] = {d0, d1, d2, d3, d4};
-                        bool out_o = false;
-#pragma unroll
-                        for (int k = 0; k < 5; ++k) {
-                            const float4 n = cvw.planes[v][k];
-                            const float dx = fabsf(dot3(n.x, n.y, n.z, g.r0.x, g.r1.x, g.r2.x));
-                            const float dy = fabsf(dot3(n.x, n.y, n.z, g.r0.y, g.r1.y, g.r2.y));
-                            const float dz = fabsf(dot3(n.x, n.y, n.z, g.r0.z, g.r1.z, g.r2.z));
-                            const float rr = (dx * hx + dy * hy) + dz * hz;
-                            out_o |= (d[k] + rr <= 0.0f);
-                        }
-                        vis = !out_o;
-                    }
-                }
-                any |= vis;
-                const bool listed = vis && (st8 & S_HAS_CLASS);
-                if (SIMPLE || R.rank == nullptr) {
-                    const uint32_t b = __ballot_sync(0xFFFFFFFFu, listed);
-                    if (lane == v) my_ballot = b;
-                } else if (listed) {
-                    uint32_t *mask = vb.mask + (size_t)v * vb.words_stride;
-                    uint32_t *cc = vb.chunk_count + ((size_t)parity * kMaxViews + v) * vb.chunks_stride;
-                    atomicOr(mask + (rnk >> 5), 1u << (rnk & 31u));
-                    atomicAdd(cc + ((rnk >> 5) / kChunkWords), 1u);
-                }
-            }
-            if (my_ballot) {
-                uint32_t *mask = vb.mask + (size_t)lane * vb.words_stride;
-                uint32_t *cc = vb.chunk_count + ((size_t)parity * kMaxViews + lane) * vb.chunks_stride;
-                const uint32_t row0 = row - lane, w0 = row0 >> 5, sh = row0 & 31u;
-                const uint32_t lo = my_ballot << sh, hi = sh ? (my_ballot >> (32u - sh)) : 0u;
-                if (lo) { atomicOr(mask + w0, lo); atomicAdd(cc + (w0 / kChunkWords), __popc(lo)); }
-                if (hi) { atomicOr(mask + w0 + 1, hi); atomicAdd(cc + ((w0 + 1) / kChunkWords), __popc(hi)); }
-            }
-            if (in_query) {
-                out = (out & ~S_VV) | (any ? (1u | (prev << 1)) : 0u);
-                vv_changed = (any ? 1u : 0u) != prev;
-                if (vv_changed) out |= S_VV_CHANGED;
-            }
-        } else {
-            out |= st8 & S_VV_CHANGED;
-        }
-        if (active && out != st8) R.state[row] = (uint8_t)out;
-        // a light row publishes what assign_objects_to_clusters needs of it (GlobalTransform::translation,
-        // ViewVisibility::get) so that the cluster kernels never touch the row arrays again
-        if (CULL && R.light_snap != nullptr && (f & F_SPHERE_GT) && active) {
-            const uint32_t ord = R.light_ord[row];     // 0xFFFFFFFF: a sphere-from-GT row that is not a current light
-            if (ord < R.n_lights) R.light_snap[ord] = make_float4(S.gt0[li].w, S.gt1[li].w, S.gt2[li].w, (out & 1u) ? 1.0f : 0.0f);
-        }
-
-        // end of tile: everybody is done with this stage; count changes; write the tile's matrices back
-        n_gt_total += (PROP && changed) ? 1u : 0u;      // per-thread tallies, reduced once at the end of the kernel
-        n_vv_total += vv_changed ? 1u : 0u;
-        if (it == 1) { TT(13); }   // cull done
-        const int any_gt = __syncthreads_or(PROP && changed);
-        if (it == 1) { TT(15); }
-        t = s.next_tile[sidx];
-        if (lr == 0) {
-            if (PROP && any_gt) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic smem writes -> async proxy
-                const uint32_t bytes = (uint32_t)tile.n_rows * 16u;
-                bulk_s2g(R.gt0 + tile.base, S.gt0 + off, bytes); bulk_s2g(R.gt1 + tile.base, S.gt1 + off, bytes);
-                bulk_s2g(R.gt2 + tile.base, S.gt2 + off, bytes);
-                asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-            }
-        }
-    }
-    if (lr == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    TT(14);
-    // block-reduce the per-thread tallies (warp shuffle, then one shared-memory atomic per warp)
-    __shared__ uint32_t s_cnt[2];
-    if (lr < 2) s_cnt[lr] = 0;
-    __syncthreads();
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) { n_gt_total += __shfl_xor_sync(0xFFFFFFFFu, n_gt_total, o); n_vv_total += __shfl_xor_sync(0xFFFFFFFFu, n_vv_total, o); }
-    if ((lr & 31u) == 0) { if (n_gt_total) atomicAdd(&s_cnt[0], n_gt_total); if (n_vv_total) atomicAdd(&s_cnt[1], n_vv_total); }
-    __syncthreads();
-    if (lr == 0) {
-        if (s_cnt[0]) atomicAdd(&stats->changed[parity][0], s_cnt[0]);
-        if (s_cnt[1]) atomicAdd(&stats->changed[parity][1], s_cnt[1]);
-    }
-}
+#define B200VIS_TILE_1B k_propagate_cull_tma
+#define B200VIS_TILE_1B_EXT false
+#include "tile_kernel_1b.cuh"
+#undef B200VIS_TILE_1B
+#undef B200VIS_TILE_1B_EXT
+// kernel 1b while GlobalTransforms written by other systems are pending (PROP+CULL and PROP-only instantiations only)
+#define B200VIS_TILE_1B k_propagate_cull_tma_ext
+#define B200VIS_TILE_1B_EXT true
+#include "tile_kernel_1b.cuh"
+#undef B200VIS_TILE_1B
+#undef B200VIS_TILE_1B_EXT
 
 // ------------------------------------------------------------------------------------------
 // Kernel 1L (B200VIS_TILE_KERNEL=lean; kernel 1b is the default): kernel 1b on an instruction and exposed-latency diet.
@@ -3701,6 +3417,21 @@ __global__ void k_unpack_gt(Rows R, uint32_t first, uint32_t count, const float 
     R.gt1[row] = make_float4(g[1], g[4], g[7], g[10]);
     R.gt2[row] = make_float4(g[2], g[5], g[8], g[11]);
 }
+// GlobalTransforms another system wrote (distinct rows): the column and the S_GT_EXT mark the next propagate pass consumes
+__global__ void k_write_gt_scattered(Rows R, uint32_t count, const uint32_t *__restrict__ rows, const float *__restrict__ src) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= count) return;
+    const float *g = src + (size_t)i * 12;   // X.xyz Y.xyz Z.xyz T.xyz
+    const uint32_t row = rows[i];
+    R.gt0[row] = make_float4(g[0], g[3], g[6], g[9]);
+    R.gt1[row] = make_float4(g[1], g[4], g[7], g[10]);
+    R.gt2[row] = make_float4(g[2], g[5], g[8], g[11]);
+    R.state[row] = (uint8_t)(R.state[row] | S_GT_EXT);
+}
+__global__ void k_clear_gt_ext(Rows R, uint32_t n) {
+    const uint32_t row = blockIdx.x * blockDim.x + threadIdx.x;
+    if (row < n && (R.state[row] & (S_GT_EXT | S_GT_HANDED))) R.state[row] = (uint8_t)(R.state[row] & ~(S_GT_EXT | S_GT_HANDED));
+}
 __global__ void k_pack_gt(Rows R, uint32_t first, uint32_t count, float *__restrict__ dst, uint32_t stride) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= count) return;
@@ -3936,19 +3667,20 @@ static void launch_scout_m(cudaStream_t st, const Rows &R, const Tile *tiles, ui
                 else launch_scout<true, false, MINB>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity); }
     else launch_scout<false, true, MINB>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity);
 }
-template <bool P, bool C, bool S, int KIND>      // KIND: 0 kernel 1b, 1 flow, 4 / 5 / 6 lean with that many CTAs per SM, 7 lean with drifting warps (PIPE)
+template <bool P, bool C, bool S, int KIND>      // KIND: 0 kernel 1b, 1 flow, 4 / 5 / 6 lean with that many CTAs per SM, 7 lean with drifting warps (PIPE), 8 kernel 1b with external GlobalTransform marks
 static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                        const VisibleBufs &vb, DevStats *stats, uint32_t static_opt, uint32_t parity, uint32_t *ticket, uint32_t *ticket_base) {
     static int grid = 0;
     static unsigned long long seen = 0;
     constexpr bool FLOW = KIND == 1;
-    constexpr size_t smem = (KIND == 4 || KIND == 7) ? sizeof(LeanSmem<true>) : KIND >= 5 ? sizeof(LeanSmem<false>) : sizeof(TmaSmem);
+    constexpr size_t smem = (KIND == 4 || KIND == 7) ? sizeof(LeanSmem<true>) : (KIND == 5 || KIND == 6) ? sizeof(LeanSmem<false>) : sizeof(TmaSmem);
     auto with_kernel = [&](auto &&fn) {
         if constexpr (KIND == 1) fn(k_propagate_cull_flow<P, C, S>);
         else if constexpr (KIND == 4) fn(k_propagate_cull_lean<P, C, S, 4>);
         else if constexpr (KIND == 5) fn(k_propagate_cull_lean<P, C, S, 5>);
         else if constexpr (KIND == 6) fn(k_propagate_cull_lean<P, C, S, 6>);
         else if constexpr (KIND == 7) fn(k_propagate_cull_lean<P, C, S, 4, P && C>);
+        else if constexpr (KIND == 8) fn(k_propagate_cull_tma_ext<P, C, S>);
         else fn(k_propagate_cull_tma<P, C, S>);
     };
     if (first_call_on_device(seen)) {
@@ -3992,7 +3724,7 @@ static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32
     if (!FLOW && dynamic && tiles_per_cta == 0 && ticket && ticket_base) { tk = ticket; base = *ticket_base; *ticket_base += n_tiles; }
     ++g_launches;
     with_kernel([&](auto kern) {
-        if constexpr (KIND >= 4) {
+        if constexpr (KIND >= 4 && KIND <= 7) {
             static int flip = -1;     // B200VIS_LEAN_WARP_FLIP=1 reverses the CTA's warp order
             if (flip < 0) { const char *e = getenv("B200VIS_LEAN_WARP_FLIP"); flip = (e && atoi(e) == 1) ? 0xE0 : 0; }
             static int probe = -1;    // B200VIS_LEAN_PROBE: timing probes, wrong results (tools/ only)
@@ -4047,6 +3779,16 @@ void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, ui
     else if (cull) { if (simple) B200VIS_LAUNCH(false, true, true); else B200VIS_LAUNCH(false, true, false); }
 #undef B200VIS_LAUNCH
 }
+void launch_propagate_cull_ext(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
+                               const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
+                               uint32_t *ticket, uint32_t *ticket_base) {
+    if (n_tiles == 0 || !(stages & 1u)) return;
+    const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
+    if (!(stages & 2u)) launch_tma<true, false, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
+    else if (simple) launch_tma<true, true, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
+    else launch_tma<true, true, false, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
+}
+bool tile_kernel_is_default() { return tile_kernel_choice() == 1; }
 void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity) {
     if (!R.n) return;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
@@ -4186,6 +3928,12 @@ void launch_scatter_trs(cudaStream_t st, const Rows &R, uint32_t count, const ui
 }
 void launch_unpack_gt(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, const float *src) {
     if (count) { ++g_launches; k_unpack_gt<<<cdiv(count, 256), 256, 0, st>>>(R, first, count, src); }
+}
+void launch_write_gt_scattered(cudaStream_t st, const Rows &R, uint32_t count, const uint32_t *rows, const float *src) {
+    if (count) { ++g_launches; k_write_gt_scattered<<<cdiv(count, 256), 256, 0, st>>>(R, count, rows, src); }
+}
+void launch_clear_gt_ext(cudaStream_t st, const Rows &R, uint32_t n) {
+    if (n) { ++g_launches; k_clear_gt_ext<<<cdiv(n, 256), 256, 0, st>>>(R, n); }
 }
 void launch_pack_gt(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, float *dst, uint32_t stride) {
     if (count) { ++g_launches; k_pack_gt<<<cdiv(count, 256), 256, 0, st>>>(R, first, count, dst, stride); }

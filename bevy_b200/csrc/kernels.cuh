@@ -10,6 +10,11 @@ void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, ui
 void launch_propagate_cull_small(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                                  const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity);
 unsigned long long kernel_launch_count();
+// kernel 1b's instantiation for frames with pending external GlobalTransform marks (S_GT_EXT); stages must include PROPAGATE
+void launch_propagate_cull_ext(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
+                               const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
+                               uint32_t *ticket, uint32_t *ticket_base);
+bool tile_kernel_is_default();   // B200VIS_TILE_KERNEL selects kernel 1b (unset, or tma)
 bool tile_kernel_is_tma();
 bool tile_kernel_is_warp();
 bool tile_kernel_publishes_light_snapshot();
@@ -43,6 +48,8 @@ void launch_cluster_lists(cudaStream_t st, const FrameConsts *fc, const ClusterB
 void launch_unpack_trs(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, const float *src, int mark_only);
 void launch_scatter_trs(cudaStream_t st, const Rows &R, uint32_t count, const uint32_t *rows, const float *src);
 void launch_unpack_gt(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, const float *src);
+void launch_write_gt_scattered(cudaStream_t st, const Rows &R, uint32_t count, const uint32_t *rows, const float *src);
+void launch_clear_gt_ext(cudaStream_t st, const Rows &R, uint32_t n);
 void launch_pack_gt(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, float *dst, uint32_t stride);
 void launch_unpack_bounds(cudaStream_t st, const Rows &R, uint32_t first, uint32_t count, const float *bounds,
                           const uint8_t *flags, const uint8_t *cls, uint8_t *cls_col);

@@ -281,9 +281,24 @@ B200VIS_API int32_t b200vis_upload_transforms_scattered(b200vis_ctx *ctx, uint32
 /* Rows that are Changed<ChildOf> | Added<GlobalTransform> | freshly orphaned without new Transform data
  * (mark_dirty_trees' input set, systems.rs:112-113). */
 B200VIS_API int32_t b200vis_mark_transforms_changed(b200vis_ctx *ctx, uint32_t first_row, uint32_t count);
-/* GlobalTransform column as it stands on the host (initial mirror / external writes):
- * gt[count][12] = Affine3A x_axis.xyz, y_axis.xyz, z_axis.xyz, translation.xyz */
+/* GlobalTransform column as it stands on the host (the initial mirror, spawn time):
+ * gt[count][12] = Affine3A x_axis.xyz, y_axis.xyz, z_axis.xyz, translation.xyz.  Sets no Changed flag; GlobalTransforms
+ * that other systems write between frames go through b200vis_write_global_transforms_scattered. */
 B200VIS_API int32_t b200vis_upload_global_transforms(b200vis_ctx *ctx, uint32_t first_row, uint32_t count, const float *gt);
+/* GlobalTransforms that another system wrote since the last run that included PROPAGATE
+ * (Changed<GlobalTransform> as the propagate system sees it, systems.rs:709-710): sets the column
+ * (gt[count][12] as in b200vis_upload_global_transforms) and marks p_global_transform.is_changed()
+ * for the next run that includes PROPAGATE, which consumes the marks.
+ * That run re-propagates the children of every marked row it visits, even when the row's recomputed value equals the
+ * written one; a marked row it does not visit keeps the written value.  A mark does not dirty the row's ancestors, and
+ * the row's own Changed<GlobalTransform> output is unaffected (the writer stamped its own tick).  A run without
+ * PROPAGATE keeps the marks and culls at the written values.  A row listed twice takes its last value.
+ * Marks are per row: b200vis_edit_topology drops a despawned row's mark, b200vis_compact_topology carries them through
+ * old_to_new, b200vis_set_topology clears them.  A run that includes PROPAGATE while marks are pending returns
+ * UNSUPPORTED, consuming nothing, when B200VIS_TILE_KERNEL selects an experiment tile kernel.
+ * Errors: NOT_READY (no b200vis_set_topology yet), INVALID_ARG (a null array, a row out of range or despawned). */
+B200VIS_API int32_t b200vis_write_global_transforms_scattered(b200vis_ctx *ctx, uint32_t count,
+                                                              const uint32_t *rows, const float *gt);
 /* Aabb / Sphere / flags / VisibilityClass / RenderLayers / VisibleEntityRanges columns:
  * bounds[count][6] = center.xyz, half_extents.xyz (Aabb) or center.xyz, radius,0,0 (Sphere);
  * class_mask: one bit per VisibilityClass the entity is in (0 => set_visible() but no list entry,

@@ -61,6 +61,7 @@ extern "C" {
     fn b200vis_upload_transforms(ctx: *mut b200vis_ctx, first: u32, count: u32, trs: *const f32) -> i32;
     fn b200vis_upload_transforms_scattered(ctx: *mut b200vis_ctx, count: u32, rows: *const u32, trs: *const f32) -> i32;
     fn b200vis_upload_global_transforms(ctx: *mut b200vis_ctx, first: u32, count: u32, gt: *const f32) -> i32;
+    fn b200vis_write_global_transforms_scattered(ctx: *mut b200vis_ctx, count: u32, rows: *const u32, gt: *const f32) -> i32;
     fn b200vis_upload_bounds(ctx: *mut b200vis_ctx, first: u32, count: u32, bounds: *const f32, flags: *const u8, class_mask: *const u8,
                              layer_mask: *const u64, range_mask: *const u32) -> i32;
     fn b200vis_upload_view_visibility(ctx: *mut b200vis_ctx, first: u32, count: u32, vv: *const u8) -> i32;
@@ -247,6 +248,21 @@ fn b200_propagate(
         }
         if !rows.is_empty() {
             vis.check(unsafe { b200vis_upload_transforms_scattered(vis.ctx, rows.len() as u32, rows.as_ptr(), trs.as_ptr()) })?;
+        }
+        // Changed<GlobalTransform> as this system sees it (systems.rs:709-710): exactly the writes of other systems, because
+        // this system's own write-back of its last run is not newer than its last_run.  Read through `q` (is_changed() on
+        // the `Mut` does not stamp a tick): a second query on GlobalTransform would conflict with q's mutable access.
+        let (mut grows, mut gts) = (Vec::new(), Vec::new());
+        for (e, _, g, _, _) in q.iter_mut() {
+            if g.is_changed() { grows.push(vis.row_of[&e]); pack_gt12(&g, &mut gts); }
+        }
+        if !grows.is_empty() {
+            vis.check(unsafe { b200vis_write_global_transforms_scattered(vis.ctx, grows.len() as u32, grows.as_ptr(), gts.as_ptr()) })?;
+            for (&r, g) in grows.iter().zip(gts.chunks(12)) {      // the host mirror holds what the other system wrote
+                let mut m = [0.0; 16];
+                m[0..3].copy_from_slice(&g[0..3]); m[4..7].copy_from_slice(&g[3..6]); m[8..11].copy_from_slice(&g[6..9]); m[12..15].copy_from_slice(&g[9..12]);
+                vis.gt_col[r as usize] = m;
+            }
         }
     }
     unsafe {
