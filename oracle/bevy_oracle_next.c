@@ -87,16 +87,19 @@ static uint32_t pack_offset_and_counts(size_t offset, uint32_t point_count, uint
            ((point_count & CLUSTER_COUNT_MASK) << CLUSTER_COUNT_SIZE) | (spot_count & CLUSTER_COUNT_MASK);
 }
 /* Input: one view's Clusters in CSR form (cluster c holds light ordinals indices[offsets[c] .. offsets[c+1])), in
- * the reference's push order), gpu_index_of_light = GlobalClusterableObjectMeta::entity_to_index for each ordinal
- * (NULL = identity).  The record stream of extract_clusters_for_cpu_clustering (:419-470) is
- * ClusterHeader(counts), Light(e)...; prepare_clusters_for_cpu_clustering (:494-520) consumes it.
+ * the reference's push order), gpu_index_of_light = GlobalClusterableObjectMeta::entity_to_index for the ordinals
+ * 0 .. n_map-1 (NULL = identity); an ordinal with no entry gets push_dummy_index's !0 (:527-533).  The record
+ * stream of extract_clusters_for_cpu_clustering (:419-470) is ClusterHeader(counts), Light(e)...;
+ * prepare_clusters_for_cpu_clustering (:494-520) consumes it.
  * storage != 0: offsets_and_counts[n][8] = (offset, point, spot, rect | probes, volumes, decals, 0) (:636-652),
  *               index_lists[n_indices] (:688-693)
  * storage == 0: offsets_and_counts[4096] packed (:622-634), index_lists[4096] = 16384 u8 slots OR-ed in (:676-686);
  *               both zeroed first (clear(), :598-606); the record loop BREAKS at the first Light seen with
- *               n_indices >= MAX_INDICES (:505-514), leaving every later cluster header unwritten. */
+ *               n_indices >= MAX_INDICES (:505-514), leaving every later cluster header unwritten.  The
+ *               dummy push skips that check; past MAX_INDICES its slot lies outside the uniform array, where
+ *               the reference's indexing panics: the oracle stops the loop there too. */
 ORC_API void orc_cluster_bindings(uint32_t n_clusters, const uint32_t *offsets, const uint32_t *indices,
-                                  const uint32_t *gpu_index_of_light, int storage, uint32_t *offsets_and_counts,
+                                  const uint32_t *gpu_index_of_light, uint32_t n_map, int storage, uint32_t *offsets_and_counts,
                                   uint32_t *index_lists, uint32_t *n_offsets_out, uint32_t *n_indices_out) {
     size_t n_indices = 0, n_offsets = 0;
     if (!storage) {
@@ -119,7 +122,8 @@ ORC_API void orc_cluster_bindings(uint32_t n_clusters, const uint32_t *offsets, 
         /* Light records */
         for (uint32_t k = offsets[c]; k < offsets[c + 1]; ++k) {
             if (n_indices >= VCB_MAX_INDICES && !storage) { stop = 1; break; }
-            const uint32_t index = gpu_index_of_light ? gpu_index_of_light[indices[k]] : indices[k];
+            const uint32_t index = !gpu_index_of_light ? indices[k]
+                                   : indices[k] < n_map ? gpu_index_of_light[indices[k]] : 0xFFFFFFFFu;
             if (storage) index_lists[n_indices] = index;
             else {
                 const size_t array_index = n_indices >> 4, component = (n_indices >> 2) & 3, sub_index = n_indices & 3;

@@ -149,7 +149,7 @@ def _declare(l):
                                                      U64P, U64P, U32P, U64P, U64P, U32P]
         l.orc_entity_pair_is_visible.restype = C.c_int
         l.orc_entity_pair_is_visible.argtypes = [U64P, U64P, C.c_uint32, C.c_uint64, C.c_uint64]
-        l.orc_cluster_bindings.argtypes = [C.c_uint32, U32P, U32P, U32P, C.c_int, U32P, U32P, U32P, U32P]
+        l.orc_cluster_bindings.argtypes = [C.c_uint32, U32P, U32P, U32P, C.c_uint32, C.c_int, U32P, U32P, U32P, U32P]
         l.orc_check_visibility_ranges.argtypes = [C.c_uint32, C.POINTER(C.c_float), C.POINTER(C.c_float), U8P,
                                                   C.POINTER(C.c_float), U8P, C.c_uint32, C.POINTER(C.c_float), U32P]
         l.orc_visibility_propagate.restype = C.c_int
@@ -432,7 +432,8 @@ def entity_pair_is_visible(render, main, entity, main_entity):
 
 
 def cluster_bindings(offsets, indices, gpu_index_of_light=None, storage=True):
-    """Clusters (CSR) -> ViewClusterBindings buffers: (offsets_and_counts, index_lists, n_offsets, n_indices)."""
+    """Clusters (CSR) -> ViewClusterBindings buffers: (offsets_and_counts, index_lists, n_offsets, n_indices).
+    `gpu_index_of_light[o]` is light ordinal o's entity_to_index; an ordinal past its end gets the dummy index !0."""
     offsets = np.ascontiguousarray(offsets, np.uint32)
     indices = np.ascontiguousarray(indices, np.uint32)
     n = len(offsets) - 1
@@ -445,7 +446,8 @@ def cluster_bindings(offsets, indices, gpu_index_of_light=None, storage=True):
     gi = None if gpu_index_of_light is None else np.ascontiguousarray(gpu_index_of_light, np.uint32)
     no, ni = C.c_uint32(0), C.c_uint32(0)
     U = C.c_uint32
-    lib().orc_cluster_bindings(n, _p(offsets, U), _p(indices, U), None if gi is None else _p(gi, U), int(bool(storage)),
+    lib().orc_cluster_bindings(n, _p(offsets, U), _p(indices, U), None if gi is None else _p(gi, U),
+                               0 if gi is None else len(gi), int(bool(storage)),
                                _p(oc, U), _p(il, U), C.byref(no), C.byref(ni))
     if storage:
         il = il[:ni.value]

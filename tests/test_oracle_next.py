@@ -84,6 +84,114 @@ def test_n2_uniform_layout_and_overflow(mean):
     assert np.array_equal(il, packed.view("<u4"))
 
 
+def view_cluster_bindings_literal(offsets, indices, entity_to_index, storage):
+    """prepare_clusters_for_cpu_clustering (bevy_pbr/src/cluster/mod.rs:494-534) over the record stream of
+    extract_clusters_for_cpu_clustering (:419-470), one record at a time into ViewClusterBindings (:596-705).
+    `entity_to_index` maps a light ordinal to its GPU index; an ordinal missing from it takes the dummy path."""
+    MAX_INDICES, MAX_UNIFORM_ITEMS = 16384, 16384 // 4 // 4
+    records = []
+    for c in range(len(offsets) - 1):
+        records.append(("header", int(offsets[c + 1] - offsets[c])))
+        records += [("light", int(e)) for e in indices[offsets[c]:offsets[c + 1]]]
+    st = dict(n_offsets=0, n_indices=0)
+    if storage:
+        oc, il = [], []
+    else:
+        oc = [[0] * 4 for _ in range(MAX_UNIFORM_ITEMS)]        # clear()
+        il = [[0] * 4 for _ in range(MAX_UNIFORM_ITEMS)]
+
+    def push_offset_and_counts(offset, point_lights):
+        if storage:
+            oc.append([offset, point_lights, 0, 0, 0, 0, 0, 0])
+        else:
+            array_index = st["n_offsets"] >> 2
+            if array_index < MAX_UNIFORM_ITEMS:
+                oc[array_index][st["n_offsets"] & 3] = ((offset & 0x3FFF) << 18) | ((point_lights & 0x1FF) << 9) | (0 & 0x1FF)
+        st["n_offsets"] += 1
+
+    def push_raw_index(index):
+        n = st["n_indices"]
+        if storage:
+            il.append(index)
+        else:
+            il[n >> 4][(n >> 2) & 3] |= (index << (8 * (n & 3))) & 0xFFFFFFFF   # u32 shift: the high bits fall off
+        st["n_indices"] += 1
+
+    for kind, value in records:
+        if kind == "header":
+            push_offset_and_counts(st["n_indices"], value)
+            continue
+        index = entity_to_index.get(value)
+        if index is None:
+            if not storage and st["n_indices"] >= MAX_INDICES:
+                break                     # data[array_index] past the array: the reference panics here
+            push_raw_index(0xFFFFFFFF)    # push_dummy_index
+            continue
+        if st["n_indices"] >= MAX_INDICES and not storage:
+            break
+        push_raw_index(index)
+    if storage:
+        return np.array(oc, np.uint32).reshape(-1, 8), np.array(il, np.uint32), st["n_offsets"], st["n_indices"]
+    return np.array(oc, np.uint32).reshape(-1), np.array(il, np.uint32).reshape(-1), st["n_offsets"], st["n_indices"]
+
+
+def binding_csr(case):
+    """Hand-built CSRs (offsets, indices, cluster count) for the packing limits."""
+    rng = np.random.default_rng(len(case))
+    if case.startswith("total_"):                  # 16383 / 16384 / 16385 indices, the last cluster closing the stream
+        total = int(case[6:])
+        counts = np.full(total // 7, 7); counts = np.concatenate([counts, [total - counts.sum()]])
+        counts = np.insert(counts, rng.integers(0, len(counts), 40), 0)
+    elif case == "break_then_empty":               # the 16384th index closes a cluster; then empty clusters, then lights
+        counts = np.concatenate([np.full(16384 // 8, 8), [0, 0, 0, 5, 0, 3]])
+    elif case == "break_mid_cluster":              # index 16384 falls inside a cluster
+        counts = np.concatenate([np.full(2047, 8), [12, 0, 4]])
+    elif case == "counts_511_512_600":             # the 9-bit count field: 511 fits, 512 wraps to 0, 600 to 88
+        counts = np.array([3, 511, 0, 512, 1, 600, 2])
+    else:
+        raise KeyError(case)
+    counts = counts.astype(np.int64)
+    offsets = np.concatenate([[0], np.cumsum(counts)]).astype(np.uint32)
+    indices = rng.integers(0, 700, int(offsets[-1])).astype(np.uint32)   # ordinals up to 699: past 255 and past a short map
+    return offsets, indices
+
+
+BINDING_CASES = ["total_16383", "total_16384", "total_16385", "break_then_empty", "break_mid_cluster", "counts_511_512_600"]
+
+
+@pytest.mark.parametrize("storage", [True, False])
+@pytest.mark.parametrize("mapping", ["identity", "full", "short"])
+@pytest.mark.parametrize("case", BINDING_CASES)
+def test_n2_bindings_at_the_packing_limits_equal_the_record_loop(case, mapping, storage):
+    offsets, indices = binding_csr(case)
+    rng = np.random.default_rng(7)
+    if mapping == "identity":
+        gmap, e2i = None, {o: o for o in range(700)}
+    else:
+        n_map = 700 if mapping == "full" else 300
+        gmap = rng.permutation(1000)[:n_map].astype(np.uint32)      # GPU indices up to 999: more than 8 bits
+        e2i = {o: int(gmap[o]) for o in range(n_map)}
+    got = orc.cluster_bindings(offsets, indices, gmap, storage=storage)
+    want = view_cluster_bindings_literal(offsets, indices, e2i, storage)
+    assert got[2:] == want[2:], f"n_offsets / n_indices {got[2:]} vs {want[2:]}"
+    assert np.array_equal(got[0], want[0]) and np.array_equal(got[1], want[1])
+    total, counts = int(offsets[-1]), np.diff(offsets)
+    # each case reaches the limit it is named for
+    if not storage:
+        assert want[3] == min(total, 16384)
+        assert want[2] == np.count_nonzero(offsets[:-1] <= 16384)
+    if case.startswith("total_"):
+        assert total == int(case[6:])
+    if case == "break_then_empty":
+        assert (offsets[:-1] == 16384).sum() == 4 and counts[offsets[:-1] == 16384].tolist() == [0, 0, 0, 5]
+    if case == "counts_511_512_600" and not storage:
+        assert [(w >> 9) & 0x1FF for w in want[0][[1, 3, 5]]] == [511, 0, 88]
+    if mapping != "identity" and storage:
+        assert (want[1] > 255).any()
+    if mapping == "short" and storage:
+        assert (want[1] == 0xFFFFFFFF).any()
+
+
 # ---- N4a --------------------------------------------------------------------------------------------
 def test_n4_visibility_ranges_against_numpy():
     rng = np.random.default_rng(3)
