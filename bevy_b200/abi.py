@@ -14,7 +14,8 @@ VIEW_ACTIVE, VIEW_NO_CPU_CULLING = 0x01, 0x02
 STAGE_PROPAGATE, STAGE_CULL, STAGE_CLUSTER_ASSIGN, STAGE_CLUSTER_LISTS = 0x1, 0x2, 0x4, 0x8
 STAGE_CLUSTER = STAGE_CLUSTER_ASSIGN | STAGE_CLUSTER_LISTS
 STAGE_ALL = 0xF
-MAX_VIEWS = 8
+MAX_VIEWS = 8          # views FrameStats reports (and views per rank with world_size > 1)
+MAX_CAMERAS = 32       # views one context may hold
 MAX_CLUSTERS = 4096
 
 ERR_NAMES = {1: "INVALID_ARG", 2: "CUDA", 3: "OUT_OF_MEMORY", 4: "HIERARCHY_CYCLE", 5: "PARENT_OUT_OF_RANGE",
@@ -153,6 +154,8 @@ _SIGNATURES = {
     "b200vis_step": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, C.c_uint32, _P(CameraDesc), _P(ClusterConfig), C.c_uint32]),
     "b200vis_run": (C.c_int32, [_vp, C.c_uint32]),
     "b200vis_download_frame_stats": (C.c_int32, [_vp, _P(FrameStats)]),
+    "b200vis_download_view_stats": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp]),
+    "b200vis_set_view_stats_sink": (C.c_int32, [_vp, _vp]),
     "b200vis_download_global_transforms": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, C.c_uint32, _vp]),
     "b200vis_download_view_visibility": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "b200vis_download_visible": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
@@ -578,6 +581,25 @@ class Context:
         s = FrameStats()
         self._check(self._lib.b200vis_download_frame_stats(self._h, C.byref(s)))
         return s
+
+    def download_view_stats(self, first_view=0, count=None):
+        """Per-view statistics of views [first_view, first_view + count) (default: every view of the context):
+        dict of visible_count, cluster_index_count, cluster_farthest_z, cluster_index_overflow arrays."""
+        count = self.max_views - first_view if count is None else count
+        out = {"visible_count": np.zeros(count, np.uint32), "cluster_index_count": np.zeros(count, np.uint32),
+               "cluster_farthest_z": np.zeros(count, np.float32), "cluster_index_overflow": np.zeros(count, np.uint32)}
+        self._check(self._lib.b200vis_download_view_stats(self._h, first_view, count, _ptr(out["visible_count"]),
+                                                          _ptr(out["cluster_index_count"]), _ptr(out["cluster_farthest_z"]),
+                                                          _ptr(out["cluster_index_overflow"])))
+        return out
+
+    def set_view_stats_sink(self, per_view):
+        """Pinned host uint32 array [max_views, 4] (visible_count, cluster_index_count, cluster_farthest_z bits, overflow)
+        that the result sink's stats publish fills; None removes it."""
+        if per_view is not None:
+            assert per_view.dtype == np.uint32 and per_view.size >= self.max_views * 4 and per_view.flags.c_contiguous
+        self._view_stats_sink = per_view
+        self._check(self._lib.b200vis_set_view_stats_sink(self._h, None if per_view is None else per_view.ctypes.data))
 
     def download_global_transforms(self, first_row, count, stride=12, want_changed=True):
         gt = np.zeros((count, stride), np.float32)

@@ -83,7 +83,7 @@ struct b200vis_ctx {
 
     uint32_t n = 0;                 // current row count
     Rows rows{};                    // device SoA (capacity cfg.max_entities)
-    uint64_t *d_layers_ext = nullptr; bool have_layers_ext = false; uint64_t view_layers_ext[kMaxViews][3] = {};   // RenderLayers blocks 1..3
+    uint64_t *d_layers_ext = nullptr; bool have_layers_ext = false; uint64_t view_layers_ext[kMaxCameras][3] = {};   // RenderLayers blocks 1..3
     uint32_t *d_parent = nullptr; uint64_t *d_layers = nullptr; uint32_t *d_range = nullptr;
     uint32_t *d_rank = nullptr, *d_row_of_rank = nullptr; uint8_t *d_dirty = nullptr;
     bool have_layers = false, have_range = false, rank_identity = true, topology_set = false;
@@ -114,7 +114,7 @@ struct b200vis_ctx {
     // Setters edit the host working copy; run() packs it into the next pinned ring slot and issues
     // ONE async H2D copy, so per-frame constant updates never block on the stream.
     FrameConsts consts{};               // host working copy
-    std::vector<float> tab_x[kMaxViews], tab_y[kMaxViews], tab_z[kMaxViews], tab_thr[kMaxViews];
+    std::vector<float> tab_x[kMaxCameras], tab_y[kMaxCameras], tab_z[kMaxCameras], tab_thr[kMaxCameras];
     static constexpr int kRing = 4;
     uint8_t *h_ring[kRing] = {nullptr, nullptr, nullptr, nullptr};   // pinned
     cudaEvent_t ring_ev[kRing] = {nullptr, nullptr, nullptr, nullptr};
@@ -159,6 +159,7 @@ struct b200vis_ctx {
     b200vis_result_sink sink{}; bool have_sink = false;
     uint32_t *sink_rows_d = nullptr, *sink_off_d = nullptr, *sink_idx_d = nullptr, *sink_stats_d = nullptr;
     uint8_t *sink_cls_d = nullptr; uint8_t *d_cls = nullptr;   // VisibilityClass masks: sink alias, per-row column
+    uint32_t *view_stats_sink = nullptr, *view_stats_d = nullptr;   // b200vis_set_view_stats_sink: [max_views][4], host and device alias
 
     b200vis_column_sinks colsink{}; bool have_colsink = false;          // b200vis_set_column_sinks (device aliases below)
     float *col_gt_d = nullptr; uint32_t *col_gt_bits_d = nullptr, *col_vv_bits_d = nullptr; uint8_t *col_vv_d = nullptr;
@@ -173,7 +174,7 @@ struct b200vis_ctx {
     // peer-memory exchange (b200vis_p2p_export / _import): [2][world][slab] + flags [2][world], mapped into every rank
     uint32_t *d_xbuf = nullptr; size_t xbuf_flag_offset = 0; void *peer_map[8] = {}; bool peer_ipc[8] = {}; bool p2p_ready = false;
     uint32_t *d_push_done = nullptr;
-    b200vis_cluster_feedback auto_fb[kMaxViews]{};   // b200vis_step: last frame's Clusters feedback
+    b200vis_cluster_feedback auto_fb[kMaxCameras]{};   // b200vis_step: last frame's Clusters feedback
 
     // staging for AoS <-> SoA conversion
     uint8_t *d_stage = nullptr; size_t stage_bytes = 0;
@@ -266,8 +267,11 @@ extern "C" int32_t b200vis_create(const b200vis_config *cfg, b200vis_ctx **out) 
     b200vis_ctx *ctx = nullptr;   // for CU(): errors before allocation go to the thread-local slot
     if (!cfg || !out) return fail(nullptr, B200VIS_ERR_INVALID_ARG, "b200vis_create: null argument");
     *out = nullptr;
-    if (cfg->max_views == 0 || cfg->max_views > B200VIS_MAX_VIEWS)
-        return fail(nullptr, B200VIS_ERR_INVALID_ARG, "max_views must be in 1..%u", B200VIS_MAX_VIEWS);
+    if (cfg->max_views == 0 || cfg->max_views > B200VIS_MAX_CAMERAS)
+        return fail(nullptr, B200VIS_ERR_INVALID_ARG, "max_views must be in 1..%u", B200VIS_MAX_CAMERAS);
+    // the cluster exchange (slab trailer, light records) and its tests cover eight views per rank
+    if (cfg->world_size > 1 && cfg->max_views > B200VIS_MAX_VIEWS)
+        return fail(nullptr, B200VIS_ERR_INVALID_ARG, "max_views > %u needs world_size 1", B200VIS_MAX_VIEWS);
     int ndev = 0;
     cudaError_t e = cudaGetDeviceCount(&ndev);
     if (e != cudaSuccess || ndev == 0)
@@ -329,7 +333,7 @@ extern "C" int32_t b200vis_create(const b200vis_config *cfg, b200vis_ctx **out) 
         vb.chunks_stride = (vb.words_stride + kChunkWords - 1) / kChunkWords + 1;
         vb.list_stride = (uint32_t)std::max<size_t>(N, 1);
         CU(dalloc(&vb.mask, (size_t)2 * vb.words_stride * V));
-        CU(dalloc(&vb.chunk_count, (size_t)3 * kMaxViews * vb.chunks_stride));
+        CU(dalloc(&vb.chunk_count, (size_t)3 * kMaxCameras * vb.chunks_stride));
         CU(dalloc(&vb.lists, (size_t)vb.list_stride * V));
         CU(dalloc(&vb.classes, (size_t)vb.list_stride * V));
         CU(dalloc(&ctx->d_cls, NP));
@@ -348,7 +352,8 @@ extern "C" int32_t b200vis_create(const b200vis_config *cfg, b200vis_ctx **out) 
         ctx->lrec_bytes = (size_t)cl.max_lights * 28;
         CU(cudaMalloc(&ctx->d_lrec, 3 * ctx->lrec_bytes)); CU(cudaMemset(ctx->d_lrec, 0, 3 * ctx->lrec_bytes));
         if (cl.world > 1) { CU(cudaMalloc(&ctx->d_lrec_all, cl.world * ctx->lrec_bytes)); CU(cudaMemset(ctx->d_lrec_all, 0, cl.world * ctx->lrec_bytes)); }
-        cl.slab_words = (uint32_t)(V * cl.words * kMaxClusters + kMaxViews);   // bit matrix + per-view farthest_z trailer
+        cl.trailer = (uint32_t)std::max<size_t>(V, kMaxViews);
+        cl.slab_words = (uint32_t)(V * cl.words * kMaxClusters + cl.trailer);   // bit matrix + per-view farthest_z trailer
         ctx->slab_bytes = (size_t)cl.slab_words * sizeof(uint32_t);
         CU(dalloc(&ctx->d_slab, ctx->slab_bytes / 4));
         cl.send = ctx->d_slab; cl.recv = ctx->d_slab;
@@ -981,7 +986,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
     ctx->vis.n_chunks = (ctx->vis.n_words + kChunkWords - 1) / kChunkWords;
     // fresh accumulation state
     CU(cudaMemset(ctx->vis.mask, 0, (size_t)2 * ctx->vis.words_stride * ctx->cfg.max_views * 4));
-    CU(cudaMemset(ctx->vis.chunk_count, 0, (size_t)3 * kMaxViews * ctx->vis.chunks_stride * 4));
+    CU(cudaMemset(ctx->vis.chunk_count, 0, (size_t)3 * kMaxCameras * ctx->vis.chunks_stride * 4));
     CU(cudaMemset(ctx->d_stats, 0, sizeof(DevStats)));
     CU(cudaMemset(ctx->d_slab, 0, ctx->slab_bytes));
     if (ctx->diff.prev) CU(cudaMemset(ctx->diff.prev, 0, (size_t)ctx->vis.words_stride * ctx->cfg.max_views * 4));   // ranks changed: old list = empty
@@ -1401,7 +1406,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
         const VisibleBufs &vb = ctx->vis;
         if (vb.words_stride > nw2) CU(cudaMemset2DAsync(vb.mask + nw2, (size_t)vb.words_stride * 4, 0, (size_t)(vb.words_stride - nw2) * 4, 2 * V, st));
         if (vb.chunks_stride > nc2) {
-            CU(cudaMemset2DAsync(vb.chunk_count + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4, 3 * kMaxViews, st));
+            CU(cudaMemset2DAsync(vb.chunk_count + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4, 3 * kMaxCameras, st));
             if (ctx->diff.chunk) CU(cudaMemset2DAsync(ctx->diff.chunk + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4, V, st));
             if (ctx->shadow.chunk_count)
                 CU(cudaMemset2DAsync(ctx->shadow.chunk_count + nc2, (size_t)vb.chunks_stride * 4, 0, (size_t)(vb.chunks_stride - nc2) * 4,
@@ -1737,7 +1742,7 @@ extern "C" int32_t b200vis_upload_render_layers_ext(b200vis_ctx *ctx, uint32_t f
     return B200VIS_OK;
 }
 extern "C" int32_t b200vis_set_view_render_layers_ext(b200vis_ctx *ctx, uint32_t view, const uint64_t blocks[3]) {
-    if (!ctx || view >= (uint32_t)kMaxViews) return B200VIS_ERR_INVALID_ARG;
+    if (!ctx || view >= std::max<uint32_t>(ctx->cfg.max_views, kMaxViews)) return B200VIS_ERR_INVALID_ARG;   // views 0..7 always
     for (int k = 0; k < 3; ++k) ctx->view_layers_ext[view][k] = blocks ? blocks[k] : 0ull;
     return B200VIS_OK;
 }
@@ -1916,13 +1921,16 @@ extern "C" int32_t b200vis_use_recorded_frame_constants(b200vis_ctx *ctx, int32_
 static const FrameConsts &active_consts(const b200vis_ctx *ctx) {
     return ctx->replay_slot >= 0 ? ctx->recorded[ctx->replay_slot].host : ctx->consts;
 }
-static CullViews make_cull_views(const FrameConsts &fc) {
+// The cull pass's view table for views base .. base + 7 (group base / 8).  n_views counts the group's own views only: the
+// kernels index on[] / planes[] by it (k_cull's lane-per-view store reads cvw.on[lane] for lane < n_views).
+static CullViews make_cull_views(const FrameConsts &fc, uint32_t base = 0) {
     CullViews c;
     memset(&c, 0, sizeof c);
-    c.n_views = fc.n_views;
-    for (uint32_t v = 0; v < fc.n_views && v < (uint32_t)kMaxViews; ++v) {
-        c.on[v] = (fc.views[v].flags & 3u) | ((fc.views[v].layer_mask & 1ull) ? 4u : 0u); c.range_index[v] = fc.views[v].range_index; c.layers[v] = fc.views[v].layer_mask;
-        for (int k = 0; k < 5; ++k) c.planes[v][k] = fc.views[v].hs[k];
+    c.n_views = std::min<uint32_t>(kMaxViews, fc.n_views - base);
+    for (uint32_t i = 0; base + i < fc.n_views && i < (uint32_t)kMaxViews; ++i) {
+        const DevView &d = fc.views[base + i];
+        c.on[i] = (d.flags & 3u) | ((d.layer_mask & 1ull) ? 4u : 0u); c.range_index[i] = d.range_index; c.layers[i] = d.layer_mask;
+        for (int k = 0; k < 5; ++k) c.planes[i][k] = d.hs[k];
     }
     return c;
 }
@@ -2130,7 +2138,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
         launch_cluster_lists(tail, ctx->open_fc, cl, ctx->d_stats, ctx->cfg.max_views);
         if (ctx->have_sink)
             launch_publish_clusters(tail, ctx->open_fc, cl, ctx->sink_off_d, ctx->sink_idx_d, ctx->sink.cluster_capacity, ctx->d_stats,
-                                    ctx->sink_stats_d, ctx->open_frame % 3u, ctx->open_frame + 1u, ctx->cfg.max_views);
+                                    ctx->sink_stats_d, ctx->open_frame % 3u, ctx->open_frame + 1u, ctx->cfg.max_views,
+                                    ctx->view_stats_d);
         CU(cudaEventRecord(ctx->ev_side[ctx->open_frame % 3u], tail));
         ctx->side_pending = true; ctx->tail_open = false;
         CU(cudaGetLastError());
@@ -2168,7 +2177,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
         fc = ctx->d_consts;
     }
     cl.blob = reinterpret_cast<const float *>(fc);
-    CullViews cvw = make_cull_views(active_consts(ctx));
+    const FrameConsts &afc = active_consts(ctx);
+    CullViews cvw = make_cull_views(afc);
     Rows R = ctx->rows;
     R.layers = ctx->have_layers ? ctx->d_layers : nullptr;
     R.layers_ext = ctx->have_layers_ext ? ctx->d_layers_ext : nullptr;
@@ -2181,6 +2191,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     VisibleBufs vb = ctx->vis;
     vb.mask = ctx->vis.mask + (size_t)mslot * ctx->vis.words_stride * ctx->cfg.max_views;
     const uint32_t n_pass = ctx->pass_begin.empty() ? 0 : (uint32_t)ctx->pass_begin.size() - 1;
+    // views past the eighth: group passes of k_cull behind the frame's last tile pass (see launch_cull_group)
+    const bool view_groups = do_cull && n_pass && afc.n_views > (uint32_t)kMaxViews;
     R.dirty = nullptr;
     R.light_snap = nullptr; R.light_ord = nullptr; R.n_lights = 0;
     if (do_prop && ctx->static_opt && n_pass > 1) {
@@ -2205,6 +2217,7 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
         bool any_small = false;
         for (uint32_t x : ctx->pass_small) any_small |= x != 0;
         tile_snap = ctx->lights_tagged && tile_kernel_publishes_light_snapshot() && !any_small;   // the 32-thread kernel does not publish snapshots
+        tile_snap = tile_snap && !view_groups;   // a light only a view >= 8 sees is visible after the group passes only
         if (tile_snap) {
             R.light_snap = ctx->light_snap_slot(cslot);
             R.light_ord = ctx->d_light_ord; R.n_lights = ctx->lights.n;
@@ -2235,6 +2248,11 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
             }
         } else if (n_pass) {
             launch_cull(st, R, cvw, vb, ctx->d_stats, cslot);
+        }
+        for (uint32_t b = kMaxViews; view_groups && b < afc.n_views; b += kMaxViews) {
+            CullViews g = make_cull_views(afc, b);
+            if (ctx->have_layers_ext) memcpy(g.layers_ext, ctx->view_layers_ext[b], sizeof g.layers_ext);
+            launch_cull_group(st, R, g, vb, ctx->d_stats, cslot, b);
         }
     }
     Lights lights = ctx->lights;
@@ -2354,7 +2372,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     // (b200vis_step with clusters runs CLUSTER right behind PROPAGATE|CULL: that run publishes the stats block once for both)
     if (ctx->have_sink && (do_cull || (stages & B200VIS_STAGE_CLUSTER_LISTS)) && !(ctx->step_defers_stats && !(stages & B200VIS_STAGE_CLUSTER_LISTS)))
         launch_publish_clusters(tail, fc, cl, (stages & B200VIS_STAGE_CLUSTER_LISTS) ? ctx->sink_off_d : nullptr, ctx->sink_idx_d,
-                                ctx->sink.cluster_capacity, ctx->d_stats, ctx->sink_stats_d, do_cull ? cslot : (frame + 2u) % 3u, frame + (do_cull ? 1u : 0u), ctx->cfg.max_views);
+                                ctx->sink.cluster_capacity, ctx->d_stats, ctx->sink_stats_d, do_cull ? cslot : (frame + 2u) % 3u, frame + (do_cull ? 1u : 0u), ctx->cfg.max_views,
+                                ctx->view_stats_d);
     if (pe) CU(cudaEventRecord(pe[4], tail));
     if (pipelined) {
         if (has_lists) { CU(cudaEventRecord(ctx->ev_side[cslot], tail)); ctx->side_pending = true; }
@@ -2384,6 +2403,25 @@ extern "C" int32_t b200vis_download_frame_stats(b200vis_ctx *ctx, b200vis_frame_
     const uint32_t lp = (ctx->frame + 2u) % 3u;   // slot the last CULL frame (frame - 1) accumulated into
     out->gt_changed_count = s.changed[lp][0]; out->vv_changed_count = s.changed[lp][1]; out->frame = ctx->frame;
     ctx->last_gt_changed = out->gt_changed_count;
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_download_view_stats(b200vis_ctx *ctx, uint32_t first_view, uint32_t count, uint32_t *visible_count,
+                                               uint32_t *cluster_index_count, float *cluster_farthest_z, uint32_t *cluster_index_overflow) {
+    CHECK_CTX_JOIN();
+    if ((uint64_t)first_view + count > ctx->cfg.max_views)
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "download_view_stats: views [%u, %u) exceed max_views %u", first_view, first_view + count,
+                    ctx->cfg.max_views);
+    CU(cudaMemcpyAsync(ctx->h_stats, ctx->d_stats, sizeof(DevStats), cudaMemcpyDeviceToHost, ctx->stream));
+    CU(cudaStreamSynchronize(ctx->stream));
+    const DevStats &s = *ctx->h_stats;
+    for (uint32_t i = 0; i < count; ++i) {
+        const uint32_t v = first_view + i;
+        if (visible_count) visible_count[i] = s.visible_count[v];
+        if (cluster_index_count) cluster_index_count[i] = s.cl_index_count[v];
+        if (cluster_farthest_z) memcpy(&cluster_farthest_z[i], &s.cl_farthest_bits[v], 4);
+        if (cluster_index_overflow) cluster_index_overflow[i] = s.cl_overflow[v];
+    }
     return B200VIS_OK;
 }
 
@@ -2790,6 +2828,16 @@ extern "C" int32_t b200vis_set_result_sink(b200vis_ctx *ctx, const b200vis_resul
     return B200VIS_OK;
 }
 
+extern "C" int32_t b200vis_set_view_stats_sink(b200vis_ctx *ctx, uint32_t *per_view) {
+    CHECK_CTX_JOIN();
+    CU(cudaStreamSynchronize(ctx->stream));
+    ctx->view_stats_sink = ctx->view_stats_d = nullptr;
+    if (!per_view) return B200VIS_OK;
+    const int32_t rc = map_host(ctx, per_view, (size_t)ctx->cfg.max_views * 16, &ctx->view_stats_d); if (rc) return rc;
+    ctx->view_stats_sink = per_view;
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_set_column_sinks(b200vis_ctx *ctx, const b200vis_column_sinks *sinks) {
     CHECK_CTX_JOIN();
     CU(cudaStreamSynchronize(ctx->stream));
@@ -2870,7 +2918,7 @@ extern "C" int32_t b200vis_download_frame(b200vis_ctx *ctx, b200vis_frame_stats 
     // sync 2: exact-size list copies
     for (uint32_t v = 0; v < V; ++v) {
         if (visible_rows) {
-            const uint32_t c = stats->visible_count[v];
+            const uint32_t c = ctx->h_stats->visible_count[v];   // every view (b200vis_frame_stats holds the first eight)
             if (c > visible_capacity) return fail(ctx, B200VIS_ERR_CAPACITY, "download_frame: view %u has %u visible rows > capacity %u", v, c, visible_capacity);
             CU(cudaMemcpyAsync(visible_rows + (size_t)v * visible_capacity, ctx->vis.lists + (size_t)v * ctx->vis.list_stride, (size_t)c * 4, cudaMemcpyDeviceToHost, st));
         }
@@ -2924,12 +2972,26 @@ extern "C" int32_t b200vis_step(b200vis_ctx *ctx, uint32_t n_changed, const uint
     else { if ((rc = b200vis_download_frame_stats(ctx, &local))) return rc; st = &local; }
     lap(5);
     ctx->last_gt_changed = st->gt_changed_count;
+    // views past the eighth: the view-stats sink when the result sink published this frame, else the device stats block
+    // (b200vis_download_frame_stats above left a copy of it in h_stats)
+    const uint32_t *wide = nullptr;
+    if (clusters && n_cameras > (uint32_t)kMaxViews && ctx->have_sink) {
+        if (ctx->view_stats_sink) wide = ctx->view_stats_sink;
+        else {
+            CU(cudaMemcpyAsync(ctx->h_stats, ctx->d_stats, sizeof(DevStats), cudaMemcpyDeviceToHost, ctx->stream));
+            CU(cudaStreamSynchronize(ctx->stream));
+        }
+    }
     if (clusters)
         for (uint32_t v = 0; v < n_cameras; ++v) {   // Clusters::last_frame_* (assign.rs:810-811)
             b200vis_cluster_feedback &fb = ctx->auto_fb[v];
             if (!ctx->consts.cviews[v].enabled) continue;
-            fb.has_farthest_z = 1; fb.farthest_z = st->cluster_farthest_z[v];
-            fb.has_index_count = 1; fb.index_count = st->cluster_index_count[v];
+            float far_z = 0.0f; uint32_t idx = 0;
+            if (v < (uint32_t)kMaxViews) { far_z = st->cluster_farthest_z[v]; idx = st->cluster_index_count[v]; }
+            else if (wide) { memcpy(&far_z, &wide[(size_t)v * 4 + 2], 4); idx = wide[(size_t)v * 4 + 1]; }
+            else { memcpy(&far_z, &ctx->h_stats->cl_farthest_bits[v], 4); idx = ctx->h_stats->cl_index_count[v]; }
+            fb.has_farthest_z = 1; fb.farthest_z = far_z;
+            fb.has_index_count = 1; fb.index_count = idx;
         }
     return B200VIS_OK;
 }

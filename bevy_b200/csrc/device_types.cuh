@@ -6,7 +6,9 @@
 namespace b200vis {
 
 constexpr int kTileRows = 256;          // rows per tile == threads per CTA of the tile kernel
-constexpr int kMaxViews = 8;
+constexpr int kMaxViews = 8;            // views one cull pass covers: CullViews, the unrolled view loops, lane-per-view ballots
+constexpr int kMaxCameras = 32;         // views one context holds (B200VIS_MAX_CAMERAS): every per-view array and counter layout;
+                                        //   views past the eighth are culled in group passes of kMaxViews (k_cull's MERGE instantiation)
 constexpr int kMaxClusters = 4096;
 constexpr int kChunkWords = 1024;       // visible-mask words per compaction chunk (32768 rows)
 constexpr uint32_t kNoParent = 0xFFFFFFFFu;
@@ -120,18 +122,18 @@ struct DevClusterView {
 
 struct FrameConsts {
     uint32_t n_views, pad[3];
-    DevView views[kMaxViews];
-    DevClusterView cviews[kMaxViews];
+    DevView views[kMaxCameras];
+    DevClusterView cviews[kMaxCameras];
 };
 
 // counters written by the kernels (one D2H copy per frame)
 struct DevStats {
-    uint32_t visible_count[kMaxViews];     // written by the expand kernel for ACTIVE views only
-    uint32_t cl_index_count[kMaxViews];    // outputs of the last cluster frame (copied from the accumulators
-    uint32_t cl_farthest_bits[kMaxViews];  //   by the lists kernel, which also re-zeroes them)
-    uint32_t cl_overflow[kMaxViews];
-    uint32_t cl_acc_index[kMaxViews];      // accumulators of the assign kernel
-    uint32_t cl_acc_far[kMaxViews];        // float bits; values > 0 only, so integer max == float max
+    uint32_t visible_count[kMaxCameras];     // written by the expand kernel for ACTIVE views only
+    uint32_t cl_index_count[kMaxCameras];    // outputs of the last cluster frame (copied from the accumulators
+    uint32_t cl_farthest_bits[kMaxCameras];  //   by the lists kernel, which also re-zeroes them)
+    uint32_t cl_overflow[kMaxCameras];
+    uint32_t cl_acc_index[kMaxCameras];      // accumulators of the assign kernel
+    uint32_t cl_acc_far[kMaxCameras];        // float bits; values > 0 only, so integer max == float max
     uint32_t changed[3][2];                // [frame % 3][0 = gt, 1 = vv]; the expand kernel of frame f zeroes the
                                            // slot frame f+2 accumulates into (frame f+1 may already be running)
 };
@@ -142,7 +144,8 @@ struct VisibleBufs {
     uint32_t words_stride;   // words per view
     uint32_t chunks_stride;  // chunk counters per view
     uint32_t *mask;          // [V][words_stride], bit = rank (two copies, the host passes frame % 2's)
-    uint32_t *chunk_count;   // [3][V][chunks_stride], slot = frame % 3
+    uint32_t *chunk_count;   // [kMaxCameras / kMaxViews groups][3][kMaxViews][chunks_stride], slot = frame % 3: a cull pass over
+                             //   one group of eight views sees the [3][kMaxViews] layout of group 0 (chunk_counter_index)
     uint32_t *lists;         // [V][list_stride] rows, ascending Entity::to_bits()
     uint32_t list_stride;
     uint8_t *classes;        // [V][list_stride] VisibilityClass mask of each listed row (the shim splits the list per class)
@@ -151,6 +154,11 @@ struct VisibleBufs {
 
 // SURVEY 8(f) N1: RenderVisibleEntitiesClass::update_cpu_culled_entities on the device -- the added / removed
 // lists between last frame's and this frame's sorted visible list of a view (all pointers null = disabled)
+// row of VisibleBufs::chunk_count holding view v's counters of frame slot `slot`
+__host__ __device__ __forceinline__ size_t chunk_counter_index(uint32_t slot, uint32_t v) {
+    return ((size_t)(v / kMaxViews) * 3u + slot) * kMaxViews + v % kMaxViews;
+}
+
 struct DiffBufs {
     uint32_t *prev;          // [V][words_stride] visible set of the last frame the view was active, bit = rank
     uint32_t *words;         // [2][V][words_stride] added / removed bits of this frame
@@ -195,7 +203,7 @@ struct ClusterBufs {
     uint32_t world, rank;
     uint32_t max_views;
     uint32_t index_cap;      // per view
-    uint32_t *send;          // this rank's slab: [V][words][kMaxClusters] + trailer [kMaxViews] (the rank's farthest_z candidate per
+    uint32_t *send;          // this rank's slab: [V][words][kMaxClusters] + trailer [trailer] (the rank's farthest_z candidate per
                              //   view, float bits: it travels with the slab, so that Clusters::last_frame_* are identical on all ranks)
     const uint32_t *recv;    // gathered: [world] slabs
     uint32_t slab_words;     // words per slab incl. the trailer == the rank stride of recv
@@ -204,7 +212,9 @@ struct ClusterBufs {
     uint32_t *indices;       // [V][index_cap]
     // peer-memory exchange (b200vis_p2p_import): every rank's gathered buffer [2 parities][world][slab] as mapped into this
     // process, the flag words behind it [2][world], and this frame's parity / stamp.  p2p == 0: recv was filled by a collective.
-    uint32_t p2p, xparity, stamp, pad;
+    uint32_t p2p, xparity, stamp;
+    uint32_t trailer;        // words of the slab's farthest_z trailer: max(max_views, kMaxViews), so that an eight-view
+                             //   context (and every multi-GPU one) keeps the eight-word trailer it always had
     uint32_t *peer[8];
     uint32_t *peer_flags[8];
 };

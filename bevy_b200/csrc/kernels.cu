@@ -2158,8 +2158,15 @@ k_tile_warp(Rows R, const WarpTile *__restrict__ tiles, const uint8_t *__restric
 // One thread per row, CTAs of 256 rows starting at multiples of 256, so a warp covers exactly one
 // 32-bit word of the rank-ordered visible mask: when rows are in Entity::to_bits() order (SIMPLE) the
 // ballot is STORED (no atomics, no zeroing of the mask between frames).
+//
+// MERGE: a group pass over views 8g .. 8g + cvw.n_views - 1 (contexts with more than kMaxViews views), run after the frame's
+// tile pass.  `vb` points at the group's masks and chunk counters (chunk_counter_index), so the view index is the
+// group-local one, as in group 0.  It writes its own views' masks and chunk counters, and merges "visible in some view of the
+// group" into the state byte the tile pass left: a row in the query that pass found invisible (bit 0 clear) had S_VV_CHANGED
+// set to last frame's bit, so prev = S_VV_CHANGED and the row becomes VV = 1 | prev << 1, changed iff prev == 0; the
+// ViewVisibility change count moves by +1 (prev 0) or -1 (prev 1).  Rows already visible and rows outside the query stay.
 // ------------------------------------------------------------------------------------------
-template <bool SIMPLE>
+template <bool SIMPLE, bool MERGE>
 __global__ void __launch_bounds__(256, 4)
 k_cull(Rows R, const __grid_constant__ CullViews cvw, VisibleBufs vb, DevStats *__restrict__ stats, uint32_t parity) {
     const uint32_t row = blockIdx.x * 256u + threadIdx.x;
@@ -2263,6 +2270,14 @@ k_cull(Rows R, const __grid_constant__ CullViews cvw, VisibleBufs vb, DevStats *
             }
         }
     }
+    if (MERGE) {
+        const bool merge = in_query && any && !(st8 & 1u);
+        const uint32_t was = (st8 & S_VV_CHANGED) ? 1u : 0u;     // last frame's bit (see above)
+        if (merge) R.state[row] = (uint8_t)((st8 & ~(S_VV | S_VV_CHANGED)) | 1u | (was << 1) | (was ? 0u : S_VV_CHANGED));
+        const uint32_t up = __ballot_sync(0xFFFFFFFFu, merge && !was), down = __ballot_sync(0xFFFFFFFFu, merge && was);
+        if (lane == 0 && up != down) atomicAdd(&stats->changed[parity][1], (uint32_t)(__popc(up) - __popc(down)));
+        return;
+    }
     uint32_t out = st8;
     bool vv_changed = false;
     if (in_query) {
@@ -2309,9 +2324,9 @@ k_expand_visible(VisibleBufs vb, DiffBufs db, const uint32_t *__restrict__ row_o
     __shared__ uint32_t s_warp[32], s_diff[32];
     __shared__ uint32_t s_base, s_total;
     const uint32_t v = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
-    uint32_t *cc = vb.chunk_count + ((size_t)parity * kMaxViews + v) * vb.chunks_stride;
+    uint32_t *cc = vb.chunk_count + chunk_counter_index(parity, v) * vb.chunks_stride;
     const uint32_t zslot = (parity + 2u) % 3u;   // the slot frame f+2 will accumulate into
-    uint32_t *cc_next = vb.chunk_count + ((size_t)zslot * kMaxViews + v) * vb.chunks_stride;
+    uint32_t *cc_next = vb.chunk_count + chunk_counter_index(zslot, v) * vb.chunks_stride;
     // every view of the grid re-arms its counters, also the ones beyond this frame's view count: the count may rise
     // again by frame f+2, and nothing else clears the slot
     if (t == 0) cc_next[chunk] = 0;
@@ -2624,7 +2639,7 @@ k_cluster_assign(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBu
     float this_far = 0.0f;
     if (!assign_one_light(cv, tb, px, py, pz, range, lane, this_far, count, [&](uint32_t ci) { atomicOr(mask + ci, bit); })) return;
     // farthest_z candidates accumulate in the slab's trailer (values > 0 only: integer max == float max)
-    if (lane == 0 && this_far > 0.0f) atomicMax(cb.send + (cb.slab_words - kMaxViews) + v, __float_as_uint(this_far));
+    if (lane == 0 && this_far > 0.0f) atomicMax(cb.send + (cb.slab_words - cb.trailer) + v, __float_as_uint(this_far));
     (void)count; (void)stats;
 }
 
@@ -2813,9 +2828,9 @@ __global__ void __launch_bounds__(256)
 k_slab_push(const FrameConsts *__restrict__ fc, ClusterBufs cb, uint32_t *__restrict__ done) {
     const uint32_t v = blockIdx.y;
     const size_t slab_words = cb.slab_words;
-    if (blockIdx.x == 0 && threadIdx.x < cb.world && v < kMaxViews) {   // the trailer: this view's farthest_z candidate
-        const size_t tr = ((size_t)cb.xparity * cb.world + cb.rank) * slab_words + (slab_words - kMaxViews) + v;
-        cb.peer[threadIdx.x][tr] = cb.send[(slab_words - kMaxViews) + v];
+    if (blockIdx.x == 0 && threadIdx.x < cb.world && v < cb.trailer) {   // the trailer: this view's farthest_z candidate
+        const size_t tr = ((size_t)cb.xparity * cb.world + cb.rank) * slab_words + (slab_words - cb.trailer) + v;
+        cb.peer[threadIdx.x][tr] = cb.send[(slab_words - cb.trailer) + v];
     }
     if (v < fc->n_views && fc->cviews[v].enabled) {
         const uint32_t nc = fc->cviews[v].n_clusters;
@@ -2928,7 +2943,7 @@ k_cluster_lists(const FrameConsts *__restrict__ fc, ClusterBufs cb, DevStats *__
     if (blk == 0 && t == 0) {
         if (!nc) stats->cl_index_count[v] = 0;
         uint32_t far = 0;                                       // max over the ranks' candidates (gathered trailers)
-        for (uint32_t r = 0; r < cb.world; ++r) far = max(far, cb.recv[r * rank_stride + (rank_stride - kMaxViews) + v]);
+        for (uint32_t r = 0; r < cb.world; ++r) far = max(far, cb.recv[r * rank_stride + (rank_stride - cb.trailer) + v]);
         stats->cl_farthest_bits[v] = far;
     }
     // NOTE: the slab is zeroed for the next frame by k_cluster_clear (a CTA here may still be re-counting it)
@@ -2976,8 +2991,13 @@ __global__ void k_publish_visible(const uint32_t *__restrict__ lists, uint32_t l
 __global__ void k_publish_clusters(const FrameConsts *__restrict__ fc, const uint32_t *__restrict__ offsets, const uint32_t *__restrict__ indices,
                                    uint32_t index_cap, uint32_t *__restrict__ host_offsets, uint32_t *__restrict__ host_indices,
                                    uint32_t host_cap, const DevStats *__restrict__ stats, uint32_t *__restrict__ host_stats,
-                                   uint32_t changed_slot, uint32_t frame) {
+                                   uint32_t changed_slot, uint32_t frame, uint32_t *__restrict__ host_view_stats) {
     const uint32_t v = blockIdx.y, t = blockIdx.x * blockDim.x + threadIdx.x;
+    // the view-stats sink: [max_views][4] visible_count, cluster_index_count, cluster_farthest_z bits, overflow (every view)
+    if (host_view_stats != nullptr && blockIdx.x == 0 && threadIdx.x < 4) {
+        const uint32_t *src[4] = {stats->visible_count, stats->cl_index_count, stats->cl_farthest_bits, stats->cl_overflow};
+        host_view_stats[(size_t)v * 4 + threadIdx.x] = src[threadIdx.x][v];
+    }
     if (v == 0 && blockIdx.x == 0 && host_stats != nullptr) {
         // b200vis_frame_stats: visible_count[8] cluster_index_count[8] cluster_farthest_z[8] overflow[8] gt vv frame pad
         if (threadIdx.x < 8) {
@@ -3070,7 +3090,7 @@ __global__ void k_cluster_clear(const FrameConsts *__restrict__ fc, ClusterBufs 
     const DevClusterView &cv = fc->cviews[v];
     if (!cv.enabled) return;
     const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c == 0) cb.send[(cb.slab_words - kMaxViews) + v] = 0;
+    if (c == 0) cb.send[(cb.slab_words - cb.trailer) + v] = 0;
     if (c >= cv.n_clusters) return;
     uint32_t *mine = cb.send + (size_t)v * cb.words * kMaxClusters;
     for (uint32_t w = 0; w < cb.words; ++w) mine[(size_t)w * kMaxClusters + c] = 0;
@@ -3792,8 +3812,18 @@ bool tile_kernel_is_default() { return tile_kernel_choice() == 1; }
 void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity) {
     if (!R.n) return;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
-    if (simple) { ++g_launches; k_cull<true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
-    else { ++g_launches; k_cull<false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
+    if (simple) { ++g_launches; k_cull<true, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
+    else { ++g_launches; k_cull<false, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
+}
+void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
+                       uint32_t view_base) {
+    if (!R.n) return;
+    VisibleBufs g = vb;     // the group's masks and counter block: k_cull indexes views 0..7 of it
+    g.mask = vb.mask + (size_t)view_base * vb.words_stride;
+    g.chunk_count = vb.chunk_count + chunk_counter_index(0, view_base) * vb.chunks_stride;
+    const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
+    if (simple) { ++g_launches; k_cull<true, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity); }
+    else { ++g_launches; k_cull<false, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity); }
 }
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R) {
     if (R.n) { ++g_launches; k_mark_dirty_global<<<cdiv(R.n, 256), 256, 0, st>>>(R); }
@@ -3876,9 +3906,10 @@ void launch_publish_visible(cudaStream_t st, const VisibleBufs &vb, const DevSta
     ++g_launches; k_publish_visible<<<dim3(min(cdiv(n_rows, 256), 2u * (uint32_t)sms), n_views), 256, 0, st>>>(vb.lists, vb.list_stride, stats, host_rows, host_stride, n_views, vb.classes, host_classes);
 }
 void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, uint32_t *host_offsets, uint32_t *host_indices,
-                             uint32_t host_cap, const DevStats *stats, uint32_t *host_stats, uint32_t changed_slot, uint32_t frame, uint32_t max_views) {
+                             uint32_t host_cap, const DevStats *stats, uint32_t *host_stats, uint32_t changed_slot, uint32_t frame, uint32_t max_views,
+                             uint32_t *host_view_stats) {
     ++g_launches; k_publish_clusters<<<dim3(kMaxClusters / 256 + 1, max_views), 256, 0, st>>>(fc, cb.offsets, cb.indices, cb.index_cap, host_offsets, host_indices,
-                                                                                host_cap, stats, host_stats, changed_slot, frame);
+                                                                                host_cap, stats, host_stats, changed_slot, frame, host_view_stats);
 }
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
                         uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot) {

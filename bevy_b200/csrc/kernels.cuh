@@ -21,6 +21,10 @@ bool tile_kernel_publishes_light_snapshot();
 void launch_tile_warp(cudaStream_t st, const Rows &R, const WarpTile *tiles, const uint8_t *sched, uint32_t n_tiles, const CullViews &cvw,
                       const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity, uint32_t *counter);
 void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity);
+// one group pass of a context with more than kMaxViews views: views view_base .. view_base + cvw.n_views - 1, merged into
+// the ViewVisibility state the tile pass left (k_cull's MERGE instantiation)
+void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
+                       uint32_t view_base);
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R);
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views);
@@ -37,7 +41,8 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
 void launch_publish_visible(cudaStream_t st, const VisibleBufs &vb, const DevStats *stats, uint32_t *host_rows, uint32_t host_stride,
                             uint32_t n_rows, uint32_t n_views, uint8_t *host_classes);
 void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, uint32_t *host_offsets, uint32_t *host_indices,
-                             uint32_t host_cap, const DevStats *stats, uint32_t *host_stats, uint32_t changed_slot, uint32_t frame, uint32_t max_views);
+                             uint32_t host_cap, const DevStats *stats, uint32_t *host_stats, uint32_t changed_slot, uint32_t frame, uint32_t max_views,
+                             uint32_t *host_view_stats = nullptr);
 void launch_tag_lights(cudaStream_t st, const Rows &R, const Lights &L, uint32_t *light_ord, uint32_t *all_tagged);
 void launch_snapshot_lights(cudaStream_t st, const Rows &R, const Lights &L, float4 *snap);
 void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, uint32_t stride, uint32_t *host_gt_bits, uint8_t *host_vv,

@@ -11,6 +11,17 @@ import numpy as np
 from . import abi
 
 
+class WideFrameStats:
+    """FrameStats of a context with more than abi.MAX_VIEWS views: the per-view fields are arrays over every view."""
+
+    def __init__(self, stats, per_view):
+        self.visible_count = per_view["visible_count"]
+        self.cluster_index_count = per_view["cluster_index_count"]
+        self.cluster_farthest_z = per_view["cluster_farthest_z"]
+        self.cluster_index_overflow = per_view["cluster_index_overflow"]
+        self.gt_changed_count, self.vv_changed_count, self.frame = stats.gt_changed_count, stats.vv_changed_count, stats.frame
+
+
 class VisibilityPipeline:
     def __init__(self, scene, device=0, static_transform_optimizations=True, max_cluster_indices=0,
                  world_size=1, rank=0, cluster_config=None, max_lights=None, max_entities=None):
@@ -111,8 +122,11 @@ class VisibilityPipeline:
         self.visible_diff = bool(enabled)
 
     def read_feedback(self):
-        """Clusters::last_frame_* (assign.rs:810-811): feeds next frame's far_z and dynamic resizing."""
+        """Clusters::last_frame_* (assign.rs:810-811): feeds next frame's far_z and dynamic resizing.  Returns the frame's
+        FrameStats; a context with more than abi.MAX_VIEWS views gets a WideFrameStats with the same fields over every view."""
         s = self.ctx.download_frame_stats()
+        if self.ctx.max_views > abi.MAX_VIEWS:
+            s = WideFrameStats(s, self.ctx.download_view_stats())
         for v in range(len(self.scene.cameras)):
             cv = self.cluster_views[v]
             if cv is None or not cv.enabled:

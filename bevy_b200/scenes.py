@@ -273,6 +273,54 @@ def propagate_bench_scene():
                  cameras=[_camera(0.0)], roots=np.array(roots, np.uint32))
 
 
+def many_cameras_lights(n_cameras=16, forest_kwargs=None, radius=4.0, name=None):
+    """examples/stress_tests/many_cameras_lights.rs: a Circle::new(4.0) base rotated -90 degrees about X, a unit Cuboid at
+    (0, 0.5, 0), NUM_LIGHTS = 5 shadow-casting point lights (PointLight::default range 20) at (sin a * 4, 2, cos a * 4), and
+    a 4x4 grid of cameras (480x270 viewports of a 1920x1080 window) at (sin a * 4, 2.5, cos a * 4) looking at the origin.
+    forest_kwargs: also add forest(**forest_kwargs, n_lights=0) behind those rows, so that the cull has real work."""
+    f32 = np.float32
+    q_base = quat_axis("x", -math.pi / 2)
+    trs = np.concatenate([_trs(np.zeros((1, 3), f32), q_base[None].astype(f32)), _trs(np.array([[0.0, 0.5, 0.0]], f32))])
+    bounds = np.zeros((2, 6), f32)
+    bounds[0, 3:6] = (4.0, 4.0, 0.0)           # Circle::new(4.0).aabb_3d: the XY disc
+    bounds[1, 3:6] = 0.5                       # Cuboid::new(1, 1, 1)
+    cols = (np.full(2, NO_PARENT, np.uint32), trs, bounds, np.full(2, F_INHERITED_VISIBLE | F_HAS_AABB, np.uint8),
+            np.full(2, CLASS_MESH, np.uint8))
+    a = np.array([np.float32(i) / np.float32(5) * np.float32(math.pi) * np.float32(2) for i in range(5)], f32)
+    pos = np.stack([np.sin(a) * f32(radius), np.full(5, 2.0, f32), np.cos(a) * f32(radius)], 1).astype(f32)
+    cols, light_row = _append_lights(cols, pos, np.full(5, 20.0, f32))
+    parent, trs, bounds, flags, cls = cols
+    roots = None
+    if forest_kwargs:
+        fo = forest(**dict(forest_kwargs, n_lights=0))
+        n0 = len(parent)
+        fp = np.where(fo.parent == NO_PARENT, NO_PARENT, fo.parent + np.uint32(n0)).astype(np.uint32)
+        parent = np.concatenate([parent, fp]); trs = np.concatenate([trs, fo.trs]); bounds = np.concatenate([bounds, fo.bounds])
+        flags = np.concatenate([flags, fo.flags]); cls = np.concatenate([cls, fo.class_mask])
+        roots = (fo.roots + np.uint32(n0)).astype(np.uint32)
+    cams = []
+    for i in range(n_cameras):
+        ang = np.float32(i) / np.float32(n_cameras) * np.float32(math.pi) * np.float32(2)
+        p = np.array([np.sin(ang) * f32(radius), 2.5, np.cos(ang) * f32(radius)], f32)
+        q = look_at_quats(p[None].astype(np.float64))[0]
+        cams.append(Camera(gt=quat_to_gt(q, p), quat=q, aspect=480.0 / 270.0))
+    return Scene(name or f"many_cameras_lights_{n_cameras}" + ("_forest" if forest_kwargs else ""), parent, trs, bounds, flags, cls,
+                 _entity_bits(len(parent)), light_row, np.full(5, 20.0, f32), cams, roots, screen=(480, 270))
+
+
+def rotate_cameras(scene, delta):
+    """rotate_cameras of many_cameras_lights.rs: Transform::rotate_around(Vec3::ZERO, Quat::from_rotation_y(delta)) moves
+    both the translation and the rotation of every camera."""
+    r = quat_axis("y", delta)
+    c, s_ = math.cos(delta), math.sin(delta)
+    for cam in scene.cameras:
+        x, y, z = (float(v) for v in cam.gt[9:12])
+        t = (c * x + s_ * z, y, -s_ * x + c * z)
+        q = quat_mul(r, cam.quat)
+        cam.quat = q / np.linalg.norm(q)
+        cam.gt = quat_to_gt(cam.quat, t)
+
+
 # ---- per-frame animation ---------------------------------------------------------------------
 def advance_cameras(scene, delta=0.15 / 60.0):
     """move_camera (many_cubes.rs:590-603): rotate_z(delta) then rotate_x(delta); Transform::rotate

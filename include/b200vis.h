@@ -76,7 +76,9 @@ enum {
 #define B200VIS_STAGE_CLUSTER        (B200VIS_STAGE_CLUSTER_ASSIGN | B200VIS_STAGE_CLUSTER_LISTS)
 #define B200VIS_STAGE_ALL            0xFu
 
-#define B200VIS_MAX_VIEWS     8u
+#define B200VIS_MAX_VIEWS     8u     /* views b200vis_frame_stats reports, and views per rank with world_size > 1 */
+#define B200VIS_MAX_CAMERAS   32u    /* views one context may hold (b200vis_config::max_views, world_size 1): views past the
+                                        eighth are culled in extra passes of eight views each (DESIGN.md section 4) */
 #define B200VIS_MAX_CLUSTERS  4096u  /* assign.rs:410-413 */
 
 typedef struct b200vis_ctx b200vis_ctx;
@@ -85,7 +87,7 @@ typedef struct b200vis_config {
     int32_t  device;              /* CUDA device ordinal */
     uint32_t max_entities;        /* row capacity */
     uint32_t max_lights;          /* point lights this context (this rank's shard) may hold */
-    uint32_t max_views;           /* <= B200VIS_MAX_VIEWS */
+    uint32_t max_views;           /* 1..B200VIS_MAX_CAMERAS; <= B200VIS_MAX_VIEWS when world_size > 1 */
     uint32_t max_cluster_indices; /* per-view capacity of the cluster index list (0 => 1<<20) */
     uint32_t world_size;          /* ranks sharing the cluster exchange (0/1 => single GPU) */
     uint32_t rank;
@@ -376,6 +378,11 @@ B200VIS_API int32_t b200vis_step(b200vis_ctx *ctx, uint32_t n_changed, const uin
 
 /* ---- results --------------------------------------------------------------------- */
 B200VIS_API int32_t b200vis_download_frame_stats(b200vis_ctx *ctx, b200vis_frame_stats *out);
+/* The per-view part of the frame statistics for views [first_view, first_view + count) of any context, up to max_views
+ * (b200vis_frame_stats holds views 0..7).  Each array receives `count` entries and may be NULL. */
+B200VIS_API int32_t b200vis_download_view_stats(b200vis_ctx *ctx, uint32_t first_view, uint32_t count, uint32_t *visible_count,
+                                                uint32_t *cluster_index_count, float *cluster_farthest_z,
+                                                uint32_t *cluster_index_overflow);
 /* gt[count][stride_floats] (stride 12, or 16 for glam's padded Affine3A layout); changed[count]:
  * 1 where the shim must stamp changed_ticks (set_if_neq semantics, systems.rs:719). Either may be NULL. */
 B200VIS_API int32_t b200vis_download_global_transforms(b200vis_ctx *ctx, uint32_t first_row, uint32_t count, float *gt,
@@ -420,6 +427,10 @@ typedef struct b200vis_result_sink {
     uint32_t *cluster_indices; uint32_t cluster_capacity;
 } b200vis_result_sink;
 B200VIS_API int32_t b200vis_set_result_sink(b200vis_ctx *ctx, const b200vis_result_sink *sink);
+/* Per-view statistics of every view, written with the result sink's stats block (so reading them needs no extra
+ * synchronisation): per_view[max_views][4] = visible_count, cluster_index_count, cluster_farthest_z (float bits),
+ * cluster_index_overflow.  Needs a result sink to be published.  Pinned or registered like the result sink; NULL removes it. */
+B200VIS_API int32_t b200vis_set_view_stats_sink(b200vis_ctx *ctx, uint32_t *per_view);
 
 /* ---- write-back of the frame's column results into the caller's ECS columns -------------------------------------------
  * The reference systems leave their results IN the ECS: GlobalTransform (+ Changed<GlobalTransform>) and ViewVisibility

@@ -74,6 +74,7 @@ extern "C" {
                                        planes_scratch: *mut f32, out: *mut b200vis_cluster_view) -> i32;
     fn b200vis_run(ctx: *mut b200vis_ctx, stages: u32) -> i32;
     fn b200vis_set_result_sink(ctx: *mut b200vis_ctx, sink: *const b200vis_result_sink) -> i32;
+    fn b200vis_set_view_stats_sink(ctx: *mut b200vis_ctx, per_view: *mut [u32; 4]) -> i32;
     fn b200vis_set_column_sinks(ctx: *mut b200vis_ctx, sinks: *const b200vis_column_sinks) -> i32;
     fn b200vis_writeback_columns_ex(ctx: *mut b200vis_ctx, which: u32) -> i32;
 }
@@ -84,7 +85,7 @@ const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04
 const F_RANGE: u8 = 0x10; const F_SPHERE_FROM_GT: u8 = 0x40;
 const VIEW_ACTIVE: u8 = 1; const VIEW_NO_CPU_CULLING: u8 = 2;
 const ERR_HIERARCHY_CYCLE: i32 = 4;
-const MAX_VIEWS: usize = 8; const MAX_CLUSTERS: usize = 4096;
+const MAX_CAMERAS: usize = 32; const MAX_CLUSTERS: usize = 4096;
 
 /// Device context, the entity <-> row map, and the pinned host buffers the GPU writes into.  `Send + Sync`: exactly one
 /// system touches it at a time (`ResMut`).  The result buffers are allocated once at full capacity and never reallocated:
@@ -104,6 +105,8 @@ pub struct B200Vis {
     light_entities: Vec<Entity>,  // light ordinal -> entity (query order of the cluster system)
     // sinks
     stats: Box<b200vis_frame_stats>,
+    view_stats: Vec<[u32; 4]>,    // every view: visible_count, cluster_index_count, cluster_farthest_z bits, overflow
+    max_views: usize,
     gt_col: Vec<[f32; 16]>, gt_bits: Vec<u32>, vv_col: Vec<u8>, vv_bits: Vec<u32>,
     visible_rows: Vec<u32>, visible_classes: Vec<u8>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
     planes_scratch: Vec<f32>,
@@ -128,11 +131,14 @@ impl B200Vis {
     }
 }
 
-pub struct B200VisibilityPlugin { pub max_entities: u32, pub max_lights: u32 }
+/// `max_cameras`: the most cameras (views) the app renders at once, 1..=32; views past the eighth cost one extra cull pass
+/// per eight views (DESIGN.md section 4), and the result buffers are sized by it.
+pub struct B200VisibilityPlugin { pub max_entities: u32, pub max_lights: u32, pub max_cameras: u32 }
 
 impl Plugin for B200VisibilityPlugin {
     fn build(&self, app: &mut App) {
-        let cfg = b200vis_config { device: 0, max_entities: self.max_entities, max_lights: self.max_lights, max_views: MAX_VIEWS as u32,
+        let max_views = (self.max_cameras as usize).clamp(1, MAX_CAMERAS);
+        let cfg = b200vis_config { device: 0, max_entities: self.max_entities, max_lights: self.max_lights, max_views: max_views as u32,
                                    max_cluster_indices: 0, world_size: 1, rank: 0, reserved: 0 };
         let mut ctx = core::ptr::null_mut();
         let rc = unsafe { b200vis_create(&cfg, &mut ctx) };
@@ -142,9 +148,9 @@ impl Plugin for B200VisibilityPlugin {
         let mut vis = B200Vis {
             ctx, max_entities: n, n: 0, row_of: Default::default(), entity_of: Vec::new(), columns_epoch: 0, bounds_epoch: u64::MAX,
             lights_epoch: u64::MAX, classes: Vec::new(), view_entities: Vec::new(), light_entities: Vec::new(),
-            stats: Box::default(), gt_col: vec![[0.0; 16]; n], gt_bits: vec![0; n.div_ceil(32)], vv_col: vec![0; n],
-            vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; MAX_VIEWS * n], visible_classes: vec![0; MAX_VIEWS * n],
-            cluster_offsets: vec![0; MAX_VIEWS * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; MAX_VIEWS * cluster_cap], cluster_cap,
+            stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, gt_col: vec![[0.0; 16]; n], gt_bits: vec![0; n.div_ceil(32)], vv_col: vec![0; n],
+            vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; max_views * n], visible_classes: vec![0; max_views * n],
+            cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
             planes_scratch: vec![0.0; 3 * 4097 * 4],
         };
         let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: vis.visible_rows.as_mut_ptr(), visible_capacity: n as u32,
@@ -152,7 +158,10 @@ impl Plugin for B200VisibilityPlugin {
             cluster_indices: vis.cluster_indices.as_mut_ptr(), cluster_capacity: cluster_cap as u32 };
         let cs = b200vis_column_sinks { global_transforms: vis.gt_col.as_mut_ptr().cast(), gt_stride_floats: 16,
             gt_changed_bits: vis.gt_bits.as_mut_ptr(), view_visibility: vis.vv_col.as_mut_ptr(), vv_changed_bits: vis.vv_bits.as_mut_ptr() };
-        unsafe { assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_column_sinks(ctx, &cs), 0); }
+        unsafe {
+            assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_column_sinks(ctx, &cs), 0);
+            assert_eq!(b200vis_set_view_stats_sink(ctx, vis.view_stats.as_mut_ptr()), 0);   // per-view stats of every view
+        }
         app.insert_resource(vis);
         // CPU clustering mode, so that `Clusters` holds `ClusterableObjects::Cpu`, which the cluster system fills (SURVEY.md 0)
         app.insert_resource(GlobalClusterSettings { gpu_clustering: None, supports_storage_buffers: true,
@@ -303,7 +312,7 @@ fn b200_check_visibility(
         // VisibleEntityRanges keeps its view -> bit table private; the shim builds its own masks below with bit v = device view v
         if visible_entity_ranges.is_some() { v.range_view_index = views.len() as i8; }
         views.push(v); vis.view_entities.push(entity);
-        if views.len() == MAX_VIEWS { break; }
+        if views.len() == vis.max_views { break; }
     }
     vis.check(unsafe { b200vis_set_views(vis.ctx, views.len() as u32, views.as_ptr()) })?;
     // ---- row columns: everything after a renumbering, otherwise the rows whose components changed, as contiguous ranges ----
@@ -364,7 +373,7 @@ fn b200_check_visibility(
         let Ok((_, mut visible_entities, _, _, camera, _)) = view_query.get_mut(*view_entity) else { continue };
         if !camera.is_active { continue; }                       // an inactive view keeps its lists (mod.rs:780-782)
         for list in visible_entities.entities.values_mut() { list.clear(); }
-        let count = vis.stats.visible_count[v] as usize;
+        let count = vis.view_stats[v][0] as usize;
         let (rows, masks) = (&vis.visible_rows[v * vis.max_entities..][..count], &vis.visible_classes[v * vis.max_entities..][..count]);
         for (row, mask) in rows.iter().zip(masks) {
             let entity = vis.entity_of[*row as usize];
@@ -463,8 +472,8 @@ fn b200_assign_lights_to_clusters(
             for i in off[c]..off[c + 1] { cell.add_point_light(vis.light_entities[idx[i as usize] as usize]); }   // ascending light order = push order (assign.rs:487)
         }
         clusters.clusterable_objects = ClusterableObjects::Cpu(cells);
-        clusters.last_frame_total_cluster_index_count = Some(vis.stats.cluster_index_count[v] as usize);
-        clusters.last_frame_farthest_z = Some(vis.stats.cluster_farthest_z[v]);     // assign.rs:810-811
+        clusters.last_frame_total_cluster_index_count = Some(vis.view_stats[v][1] as usize);
+        clusters.last_frame_farthest_z = Some(f32::from_bits(vis.view_stats[v][2]));     // assign.rs:810-811
     }
     Ok(())
 }
