@@ -89,6 +89,53 @@ class ColumnSinks(C.Structure):
                 ("view_visibility", C.c_void_p), ("vv_changed_bits", C.c_void_p)]
 
 
+WB_GLOBAL_TRANSFORM, WB_VIEW_VISIBILITY = 0x1, 0x2
+MAX_TABLES = 4096
+UNMAPPED = 0xFFFFFFFF
+
+
+class Table(C.Structure):
+    """b200vis_table: one archetype table's GlobalTransform / ViewVisibility columns and their changed_ticks columns."""
+    _fields_ = [("global_transforms", C.c_void_p), ("gt_changed_ticks", C.c_void_p), ("view_visibility", C.c_void_p),
+                ("vv_changed_ticks", C.c_void_p), ("len", C.c_uint32), ("capacity", C.c_uint32)]
+
+
+class HostTable:
+    """An archetype table's four columns as numpy views: gt [capacity, 16] float32 (glam Affine3A), gt_ticks [capacity]
+    uint32, vv [capacity] uint8, vv_ticks [capacity] uint32.  host_tables() carves several of them out of one buffer."""
+
+    def __init__(self, gt, gt_ticks, vv, vv_ticks, length):
+        self.gt, self.gt_ticks, self.vv, self.vv_ticks, self.len = gt, gt_ticks, vv, vv_ticks, int(length)
+        self.capacity = len(vv)
+
+    def desc(self, columns=("gt", "gt_ticks", "vv", "vv_ticks")):
+        """The b200vis_table of this table; columns left out are passed as NULL."""
+        p = lambda name: getattr(self, name).ctypes.data if name in columns else None
+        return Table(p("gt"), p("gt_ticks"), p("vv"), p("vv_ticks"), self.len, self.capacity)
+
+
+def host_tables(capacities, lengths=None, gt_fill=np.nan, tick_fill=0, vv_fill=0, pad=64):
+    """Tables over ONE plain (unpinned) numpy buffer, back to back: the columns of neighbouring tables share pages, as
+    small tables from one heap do.  The tables start on a page boundary and the buffer owns every page they touch, so the
+    library's page-rounded registration never reaches another allocation.  Returns (tables, buffer); the buffer must
+    outlive the registration."""
+    lengths = capacities if lengths is None else lengths
+    al = lambda b: (b + pad - 1) // pad * pad
+    sizes = [(al(c * 64), al(c * 4), al(max(c, 1)), al(c * 4)) for c in capacities]
+    page = 4096
+    buf = np.zeros((sum(sum(s) for s in sizes) + 2 * page - 1) // page * page + page, np.uint8)
+    base = (-buf.ctypes.data) % page
+    out, o = [], base
+    for c, n, (a, b, v, d) in zip(capacities, lengths, sizes):
+        gt = buf[o:o + c * 64].view(np.float32).reshape(c, 16); o += a
+        gtt = buf[o:o + c * 4].view(np.uint32); o += b
+        vv = buf[o:o + c]; o += v
+        vvt = buf[o:o + c * 4].view(np.uint32); o += d
+        gt[:] = gt_fill; gtt[:] = tick_fill; vv[:] = vv_fill; vvt[:] = tick_fill
+        out.append(HostTable(gt, gtt, vv, vvt, n))
+    return out, buf
+
+
 class ShadowItem(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("light_row", C.c_uint32), ("range", C.c_float), ("range_view_index", C.c_int32),
                 ("layer_mask", C.c_uint64), ("frusta", C.c_float * 144)]
@@ -129,6 +176,9 @@ _SIGNATURES = {
     "b200vis_set_column_sinks": (C.c_int32, [_vp, _P(ColumnSinks)]),
     "b200vis_writeback_columns": (C.c_int32, [_vp]),
     "b200vis_writeback_columns_ex": (C.c_int32, [_vp, C.c_uint32]),
+    "b200vis_set_tables": (C.c_int32, [_vp, C.c_uint32, _vp]),
+    "b200vis_set_table_rows": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32, _vp]),
+    "b200vis_writeback_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
     "b200vis_host_plan_summary": (C.c_int32, [C.c_uint32, _vp, _P(C.c_uint32)]),
     "b200vis_host_tile_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp]),
     "b200vis_host_warp_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp, _vp, _vp]),
@@ -769,6 +819,20 @@ class Context:
     def writeback_columns(self, which=3):
         """which: 1 = GlobalTransform (+ its change bits), 2 = ViewVisibility (+ its change bits), 3 = both."""
         self._check(self._lib.b200vis_writeback_columns_ex(self._h, which))
+
+    def set_tables(self, tables):
+        """b200vis_set_tables: `tables` are Table structs or HostTables (whose memory must outlive the registration)."""
+        descs = [t.desc() if isinstance(t, HostTable) else t for t in tables]
+        arr = (Table * max(len(descs), 1))(*descs)
+        self._check(self._lib.b200vis_set_tables(self._h, len(descs), arr))
+
+    def set_table_rows(self, table, first_slot, rows):
+        """b200vis_set_table_rows: slots [first_slot, first_slot + len(rows)) of `table` -> rows (UNMAPPED = unmapped)."""
+        r = _arr(rows, np.uint32)
+        self._check(self._lib.b200vis_set_table_rows(self._h, table, first_slot, len(r), _ptr(r) if len(r) else None))
+
+    def writeback_tables(self, which=WB_GLOBAL_TRANSFORM | WB_VIEW_VISIBILITY, gt_tick=0, vv_tick=0):
+        self._check(self._lib.b200vis_writeback_tables(self._h, which, gt_tick, vv_tick))
 
     def p2p_export(self):
         """CUDA IPC handle (64 bytes) of this rank's gathered buffer."""

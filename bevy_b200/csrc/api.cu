@@ -16,6 +16,7 @@
 #include <chrono>
 #include <cuda_runtime.h>
 #include <dlfcn.h>
+#include <unistd.h>
 
 #include "../../include/b200vis.h"
 #include "device_types.cuh"
@@ -168,6 +169,18 @@ struct b200vis_ctx {
     bool step_defers_stats = false;     // inside b200vis_step: the CULL run leaves the sink's stats block to the CLUSTER run
     float *d_gt_aos = nullptr;          // dense write-back: the GlobalTransform column in the host's layout, copied by the DMA engine
     uint32_t last_gt_changed = 0;       // Changed<GlobalTransform> rows of the last frame whose statistics the host has seen
+    // b200vis_set_tables: the registry, the host copy of the slot -> row maps (every table's map back to back, as on the
+    // device) and its inverse, and the host-memory registrations the library owns
+    bool tables_set = false;
+    std::vector<b200vis_table> h_tabs; std::vector<uint32_t> tab_off;   // tab_off[t] = table t's first map entry
+    std::vector<uint32_t> h_tab_map, row_slot;                           // row_slot[row] = the row's map entry, or kNoParent
+    std::vector<std::pair<uintptr_t, size_t>> host_regs;
+    DevTable *d_tabs = nullptr; uint32_t *d_tab_chunks = nullptr; uint32_t tab_chunks_cap = 0, n_tab_chunks = 0;
+    uint32_t *d_tab_map = nullptr; size_t tab_map_cap = 0; uint32_t *d_tab_total = nullptr;
+    uint8_t *d_tvv_shadow = nullptr;    // per row: the ViewVisibility byte the row's table slot holds (0xFF = unknown)
+    uint8_t *d_tab_upd = nullptr; size_t tab_upd_cap = 0;   // map updates on their way to k_update_table_map
+    std::vector<uint32_t> pend_touched, pend_reset;          // queued map entries / shadow resets, sent by flush_table_updates
+    uint8_t *h_tab_stage = nullptr; size_t h_tab_stage_cap = 0; cudaEvent_t ev_tab = nullptr;   // pinned staging of a batch
     double step_t[6] = {0, 0, 0, 0, 0, 0}; uint64_t step_n = 0;   // B200VIS_STEP_TRACE: host time per phase of b200vis_step
     void *nccl_comm = nullptr;          // b200vis_comm_init
     uint32_t *d_gather = nullptr;       // [world][slab] when the library owns the exchange
@@ -227,8 +240,13 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->bind.oc, ctx->bind.il, ctx->bind.count, ctx->d_bind_map,
                    ctx->d_range_se, ctx->d_range_ua, ctx->d_range_views, ctx->d_visibility, ctx->d_iv_changed,
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
-                   ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2};
+                   ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
+                   ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd};
     for (void *p : dev) if (p) cudaFree(p);
+    for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
+    cudaGetLastError();
+    if (ctx->h_tab_stage) cudaFreeHost(ctx->h_tab_stage);
+    if (ctx->ev_tab) cudaEventDestroy(ctx->ev_tab);
     if (ctx->h_edit) cudaFreeHost(ctx->h_edit);
     if (ctx->ev_edit) cudaEventDestroy(ctx->ev_edit);
     free_plan(ctx->hplan);
@@ -935,6 +953,12 @@ static int32_t plan_world(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, 
     return B200VIS_OK;
 }
 
+// the slot -> row maps of b200vis_set_tables follow the row numbering
+static int32_t tables_unmap_all(b200vis_ctx *ctx);
+static int32_t tables_unmap_rows(b200vis_ctx *ctx, uint32_t n_rows, const uint32_t *rows);
+static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_to_new);
+static int32_t flush_table_updates(b200vis_ctx *ctx);
+
 extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, const uint64_t *entity_bits) {
     CHECK_CTX_JOIN();
     if (n && (!parent || !entity_bits)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_topology: null array");
@@ -1001,7 +1025,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         ctx->keys_resident = false;
         ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
     }
-    return B200VIS_OK;
+    return tables_unmap_all(ctx);
 }
 
 static int32_t grow_edit_staging(b200vis_ctx *ctx, size_t bytes) {
@@ -1182,7 +1206,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
     // n_words / n_chunks needs no clearing
     ctx->vis.n_chunks = (ctx->vis.n_words + kChunkWords - 1) / kChunkWords;
     ctx->gt_aos_valid = false;
-    return B200VIS_OK;
+    return tables_unmap_rows(ctx, n_despawn, despawn_rows);
 }
 
 extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparent, const uint32_t *reparent_rows,
@@ -1260,6 +1284,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
         for (void *p : {(void *)R.flags, (void *)R.state, (void *)ctx->d_cls, (void *)ctx->d_range_ua, (void *)ctx->d_visibility,
                         (void *)ctx->d_iv_changed, (void *)ctx->d_caster}) add(p, 1, 1, 0);
         add(ctx->d_vv_shadow, 1, 1, 0xFF);                                 // the host's value unknown
+        add(ctx->d_tvv_shadow, 1, 1, 0xFF);                                // the same for the table write-back
     }
     // ---- device scratch: the maps, then the permuted columns (a group at a time) and the reparented rows ----
     auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
@@ -1342,6 +1367,11 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
     }
     // ---- the lists results hold, renumbered in place (survivors keep their rank order, so every list stays sorted) ----
     for (uint32_t i = 0; i < n_lists; ++i) launch_renumber_listed_rows(st, lists[i], n, d_o2n, n);
+    if ((rc = flush_table_updates(ctx))) return rc;      // queued map updates carry the old row numbers
+    if (ctx->tables_set && !ctx->h_tab_map.empty()) {   // the tables' slot -> row maps: mapped rows are live, none is dropped
+        const uint32_t slots = (uint32_t)ctx->h_tab_map.size();
+        launch_renumber_listed_rows(st, RowLists{ctx->d_tab_map, slots, 1, 1, ctx->d_tab_total}, slots, d_o2n, n);
+    }
     CU(cudaGetLastError());
     // ---- the row permutation of every resident per-row column, in groups that fit the staging buffer ----
     {
@@ -1432,6 +1462,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
     ctx->vis.n_words = nw2;
     ctx->vis.n_chunks = nc2;
     ctx->gt_aos_valid = false;
+    tables_renumber(ctx, o2n);
     if (old_to_new_out) memcpy(old_to_new_out, o2n.data(), (size_t)n * 4);
     if (trace) {
         const double dev_ms = std::chrono::duration<double, std::milli>(clk::now() - t_dev0).count();
@@ -2892,6 +2923,275 @@ extern "C" int32_t b200vis_writeback_columns_ex(b200vis_ctx *ctx, uint32_t which
     if (gt_sink) ctx->gt_aos_valid = false;   // rows written straight to the host bypass the staging copy: it is stale from here on
     launch_writeback_columns(ctx->stream, ctx->rows, gt_sink, ctx->colsink.gt_stride_floats, wgt ? ctx->col_gt_bits_d : nullptr,
                              wvv ? ctx->col_vv_d : nullptr, wvv ? ctx->col_vv_bits_d : nullptr, ctx->d_vv_shadow);
+    CU(cudaGetLastError());
+    return B200VIS_OK;
+}
+
+// ---- write-back into the caller's archetype tables (b200vis_set_tables) ------------------------------------------------
+// The host keeps the slot -> row maps of every table back to back exactly as the device holds them, plus the inverse
+// row -> map entry it needs to validate calls and to apply moves.  Updates reach the device as (entry, row) pairs.
+static constexpr uint32_t kUnmapped = B200VIS_UNMAPPED;
+
+// Map updates are queued on the host and sent as one batch right before the device next reads the maps
+// (b200vis_writeback_tables, b200vis_compact_topology, b200vis_set_tables), so b200vis_set_table_rows and the edits never
+// wait for the stream.  A batch = the touched map entries with their host values at flush time + the shadow resets.
+static void queue_table_updates(b200vis_ctx *ctx, const std::vector<uint32_t> &touched, const std::vector<uint32_t> &reset) {
+    ctx->pend_touched.insert(ctx->pend_touched.end(), touched.begin(), touched.end());
+    ctx->pend_reset.insert(ctx->pend_reset.end(), reset.begin(), reset.end());
+}
+static int32_t flush_table_updates(b200vis_ctx *ctx) {
+    std::vector<uint32_t> &touched = ctx->pend_touched, &reset = ctx->pend_reset;
+    if (touched.empty() && reset.empty()) return B200VIS_OK;
+    std::sort(touched.begin(), touched.end());
+    touched.erase(std::unique(touched.begin(), touched.end()), touched.end());
+    const size_t n_set = touched.size(), n_reset = reset.size(), set_bytes = n_set * 8, bytes = set_bytes + n_reset * 4;
+    if (ctx->ev_tab) CU(cudaEventSynchronize(ctx->ev_tab));   // the last batch's staging copy has been read
+    else CU(cudaEventCreateWithFlags(&ctx->ev_tab, cudaEventDisableTiming));
+    if (bytes > ctx->h_tab_stage_cap) {
+        if (ctx->h_tab_stage) cudaFreeHost(ctx->h_tab_stage);
+        ctx->h_tab_stage = nullptr; ctx->h_tab_stage_cap = 0;
+        const size_t cap = std::max<size_t>(2 * bytes, 4096);
+        CU(cudaMallocHost(&ctx->h_tab_stage, cap));
+        ctx->h_tab_stage_cap = cap;
+    }
+    if (bytes > ctx->tab_upd_cap) {
+        CU(cudaStreamSynchronize(ctx->stream));               // an earlier batch's kernel may still read the old buffer
+        if (ctx->d_tab_upd) cudaFree(ctx->d_tab_upd);
+        ctx->d_tab_upd = nullptr; ctx->tab_upd_cap = 0;
+        CU(dalloc(&ctx->d_tab_upd, ctx->h_tab_stage_cap));
+        ctx->tab_upd_cap = ctx->h_tab_stage_cap;
+    }
+    uint2 *set = reinterpret_cast<uint2 *>(ctx->h_tab_stage);
+    for (size_t i = 0; i < n_set; ++i) set[i] = make_uint2(touched[i], ctx->h_tab_map[touched[i]]);
+    if (n_reset) memcpy(ctx->h_tab_stage + set_bytes, reset.data(), n_reset * 4);
+    CU(cudaMemcpyAsync(ctx->d_tab_upd, ctx->h_tab_stage, bytes, cudaMemcpyHostToDevice, ctx->stream));
+    launch_update_table_map(ctx->stream, ctx->d_tab_map, reinterpret_cast<const uint2 *>(ctx->d_tab_upd), (uint32_t)n_set, ctx->d_tvv_shadow,
+                            reinterpret_cast<const uint32_t *>(ctx->d_tab_upd + set_bytes), (uint32_t)n_reset);
+    CU(cudaGetLastError());
+    CU(cudaEventRecord(ctx->ev_tab, ctx->stream));
+    touched.clear(); reset.clear();
+    return B200VIS_OK;
+}
+
+// b200vis_set_topology: every slot unmapped (the tables stay registered)
+static int32_t tables_unmap_all(b200vis_ctx *ctx) {
+    if (!ctx->tables_set) return B200VIS_OK;
+    std::fill(ctx->h_tab_map.begin(), ctx->h_tab_map.end(), kUnmapped);
+    std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
+    ctx->pend_touched.clear();                                // every entry is unmapped below
+    if (!ctx->h_tab_map.empty()) CU(cudaMemsetAsync(ctx->d_tab_map, 0xFF, ctx->h_tab_map.size() * 4, ctx->stream));
+    return B200VIS_OK;
+}
+
+// b200vis_edit_topology: the despawned rows leave their slots
+static int32_t tables_unmap_rows(b200vis_ctx *ctx, uint32_t n_rows, const uint32_t *rows) {
+    if (!ctx->tables_set) return B200VIS_OK;
+    std::vector<uint32_t> touched;
+    for (uint32_t i = 0; i < n_rows; ++i) {
+        const uint32_t r = rows[i];
+        if (r >= ctx->row_slot.size() || ctx->row_slot[r] == kUnmapped) continue;
+        ctx->h_tab_map[ctx->row_slot[r]] = kUnmapped;
+        touched.push_back(ctx->row_slot[r]);
+        ctx->row_slot[r] = kUnmapped;
+    }
+    queue_table_updates(ctx, touched, {});
+    return B200VIS_OK;
+}
+
+// b200vis_compact_topology, host side (the device maps are renumbered by the compaction's own kernels): every mapped row
+// is live, so it survives
+static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_to_new) {
+    if (!ctx->tables_set) return;
+    std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
+    for (size_t i = 0; i < ctx->h_tab_map.size(); ++i) {
+        uint32_t &r = ctx->h_tab_map[i];
+        if (r == kUnmapped) continue;
+        r = old_to_new[r];
+        ctx->row_slot[r] = (uint32_t)i;
+    }
+}
+
+extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_tables: world_size > 1");
+    if (n_tables && !tables) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: null tables");
+    if (n_tables > B200VIS_MAX_TABLES) return fail(ctx, B200VIS_ERR_CAPACITY, "set_tables: %u tables > %u", n_tables, B200VIS_MAX_TABLES);
+    uint64_t total = 0, chunks = 0;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        if (tables[t].len > tables[t].capacity)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u has len %u > capacity %u", t, tables[t].len, tables[t].capacity);
+        // the kernel stores float4 matrices and u32 ticks
+        if ((uintptr_t)tables[t].global_transforms % 16u || (uintptr_t)tables[t].gt_changed_ticks % 4u || (uintptr_t)tables[t].vv_changed_ticks % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u: GlobalTransform needs 16-byte, tick columns 4-byte alignment", t);
+        total += tables[t].capacity;
+        chunks += (tables[t].len + 127u) / 128u;
+    }
+    if (total > (1ull << 31)) return fail(ctx, B200VIS_ERR_CAPACITY, "set_tables: %llu slots in all > 2^31", (unsigned long long)total);
+    CU(cudaStreamSynchronize(ctx->stream));   // no write-back in flight reads the old registry or registrations
+    { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }   // queued entries index the current layout
+    const uint32_t n_old = (uint32_t)ctx->h_tabs.size();
+    auto moved = [&](uint32_t t) {            // table t's memory is not what it was (or t is new or gone)
+        if (t >= n_old || t >= n_tables) return true;
+        const b200vis_table &a = ctx->h_tabs[t], &b = tables[t];
+        return a.global_transforms != b.global_transforms || a.gt_changed_ticks != b.gt_changed_ticks ||
+               a.view_visibility != b.view_visibility || a.vv_changed_ticks != b.vv_changed_ticks || a.capacity != b.capacity;
+    };
+    // ---- the new maps: the entries below both capacities carry over ----
+    std::vector<uint32_t> off(n_tables), map((size_t)total, kUnmapped), reset;
+    bool same_layout = ctx->tables_set && n_tables == n_old;
+    for (uint32_t t = 0, o = 0; t < n_tables; o += tables[t].capacity, ++t) {
+        off[t] = o;
+        if (t >= n_old) continue;
+        const uint32_t keep = std::min(tables[t].capacity, ctx->h_tabs[t].capacity);
+        same_layout &= tables[t].capacity == ctx->h_tabs[t].capacity;
+        std::copy_n(ctx->h_tab_map.begin() + ctx->tab_off[t], keep, map.begin() + o);
+        if (tables[t].view_visibility != ctx->h_tabs[t].view_visibility)   // a new column: its bytes are sent again
+            for (uint32_t s = 0; s < keep; ++s) if (map[o + s] != kUnmapped) reset.push_back(map[o + s]);
+    }
+    // ---- registrations: page-rounded column ranges, overlapping ones merged; stale ones released before new ones ----
+    using Range = std::pair<uintptr_t, uintptr_t>;
+    const uintptr_t page = (uintptr_t)sysconf(_SC_PAGESIZE);
+    auto ours = [&](uintptr_t p) {
+        for (const auto &r : ctx->host_regs) if (p >= r.first && p < r.first + r.second) return true;
+        return false;
+    };
+    auto columns = [](const b200vis_table &tb, auto &&fn) {
+        const size_t cap = tb.capacity;
+        fn((void *)tb.global_transforms, cap * 64); fn((void *)tb.gt_changed_ticks, cap * 4);
+        fn((void *)tb.view_visibility, cap); fn((void *)tb.vv_changed_ticks, cap * 4);
+    };
+    auto rounded = [&](void *p, size_t bytes) { const uintptr_t a = (uintptr_t)p; return Range{a & ~(page - 1), (a + bytes + page - 1) & ~(page - 1)}; };
+    std::vector<Range> need, changed;
+    for (uint32_t t = 0; t < n_tables; ++t)
+        columns(tables[t], [&](void *p, size_t bytes) {
+            if (!p || !bytes) return;
+            if (moved(t)) changed.push_back(rounded(p, bytes));
+            void *d = nullptr;
+            if (!ours((uintptr_t)p) && cudaHostGetDevicePointer(&d, p, 0) == cudaSuccess) return;   // pinned by its owner
+            cudaGetLastError();
+            need.push_back(rounded(p, bytes));
+        });
+    for (uint32_t t = 0; t < n_old; ++t)
+        if (moved(t)) columns(ctx->h_tabs[t], [&](void *p, size_t bytes) { if (p && bytes) changed.push_back(rounded(p, bytes)); });
+    std::sort(need.begin(), need.end());
+    std::vector<Range> merged;
+    for (const Range &r : need) {
+        if (!merged.empty() && r.first < merged.back().second) merged.back().second = std::max(merged.back().second, r.second);
+        else merged.push_back(r);
+    }
+    std::vector<std::pair<uintptr_t, size_t>> regs;
+    ctx->n_tab_chunks = 0;   // until the new registry is committed, no write-back reaches a released range
+    for (const auto &r : ctx->host_regs) {
+        const uintptr_t lo = r.first, hi = r.first + r.second;
+        bool stale = std::find(merged.begin(), merged.end(), Range{lo, hi}) == merged.end();
+        for (const Range &c : changed) stale |= c.first < hi && lo < c.second;
+        if (stale) cudaHostUnregister(reinterpret_cast<void *>(lo));
+        else regs.push_back(r);
+    }
+    cudaGetLastError();
+    ctx->host_regs = regs;
+    for (const Range &r : merged) {
+        if (std::find(regs.begin(), regs.end(), std::make_pair(r.first, (size_t)(r.second - r.first))) != regs.end()) continue;
+        const cudaError_t e = cudaHostRegister(reinterpret_cast<void *>(r.first), r.second - r.first, cudaHostRegisterMapped | cudaHostRegisterPortable);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            for (const auto &q : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(q.first));
+            cudaGetLastError();
+            ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
+            std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
+            ctx->n_tab_chunks = 0;
+            return fail(ctx, B200VIS_ERR_CUDA, "set_tables: cudaHostRegister of %zu bytes at %p failed: %s", (size_t)(r.second - r.first),
+                        reinterpret_cast<void *>(r.first), cudaGetErrorString(e));
+        }
+        ctx->host_regs.emplace_back(r.first, (size_t)(r.second - r.first));
+    }
+    // ---- the device registry: table descriptors, chunk -> table, and the maps when their layout changed ----
+    std::vector<DevTable> dt(n_tables);
+    std::vector<uint32_t> chunk_table((size_t)chunks);
+    for (uint32_t t = 0, c = 0; t < n_tables; ++t) {
+        const b200vis_table &tb = tables[t];
+        void *alias[4] = {tb.global_transforms, tb.gt_changed_ticks, tb.view_visibility, tb.vv_changed_ticks};
+        for (void *&p : alias) if (p && tb.capacity) { void *d = nullptr; CU(cudaHostGetDevicePointer(&d, p, 0)); p = d; } else p = nullptr;
+        dt[t] = DevTable{static_cast<float4 *>(alias[0]), static_cast<uint32_t *>(alias[1]), static_cast<uint8_t *>(alias[2]),
+                         static_cast<uint32_t *>(alias[3]), tb.len, off[t], c, 0};
+        for (uint32_t k = 0; k < (tb.len + 127u) / 128u; ++k) chunk_table[c++] = t;
+    }
+    const size_t N = ctx->cfg.max_entities;
+    if (!ctx->d_tabs) CU(dalloc(&ctx->d_tabs, B200VIS_MAX_TABLES));
+    if (!ctx->d_tab_total) CU(dalloc(&ctx->d_tab_total, 1));
+    if (!ctx->d_tvv_shadow) { CU(dalloc(&ctx->d_tvv_shadow, N + 32)); CU(cudaMemset(ctx->d_tvv_shadow, 0xFF, N + 32)); }
+    if (chunks > ctx->tab_chunks_cap) {
+        if (ctx->d_tab_chunks) cudaFree(ctx->d_tab_chunks);
+        ctx->d_tab_chunks = nullptr; ctx->tab_chunks_cap = 0;
+        CU(dalloc(&ctx->d_tab_chunks, (size_t)chunks));
+        ctx->tab_chunks_cap = (uint32_t)chunks;
+    }
+    if (total > ctx->tab_map_cap) {
+        if (ctx->d_tab_map) cudaFree(ctx->d_tab_map);
+        ctx->d_tab_map = nullptr; ctx->tab_map_cap = 0;
+        CU(dalloc(&ctx->d_tab_map, (size_t)total));
+        ctx->tab_map_cap = (size_t)total;
+    }
+    cudaStream_t st = ctx->stream;
+    const uint32_t total32 = (uint32_t)total;
+    if (n_tables) CU(cudaMemcpyAsync(ctx->d_tabs, dt.data(), dt.size() * sizeof(DevTable), cudaMemcpyHostToDevice, st));
+    if (chunks) CU(cudaMemcpyAsync(ctx->d_tab_chunks, chunk_table.data(), (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
+    if (!same_layout && total) CU(cudaMemcpyAsync(ctx->d_tab_map, map.data(), (size_t)total * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(ctx->d_tab_total, &total32, 4, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    // ---- commit ----
+    ctx->h_tabs.assign(tables, tables + n_tables);
+    ctx->tab_off = std::move(off);
+    ctx->h_tab_map = std::move(map);
+    ctx->row_slot.assign(N, kUnmapped);
+    for (size_t i = 0; i < ctx->h_tab_map.size(); ++i) if (ctx->h_tab_map[i] != kUnmapped) ctx->row_slot[ctx->h_tab_map[i]] = (uint32_t)i;
+    ctx->n_tab_chunks = (uint32_t)chunks;
+    ctx->tables_set = true;
+    queue_table_updates(ctx, {}, reset);
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uint32_t first_slot, uint32_t count, const uint32_t *rows) {
+    CHECK_CTX();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_table_rows: world_size > 1");
+    if (table >= ctx->h_tabs.size()) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_rows: table %u of %zu", table, ctx->h_tabs.size());
+    if ((uint64_t)first_slot + count > ctx->h_tabs[table].capacity)
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_rows: slots [%u, %llu) past table %u's capacity %u", first_slot,
+                    (unsigned long long)first_slot + count, table, ctx->h_tabs[table].capacity);
+    if (count && !rows) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_rows: null rows");
+    const Plan *hp = ctx->topology_set ? ctx->hplan : nullptr;
+    for (uint32_t i = 0; i < count; ++i) {
+        const uint32_t r = rows[i];
+        if (r != kUnmapped && (!hp || r >= ctx->n || !hp->alive[r]))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_rows: row %u (slot %u) is out of range or despawned", r, first_slot + i);
+    }
+    std::vector<uint32_t> touched, reset;
+    const uint32_t base = ctx->tab_off[table] + first_slot;
+    for (uint32_t i = 0; i < count; ++i) {
+        const uint32_t e = base + i, r = rows[i], old = ctx->h_tab_map[e];
+        if (old == r) continue;
+        if (old != kUnmapped) ctx->row_slot[old] = kUnmapped;
+        if (r != kUnmapped) {
+            const uint32_t prev = ctx->row_slot[r];
+            if (prev != kUnmapped) { ctx->h_tab_map[prev] = kUnmapped; touched.push_back(prev); }
+            ctx->row_slot[r] = e;
+            reset.push_back(r);          // a new slot: what it holds is unknown
+        }
+        ctx->h_tab_map[e] = r;
+        touched.push_back(e);
+    }
+    queue_table_updates(ctx, touched, reset);
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick) {
+    CHECK_CTX();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "writeback_tables: world_size > 1");
+    if (!ctx->tables_set) return fail(ctx, B200VIS_ERR_NOT_READY, "writeback_tables: call b200vis_set_tables first");
+    { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }
+    // on the main stream, right behind the tile pass, like the column write-back
+    const TableBufs tb{ctx->d_tabs, ctx->d_tab_chunks, ctx->n_tab_chunks, ctx->d_tab_map, ctx->d_tvv_shadow};
+    launch_writeback_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_WB_GLOBAL_TRANSFORM | B200VIS_WB_VIEW_VISIBILITY), gt_tick, vv_tick);
     CU(cudaGetLastError());
     return B200VIS_OK;
 }

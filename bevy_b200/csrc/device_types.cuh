@@ -264,6 +264,23 @@ struct RowEdit {
     float2 *range_se;
 };
 
+// b200vis_set_tables: one registered archetype table as k_writeback_tables sees it (device aliases of the caller's columns,
+// nullptr = not delivered)
+struct DevTable {
+    float4 *gt; uint32_t *gt_ticks; uint8_t *vv; uint32_t *vv_ticks;
+    uint32_t len;            // slots [0, len) are written
+    uint32_t map_off;        // the table's slot -> row map starts at TableBufs::map[map_off]
+    uint32_t chunk_begin;    // the table's first 128-slot chunk in the launch's chunk numbering
+    uint32_t pad;
+};
+struct TableBufs {
+    const DevTable *tables;
+    const uint32_t *chunk_table;   // [n_chunks] the table each chunk belongs to (built on the host when the registry changes)
+    uint32_t n_chunks;
+    const uint32_t *map;           // slot -> row of every table, 0xFFFFFFFF = unmapped
+    uint8_t *vv_shadow;            // per row: the ViewVisibility byte its slot holds (0xFF = unknown)
+};
+
 // b200vis_compact_topology: row-valued lists (list l = rows[l * stride .. + count[l * count_step]))
 struct RowLists {
     uint32_t *rows;

@@ -3022,6 +3022,34 @@ __global__ void k_publish_clusters(const FrameConsts *__restrict__ fc, const uin
 // bit sets, a ViewVisibility word crosses PCIe only when one of its four bytes differs from what the host already holds
 // (device-side shadow), and the changed rows' matrices are transposed through shared memory so that every store
 // instruction covers up to 512 contiguous bytes of the host column (whole PCIe write bursts).
+//
+// The changed rows of one 32-entry group of a host column: lane `lane` (when bit lane of gbits is set) transposes `row`'s
+// matrix into the warp's shared slab s_w in the host layout, then the warp stores the group's changed entries to dst
+// (entry 0 of the group), consecutive lanes to consecutive 16-byte pieces.
+template <int STRIDE>
+__device__ __forceinline__ void store_changed_affines(const Rows &R, uint32_t row, uint32_t gbits, uint32_t lane, float4 *s_w,
+                                                      float4 *dst) {
+    constexpr int Q = STRIDE / 4;                             // float4 per row in the host layout
+    if ((gbits >> lane) & 1u) {
+        const float4 a = R.gt0[row], b = R.gt1[row], c = R.gt2[row];
+        float4 *o = &s_w[lane * Q];
+        if (STRIDE == 16) {                                   // glam Affine3A: x_axis, y_axis, z_axis, translation as Vec3A
+            o[0] = make_float4(a.x, b.x, c.x, 0.0f); o[1] = make_float4(a.y, b.y, c.y, 0.0f);
+            o[2] = make_float4(a.z, b.z, c.z, 0.0f); o[3] = make_float4(a.w, b.w, c.w, 0.0f);
+        } else {                                              // packed X.xyz Y.xyz Z.xyz T.xyz
+            o[0] = make_float4(a.x, b.x, c.x, a.y); o[1] = make_float4(b.y, c.y, a.z, b.z);
+            o[2] = make_float4(c.z, a.w, b.w, c.w);
+        }
+    }
+    __syncwarp();
+#pragma unroll
+    for (int k = 0; k < Q; ++k) {
+        const uint32_t idx = k * 32u + lane;                  // consecutive lanes -> consecutive 16-byte pieces of the column
+        if ((gbits >> (idx / Q)) & 1u) dst[idx] = s_w[idx];
+    }
+    __syncwarp();
+}
+
 template <int STRIDE>
 __global__ void __launch_bounds__(256)
 k_writeback_columns(Rows R, float *__restrict__ host_gt, uint32_t *__restrict__ host_gt_bits, uint8_t *__restrict__ host_vv,
@@ -3059,28 +3087,52 @@ k_writeback_columns(Rows R, float *__restrict__ host_gt, uint32_t *__restrict__ 
         for (uint32_t j = 0; j < 4; ++j) {
             const uint32_t gbits = __shfl_sync(0xFFFFFFFFu, g, j * 8u);
             if (!gbits) continue;
-            const uint32_t row = grp * 128u + j * 32u + lane;
-            if ((gbits >> lane) & 1u) {
-                const float4 a = R.gt0[row], b = R.gt1[row], c = R.gt2[row];
-                float4 *o = &s_t[warp][lane * Q];
-                if (STRIDE == 16) {                           // glam Affine3A: x_axis, y_axis, z_axis, translation as Vec3A
-                    o[0] = make_float4(a.x, b.x, c.x, 0.0f); o[1] = make_float4(a.y, b.y, c.y, 0.0f);
-                    o[2] = make_float4(a.z, b.z, c.z, 0.0f); o[3] = make_float4(a.w, b.w, c.w, 0.0f);
-                } else {                                      // packed X.xyz Y.xyz Z.xyz T.xyz
-                    o[0] = make_float4(a.x, b.x, c.x, a.y); o[1] = make_float4(b.y, c.y, a.z, b.z);
-                    o[2] = make_float4(c.z, a.w, b.w, c.w);
-                }
-            }
-            __syncwarp();
-            float4 *dst = reinterpret_cast<float4 *>(host_gt) + ((size_t)grp * 128u + j * 32u) * Q;
-#pragma unroll
-            for (int k = 0; k < Q; ++k) {
-                const uint32_t idx = k * 32u + lane;          // consecutive lanes -> consecutive 16-byte pieces of the column
-                if ((gbits >> (idx / Q)) & 1u) dst[idx] = s_t[warp][idx];
-            }
-            __syncwarp();
+            store_changed_affines<STRIDE>(R, grp * 128u + j * 32u + lane, gbits, lane, s_t[warp],
+                                          reinterpret_cast<float4 *>(host_gt) + ((size_t)grp * 128u + j * 32u) * Q);
         }
     }
+}
+
+// ---- table write-back: the same results into the caller's archetype tables (b200vis_set_tables), each walked in its own
+// slot order.  One warp per 128-slot chunk of a table, 32 slots at a time: each lane gathers its slot's row through the
+// slot -> row map, then the stores go to consecutive slots -- matrices through the shared-memory transpose above (up to 512
+// contiguous bytes per store instruction however the rows are shuffled), ticks as contiguous 4-byte stores masked by the
+// change bit, ViewVisibility bytes where they differ from what the slot is known to hold (per-row shadow).
+__global__ void __launch_bounds__(256)
+k_writeback_tables(Rows R, TableBufs tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick) {
+    __shared__ float4 s_t[8][32 * 4];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const bool wgt = which & 1u, wvv = which & 2u;
+    for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
+        const DevTable T = tb.tables[tb.chunk_table[ch]];
+        const uint32_t base = (ch - T.chunk_begin) * 128u;
+#pragma unroll 1
+        for (uint32_t j = 0; j < 4u; ++j) {
+            const uint32_t s0 = base + j * 32u, slot = s0 + lane;
+            if (s0 >= T.len) break;                           // the same for the whole warp
+            const uint32_t row = slot < T.len ? tb.map[T.map_off + slot] : kNoParent;
+            const uint32_t st8 = row != kNoParent ? R.state[row] : 0u;
+            const bool gch = wgt && (st8 & S_GT_CHANGED);
+            if (wgt && T.gt != nullptr) {
+                const uint32_t gbits = __ballot_sync(0xFFFFFFFFu, gch);
+                if (gbits) store_changed_affines<16>(R, row, gbits, lane, s_t[warp], T.gt + (size_t)s0 * 4u);
+            }
+            if (gch && T.gt_ticks != nullptr) T.gt_ticks[slot] = gt_tick;
+            if (wvv && row != kNoParent) {
+                const uint8_t vv = (uint8_t)(st8 & S_VV);
+                if (T.vv != nullptr && tb.vv_shadow[row] != vv) { T.vv[slot] = vv; tb.vv_shadow[row] = vv; }
+                if (T.vv_ticks != nullptr && (st8 & S_VV_CHANGED)) T.vv_ticks[slot] = vv_tick;
+            }
+        }
+    }
+}
+
+__global__ void __launch_bounds__(256) k_update_table_map(uint32_t *__restrict__ map, const uint2 *__restrict__ set, uint32_t n_set,
+                                                          uint8_t *__restrict__ vv_shadow, const uint32_t *__restrict__ reset,
+                                                          uint32_t n_reset) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_set) map[set[i].x] = set[i].y;
+    if (i < n_reset) vv_shadow[reset[i]] = 0xFF;
 }
 
 // zero this rank's slab for the next frame's assign kernel (only the words in use)
@@ -3933,6 +3985,16 @@ void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, ui
     const unsigned groups = cdiv(R.n, 128), grid = groups < 8u * 1184u ? cdiv(groups, 8) : 1184u;
     if (stride == 16) { ++g_launches; k_writeback_columns<16><<<grid, 256, 0, st>>>(R, host_gt, host_gt_bits, host_vv, host_vv_bits, vv_shadow); }
     else { ++g_launches; k_writeback_columns<12><<<grid, 256, 0, st>>>(R, host_gt, host_gt_bits, host_vv, host_vv_bits, vv_shadow); }
+}
+void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick) {
+    if (!tb.n_chunks) return;
+    const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
+    ++g_launches; k_writeback_tables<<<grid, 256, 0, st>>>(R, tb, which, gt_tick, vv_tick);
+}
+void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
+                             uint32_t n_reset) {
+    const uint32_t n = std::max(n_set, n_reset);
+    if (n) { ++g_launches; k_update_table_map<<<cdiv(n, 256), 256, 0, st>>>(map, set, n_set, vv_shadow, reset, n_reset); }
 }
 void launch_record_push(cudaStream_t st, const uint32_t *block, uint32_t block_words, const ClusterBufs &cb) {
     ++g_launches; k_record_push<<<cb.world, 256, 0, st>>>(block, block_words, cb);

@@ -47,6 +47,10 @@ void launch_tag_lights(cudaStream_t st, const Rows &R, const Lights &L, uint32_t
 void launch_snapshot_lights(cudaStream_t st, const Rows &R, const Lights &L, float4 *snap);
 void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, uint32_t stride, uint32_t *host_gt_bits, uint8_t *host_vv,
                               uint32_t *host_vv_bits, uint8_t *vv_shadow);
+void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
+// set_table_rows / set_tables / edit_topology: map[set[i].x] = set[i].y, then vv_shadow[reset[i]] = 0xFF
+void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
+                             uint32_t n_reset);
 void launch_record_push(cudaStream_t st, const uint32_t *block, uint32_t block_words, const ClusterBufs &cb);
 void launch_slab_push(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, uint32_t *done, uint32_t max_views);
 void launch_cluster_lists(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, DevStats *stats, uint32_t max_views);

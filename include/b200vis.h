@@ -461,6 +461,58 @@ B200VIS_API int32_t b200vis_writeback_columns(b200vis_ctx *ctx);
 B200VIS_API int32_t b200vis_writeback_columns_ex(b200vis_ctx *ctx, uint32_t which);
 #define B200VIS_STEP_WRITEBACK 0x2u  /* b200vis_step: enqueue the column write-back right behind the tile pass */
 
+/* ---- write-back straight into the caller's archetype tables -------------------------------------------------------------
+ * In Bevy, GlobalTransform and ViewVisibility live in one column per archetype table, each in the table's own slot order
+ * (crates/bevy_ecs/src/storage/table/mod.rs), and a hierarchy spans several tables (roots, inner nodes and leaves differ in
+ * ChildOf / Children).  A table registry lets the GPU write every result, and the change tick itself, into those columns:
+ * b200vis_writeback_tables walks each table in slot order and gathers each slot's row through a slot -> row map that lives
+ * on the device.
+ *   global_transforms  [capacity] glam Affine3A, 64 B per slot: ONLY slots whose row's GlobalTransform changed this frame
+ *                      are written (the set_if_neq rule of the column sinks), padding lanes as 0
+ *   gt_changed_ticks   [capacity] GlobalTransform's changed_ticks column: gt_tick where that write happened
+ *   view_visibility    [capacity] the ViewVisibility byte, written where it differs from what the slot is known to hold
+ *   vv_changed_ticks   [capacity] vv_tick exactly where Changed<ViewVisibility> fires
+ * Any column may be NULL (not delivered / not stamped).  Only slots [0, len) that are mapped to a live row are ever
+ * written; every other byte and tick keeps its value.  The library registers the page-rounded [0, capacity) ranges of
+ * memory that is not pinned (cudaHostRegister, mapped; overlapping ranges of different tables become one registration),
+ * owns those registrations and releases them when a table's columns or capacity change and in b200vis_destroy.  Memory
+ * that is already pinned by its owner is used through its device alias.  A registration covers whole pages, so other
+ * allocations on those pages are page-locked with it, and a CUDA copy from pageable memory that lies only partly inside a
+ * registered range can fail with cudaErrorInvalidValue: small tables are best allocated from page-aligned memory that owns
+ * its pages.  world_size > 1: UNSUPPORTED. */
+#define B200VIS_MAX_TABLES 4096u
+typedef struct b200vis_table {
+    void     *global_transforms;  /* [capacity] GlobalTransform (Affine3A, 64 B per slot); NULL = not delivered */
+    uint32_t *gt_changed_ticks;   /* [capacity] Tick (u32); NULL = not stamped */
+    uint8_t  *view_visibility;    /* [capacity]; NULL = not delivered */
+    uint32_t *vv_changed_ticks;   /* [capacity] */
+    uint32_t  len;                /* Table::entity_count: only slots [0, len) are ever written */
+    uint32_t  capacity;           /* Table::capacity: the extent that is registered */
+} b200vis_table;
+/* Replaces the registry: table t of the call is table t from then on.  The slot maps of tables that stay keep their
+ * entries below the new capacity; slots at or past it, and the tables past n_tables, are unmapped.  When a table's
+ * view_visibility column moves, its slots are sent their ViewVisibility byte again by the next write-back.
+ * n_tables == 0 empties the registry.  Errors: INVALID_ARG (len > capacity, a global_transforms column not 16-byte aligned,
+ * a ticks column not 4-byte aligned), CAPACITY (more than B200VIS_MAX_TABLES tables, or more than 2^31 slots in all), UNSUPPORTED (world_size > 1); nothing
+ * changes then.  On B200VIS_ERR_CUDA (cudaHostRegister refused the memory) the registry is left empty. */
+B200VIS_API int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables);
+/* Maps slots [first_slot, first_slot + count) of `table` to rows[i] (B200VIS_UNMAPPED = unmapped), in order.  The call does
+ * not wait for the stream: map changes are queued and reach the device as one batch at the next write-back.  Mapping row r
+ * to (table, slot) removes r's previous mapping, and the row that slot held before becomes unmapped: an archetype move, or
+ * the swap_remove behind it (table/mod.rs), is one or two such calls.  All or nothing.  Errors: INVALID_ARG (a table out of
+ * range, slots past the table's capacity, a row out of range or despawned, a null rows with count > 0), UNSUPPORTED
+ * (world_size > 1).
+ * Rows move with the world: b200vis_set_topology unmaps every slot (the tables stay registered), b200vis_edit_topology unmaps
+ * the rows it despawns, b200vis_compact_topology renumbers the maps itself (the caller does nothing to its tables). */
+#define B200VIS_UNMAPPED 0xFFFFFFFFu
+B200VIS_API int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uint32_t first_slot, uint32_t count,
+                                           const uint32_t *rows);
+/* Enqueues the write-back of `which` (B200VIS_WB_*) on the context's stream, behind the frame's tile pass, like
+ * b200vis_writeback_columns_ex; the results are complete after b200vis_synchronize.  gt_tick / vv_tick = the tick stamped
+ * into the changed_ticks columns (the writing system's this_run).  Errors: NOT_READY (no b200vis_set_tables yet),
+ * UNSUPPORTED (world_size > 1). */
+B200VIS_API int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
+
 /* ---- SURVEY.md 8(f) N1: the render world's visible-entity diff ---------------------------------------------
  * RenderVisibleEntitiesClass::update_cpu_culled_entities (crates/bevy_render/src/view/visibility/mod.rs:194-249)
  * marches over last frame's and this frame's sorted list to find the newly added and newly removed entities.  With

@@ -16,12 +16,16 @@
 //! ViewVisibility bytes + change bits can be written straight into the column instead (`forked-bevy` feature below).
 //!
 //! Data flow (INTEGRATION.md section 2): ECS columns -> `upload_*` on change; results -> pinned host buffers the GPU
-//! writes itself (`b200vis_set_result_sink`, `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system.
+//! writes itself (`b200vis_set_result_sink`, `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system;
+//! GlobalTransform (and, forked, ViewVisibility) with their change ticks straight into the archetype tables
+//! (`b200vis_set_tables`, `b200vis_writeback_tables`).
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
 use bevy::camera::primitives::{Aabb, Frustum, Sphere};
 use bevy::camera::visibility::*;
+use bevy::ecs::component::Tick;
 use bevy::ecs::entity::EntityHashMap;
 use bevy::ecs::schedule::ScheduleCleanupPolicy::RemoveSystemsOnly;
+use bevy::ecs::system::SystemChangeTick;
 use bevy::light::{cluster::*, PointLight, SimulationLightSystems};
 use bevy::prelude::*;
 use bevy::transform::{systems::*, TransformSystems};
@@ -49,6 +53,9 @@ pub struct b200vis_cluster_feedback { has_farthest_z: u32, farthest_z: f32, has_
     visible_classes: *mut u8, cluster_offsets: *mut u32, cluster_indices: *mut u32, cluster_capacity: u32 }
 #[repr(C)] pub struct b200vis_column_sinks { global_transforms: *mut f32, gt_stride_floats: u32, gt_changed_bits: *mut u32,
     view_visibility: *mut u8, vv_changed_bits: *mut u32 }
+#[repr(C)] #[derive(Clone, Copy, PartialEq)]
+pub struct b200vis_table { global_transforms: *mut GlobalTransform, gt_changed_ticks: *mut Tick, view_visibility: *mut ViewVisibility,
+    vv_changed_ticks: *mut Tick, len: u32, capacity: u32 }
 
 #[link(name = "b200vis")]
 extern "C" {
@@ -77,10 +84,13 @@ extern "C" {
     fn b200vis_set_view_stats_sink(ctx: *mut b200vis_ctx, per_view: *mut [u32; 4]) -> i32;
     fn b200vis_set_column_sinks(ctx: *mut b200vis_ctx, sinks: *const b200vis_column_sinks) -> i32;
     fn b200vis_writeback_columns_ex(ctx: *mut b200vis_ctx, which: u32) -> i32;
+    fn b200vis_set_tables(ctx: *mut b200vis_ctx, n: u32, tables: *const b200vis_table) -> i32;
+    fn b200vis_set_table_rows(ctx: *mut b200vis_ctx, table: u32, first_slot: u32, count: u32, rows: *const u32) -> i32;
+    fn b200vis_writeback_tables(ctx: *mut b200vis_ctx, which: u32, gt_tick: u32, vv_tick: u32) -> i32;
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
-const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2;
+const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2; const UNMAPPED: u32 = 0xFFFF_FFFF;
 const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04; const F_NO_FRUSTUM: u8 = 0x08;
 const F_RANGE: u8 = 0x10; const F_SPHERE_FROM_GT: u8 = 0x40;
 const VIEW_ACTIVE: u8 = 1; const VIEW_NO_CPU_CULLING: u8 = 2;
@@ -107,9 +117,12 @@ pub struct B200Vis {
     stats: Box<b200vis_frame_stats>,
     view_stats: Vec<[u32; 4]>,    // every view: visible_count, cluster_index_count, cluster_farthest_z bits, overflow
     max_views: usize,
-    gt_col: Vec<[f32; 16]>, gt_bits: Vec<u32>, vv_col: Vec<u8>, vv_bits: Vec<u32>,
+    vv_col: Vec<u8>, vv_bits: Vec<u32>,
     visible_rows: Vec<u32>, visible_classes: Vec<u8>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
     planes_scratch: Vec<f32>,
+    // the archetype tables registered with b200vis_set_tables (one entry per table holding GlobalTransform, with its
+    // ViewVisibility column in the forked build), the entities each slot map was built from, and the rows epoch of the maps
+    tables: Vec<b200vis_table>, table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -148,16 +161,18 @@ impl Plugin for B200VisibilityPlugin {
         let mut vis = B200Vis {
             ctx, max_entities: n, n: 0, row_of: Default::default(), entity_of: Vec::new(), columns_epoch: 0, bounds_epoch: u64::MAX,
             lights_epoch: u64::MAX, classes: Vec::new(), view_entities: Vec::new(), light_entities: Vec::new(),
-            stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, gt_col: vec![[0.0; 16]; n], gt_bits: vec![0; n.div_ceil(32)], vv_col: vec![0; n],
+            stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, vv_col: vec![0; n],
             vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; max_views * n], visible_classes: vec![0; max_views * n],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
-            planes_scratch: vec![0.0; 3 * 4097 * 4],
+            planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_entities: Vec::new(), maps_epoch: u64::MAX,
         };
         let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: vis.visible_rows.as_mut_ptr(), visible_capacity: n as u32,
             visible_classes: vis.visible_classes.as_mut_ptr(), cluster_offsets: vis.cluster_offsets.as_mut_ptr(),
             cluster_indices: vis.cluster_indices.as_mut_ptr(), cluster_capacity: cluster_cap as u32 };
-        let cs = b200vis_column_sinks { global_transforms: vis.gt_col.as_mut_ptr().cast(), gt_stride_floats: 16,
-            gt_changed_bits: vis.gt_bits.as_mut_ptr(), view_visibility: vis.vv_col.as_mut_ptr(), vv_changed_bits: vis.vv_bits.as_mut_ptr() };
+        // GlobalTransform goes straight into the archetype tables (b200vis_set_tables); the column sink carries the
+        // ViewVisibility bytes the unforked cull turns into set_visible() calls
+        let cs = b200vis_column_sinks { global_transforms: core::ptr::null_mut(), gt_stride_floats: 16,
+            gt_changed_bits: core::ptr::null_mut(), view_visibility: vis.vv_col.as_mut_ptr(), vv_changed_bits: vis.vv_bits.as_mut_ptr() };
         unsafe {
             assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_column_sinks(ctx, &cs), 0);
             assert_eq!(b200vis_set_view_stats_sink(ctx, vis.view_stats.as_mut_ptr()), 0);   // per-view stats of every view
@@ -172,12 +187,12 @@ impl Plugin for B200VisibilityPlugin {
             app.remove_systems_in_set(schedule, mark_dirty_trees, RemoveSystemsOnly);
             app.remove_systems_in_set(schedule, propagate_parent_transforms, RemoveSystemsOnly);
             app.remove_systems_in_set(schedule, sync_simple_transforms, RemoveSystemsOnly);
-            app.add_systems(schedule, b200_propagate.in_set(TransformSystems::Propagate));
+            app.add_systems(schedule, (b200_sync_tables, b200_propagate).chain().in_set(TransformSystems::Propagate));
         }
         app.remove_systems_in_set(PostUpdate, check_visibility_cpu_culling, RemoveSystemsOnly);
         app.remove_systems_in_set(PostUpdate, SimulationLightSystems::AssignLightsToClusters, RemoveSystemsOnly);
         app.add_systems(PostUpdate, (
-            b200_check_visibility.in_set(VisibilitySystems::CheckVisibility),
+            (b200_sync_tables, b200_check_visibility).chain().in_set(VisibilitySystems::CheckVisibility),
             b200_assign_lights_to_clusters.in_set(SimulationLightSystems::AssignLightsToClusters)
                 .after(TransformSystems::Propagate).after(VisibilitySystems::CheckVisibility),
         ));
@@ -194,22 +209,10 @@ fn pack_gt12(g: &GlobalTransform, out: &mut Vec<f32>) {
                             a.matrix3.y_axis.z, a.matrix3.z_axis.x, a.matrix3.z_axis.y, a.matrix3.z_axis.z, a.translation.x,
                             a.translation.y, a.translation.z]);
 }
-fn affine_from_col(m: &[f32; 16]) -> GlobalTransform {
-    // the sink's layout IS glam's Affine3A: x_axis, y_axis, z_axis, translation as four 16-byte Vec3A lanes
-    GlobalTransform::from(bevy::math::Affine3A::from_cols(
-        bevy::math::Vec3A::new(m[0], m[1], m[2]), bevy::math::Vec3A::new(m[4], m[5], m[6]),
-        bevy::math::Vec3A::new(m[8], m[9], m[10]), bevy::math::Vec3A::new(m[12], m[13], m[14])))
-}
-fn set_bits(words: &[u32], n: usize) -> impl Iterator<Item = usize> + '_ {
-    words.iter().enumerate().flat_map(move |(w, &bits)| {
-        let mut b = bits;
-        core::iter::from_fn(move || { if b == 0 { None } else { let k = b.trailing_zeros() as usize; b &= b - 1; Some(w * 32 + k) } })
-    }).filter(move |r| *r < n)
-}
-
 /// propagate: the data propagate_parent_transforms' queries (systems.rs:506-520) and sync_simple_transforms'
 /// (systems.rs:42-55) read and write, as one query.
 fn b200_propagate(
+    this_run: SystemChangeTick,
     mut vis: ResMut<B200Vis>,
     mut q: Query<(Entity, Ref<Transform>, &mut GlobalTransform, Option<&Children>, Option<&ChildOf>)>,
     structure_changed: Query<(), Or<(Added<GlobalTransform>, Changed<ChildOf>)>>,
@@ -241,8 +244,6 @@ fn b200_propagate(
         for e in &vis.entity_of {
             let (_, t, g, _, _) = q.get(*e).unwrap();
             pack_trs(&t, &mut trs); pack_gt12(&g, &mut gt);
-            vis.gt_col[vis.row_of[e] as usize] = { let mut m = [0.0; 16]; let a = g.affine().to_cols_array(); // 12 floats, column major
-                m[0..3].copy_from_slice(&a[0..3]); m[4..7].copy_from_slice(&a[3..6]); m[8..11].copy_from_slice(&a[6..9]); m[12..15].copy_from_slice(&a[9..12]); m };
         }
         // upload_transforms marks every row Changed<Transform>: the first propagate visits everything, like Added<GlobalTransform>
         vis.check(unsafe { b200vis_upload_transforms(vis.ctx, 0, n as u32, trs.as_ptr()) })?;
@@ -267,32 +268,83 @@ fn b200_propagate(
         }
         if !grows.is_empty() {
             vis.check(unsafe { b200vis_write_global_transforms_scattered(vis.ctx, grows.len() as u32, grows.as_ptr(), gts.as_ptr()) })?;
-            for (&r, g) in grows.iter().zip(gts.chunks(12)) {      // the host mirror holds what the other system wrote
-                let mut m = [0.0; 16];
-                m[0..3].copy_from_slice(&g[0..3]); m[4..7].copy_from_slice(&g[3..6]); m[8..11].copy_from_slice(&g[6..9]); m[12..15].copy_from_slice(&g[9..12]);
-                vis.gt_col[r as usize] = m;
-            }
         }
     }
+    // the registry b200_sync_tables left is current for this frame's tables; a rebuild above renumbered the rows and
+    // b200vis_set_topology unmapped every slot, so the maps are sent again
+    if rebuild { send_table_maps(vis, None)?; }
     unsafe {
         vis.check(b200vis_set_static_transform_optimizations(vis.ctx, opts.is_enabled() as i32))?;
         vis.check(b200vis_run(vis.ctx, STAGE_PROPAGATE))?;
-        vis.check(b200vis_writeback_columns_ex(vis.ctx, WB_GLOBAL_TRANSFORM))?;      // changed rows only, straight into gt_col
+        // the changed matrices into the tables, each stamped with this run's tick (set_if_neq semantics, systems.rs:719:
+        // what assigning through `Mut` does, change_detection/params.rs:1093-1135)
+        vis.check(b200vis_writeback_tables(vis.ctx, WB_GLOBAL_TRANSFORM, this_run.this_run().get(), 0))?;
         vis.check(b200vis_synchronize(vis.ctx))?;
     }
-    // set_if_neq semantics (systems.rs:719): only the rows whose bits changed are written, and exactly those get their
-    // change tick stamped (assigning through `Mut` does both).  When the table rows happen to be in device-row order the
-    // same can be done in bulk: `q.contiguous_iter_mut()` -> `ContiguousMut::bypass_change_detection()` as the column sink
-    // itself and `changed_ticks_slice_mut()[r] = this_run_tick()` per set bit (change_detection/params.rs:1079-1142).
-    for r in set_bits(&vis.gt_bits, vis.n) {
-        if let Ok((_, _, mut g, _, _)) = q.get_mut(vis.entity_of[r]) { *g = affine_from_col(&vis.gt_col[r]); }
+    Ok(())
+}
+
+/// The table registry (INTEGRATION.md section 2): one entry per archetype table that holds GlobalTransform -- that column and
+/// its changed ticks, and in the forked build the table's ViewVisibility column and ticks -- read from
+/// `World::storages().tables` with `Table::entity_count` / `Table::capacity` (storage/table/mod.rs).  Exclusive and chained
+/// right before each write-back system, so no table moves between the registration and the write-back that uses it.  The
+/// registry is replaced when a table's pointers, len or capacity changed; a table's slot -> row map is sent again when its
+/// entity list differs from the one the map was built from (an archetype move or swap_remove reorders slots without changing
+/// len) or the rows were renumbered.  Bevy never removes a table, so a table keeps its index in the registry.
+fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
+    let Some(gt_id) = world.component_id::<GlobalTransform>() else { return Ok(()) };
+    #[cfg(feature = "forked-bevy")]
+    let vv_id = world.component_id::<ViewVisibility>();
+    #[cfg(not(feature = "forked-bevy"))]
+    let vv_id: Option<bevy::ecs::component::ComponentId> = None;
+    world.resource_scope(|world, mut vis: Mut<B200Vis>| {
+        let vis = &mut *vis;
+        let (mut descs, mut entities) = (Vec::new(), Vec::new());
+        for table in world.storages().tables.iter() {
+            if !table.has_column(gt_id) { continue; }
+            // SAFETY: the columns hold GlobalTransform / ViewVisibility.  Only raw pointers are kept; the GPU writes through
+            // them inside the write-back systems, which hold the only access to those columns while they run.
+            let gt = unsafe { table.get_data_slice_for::<GlobalTransform>(gt_id) }.unwrap();
+            let gt_ticks = table.get_changed_ticks_slice_for(gt_id).unwrap();
+            let (vv, vv_ticks) = match vv_id.filter(|id| table.has_column(*id)) {
+                Some(id) => (unsafe { table.get_data_slice_for::<ViewVisibility>(id) }.unwrap().as_ptr() as *mut ViewVisibility,
+                             table.get_changed_ticks_slice_for(id).unwrap().as_ptr() as *mut Tick),
+                None => (core::ptr::null_mut(), core::ptr::null_mut()),
+            };
+            descs.push(b200vis_table { global_transforms: gt.as_ptr() as *mut GlobalTransform, gt_changed_ticks: gt_ticks.as_ptr() as *mut Tick,
+                                       view_visibility: vv, vv_changed_ticks: vv_ticks, len: table.entity_count(),
+                                       capacity: table.capacity() as u32 });
+            entities.push(table.entities());
+        }
+        if descs != vis.tables {
+            vis.check(unsafe { b200vis_set_tables(vis.ctx, descs.len() as u32, descs.as_ptr()) })?;
+            vis.tables = descs;
+        }
+        let renumbered = vis.maps_epoch != vis.columns_epoch;
+        let stale: Vec<bool> = entities.iter().enumerate()
+            .map(|(t, e)| renumbered || vis.table_entities.get(t).map_or(true, |old| old.as_slice() != *e)).collect();
+        vis.table_entities = entities.iter().map(|e| e.to_vec()).collect();
+        send_table_maps(vis, Some(&stale))
+    })
+}
+
+/// b200vis_set_table_rows for every table (`only` = None) or the tables marked in `only`: slot s -> the row of the entity
+/// in it, B200VIS_UNMAPPED for an entity without a row (GlobalTransform without Transform).  The calls only queue the
+/// changes; they reach the device with the next write-back.
+fn send_table_maps(vis: &mut B200Vis, only: Option<&[bool]>) -> Result<(), BevyError> {
+    for (t, entities) in vis.table_entities.iter().enumerate() {
+        if only.is_some_and(|o| !o[t]) { continue; }
+        let rows: Vec<u32> = entities.iter().map(|e| vis.row_of.get(e).copied().unwrap_or(UNMAPPED)).collect();
+        vis.check(unsafe { b200vis_set_table_rows(vis.ctx, t as u32, 0, rows.len() as u32, rows.as_ptr()) })?;
     }
+    vis.maps_epoch = vis.columns_epoch;
     Ok(())
 }
 
 /// cull: the parameter list of check_visibility_cpu_culling (visibility/mod.rs:748-774); `Ref` instead of `&` where the shim
 /// needs change detection for its column mirror.
 fn b200_check_visibility(
+    this_run: SystemChangeTick,
     mut vis: ResMut<B200Vis>,
     mut view_query: Query<(Entity, &mut VisibleEntities, &Frustum, Option<&RenderLayers>, &Camera, Has<NoCpuCulling>)>,
     mut visible_aabb_query: Query<(Entity, Ref<InheritedVisibility>, &mut ViewVisibility, Option<Ref<VisibilityClass>>, Option<Ref<RenderLayers>>,
@@ -361,9 +413,14 @@ fn b200_check_visibility(
           vis.check(unsafe { b200vis_upload_view_visibility(vis.ctx, 0, n as u32, vv.as_ptr()) })?; }
         vis.bounds_epoch = vis.columns_epoch;
     }
+    // forked: the tables b200_sync_tables registered carry the ViewVisibility columns too; they receive the bytes and, where
+    // Changed<ViewVisibility> fires, this run's tick
     unsafe {
         vis.check(b200vis_run(vis.ctx, STAGE_CULL))?;
+        #[cfg(not(feature = "forked-bevy"))]
         vis.check(b200vis_writeback_columns_ex(vis.ctx, WB_VIEW_VISIBILITY))?;
+        #[cfg(feature = "forked-bevy")]
+        vis.check(b200vis_writeback_tables(vis.ctx, WB_VIEW_VISIBILITY, 0, this_run.this_run().get()))?;
         vis.check(b200vis_synchronize(vis.ctx))?;       // stats, sorted lists + class masks, ViewVisibility bytes are in host memory now
     }
     // ---- VisibleEntities: one sorted Vec per class; an entity is pushed once per class it carries (mod.rs:846-857).  The device
@@ -386,13 +443,7 @@ fn b200_check_visibility(
     for (r, byte) in vis.vv_col[..n].iter().enumerate() {        // the CPU bracket systems own the 2-bit state machine and the ticks
         if byte & 1 != 0 { if let Ok(mut q) = visible_aabb_query.get_mut(vis.entity_of[r]) { q.2.set_visible(); } }
     }
-    #[cfg(feature = "forked-bevy")]
-    for r in 0..n {                                              // the device owns it: bytes via bypass, ticks where the bit is set
-        if let Ok(mut q) = visible_aabb_query.get_mut(vis.entity_of[r]) {
-            *q.2.bypass_change_detection() = ViewVisibility::from_bits(vis.vv_col[r]);
-            if vis.vv_bits[r / 32] >> (r % 32) & 1 != 0 { q.2.set_changed(); }
-        }
-    }
+    // forked: nothing left to do -- the device owns the state machine and wrote bytes and ticks into the tables
     Ok(())
 }
 
