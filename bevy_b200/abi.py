@@ -136,6 +136,66 @@ def host_tables(capacities, lengths=None, gt_fill=np.nan, tick_fill=0, vv_fill=0
     return out, buf
 
 
+RD_TRANSFORM, RD_GLOBAL_TRANSFORM = 0x1, 0x2
+
+
+class TransformLayout(C.Structure):
+    """b200vis_transform_layout: bytes per slot and byte offsets of Transform's translation, rotation and scale."""
+    _fields_ = [("stride", C.c_uint32), ("translation", C.c_uint32), ("rotation", C.c_uint32), ("scale", C.c_uint32)]
+
+
+# glam's Quat is 16-byte aligned and rustc puts it first: rotation @ 0, translation @ 16, scale @ 28, 48 bytes per slot
+BEVY_TRANSFORM_LAYOUT = (48, 16, 0, 28)
+
+
+class TableInputs(C.Structure):
+    """b200vis_table_inputs: one table's Transform column and its changed_ticks column (both NULL = not read)."""
+    _fields_ = [("transforms", C.c_void_p), ("transform_changed_ticks", C.c_void_p)]
+
+
+class HostInputs:
+    """A table's Transform column as raw bytes [capacity, stride] in `layout` (stride, translation, rotation, scale)
+    and its ticks [capacity] uint32.  put / get move the packed 10 floats (translation.xyz, rotation.xyzw, scale.xyz)
+    of b200vis_upload_transforms_scattered in and out of slots."""
+
+    def __init__(self, trs, ticks, layout):
+        self.trs, self.ticks, self.layout = trs, ticks, tuple(layout)
+
+    def _floats(self, slots):
+        _, t, r, s = self.layout
+        b = self.trs[np.asarray(slots, np.int64)]
+        return [b[:, o:o + 4 * k] for o, k in ((t, 3), (r, 4), (s, 3))]
+
+    def put(self, slots, trs10):
+        v = np.ascontiguousarray(trs10, np.float32).reshape(-1, 10).view(np.uint8).reshape(-1, 40)
+        slots = np.asarray(slots, np.int64)
+        _, t, r, s = self.layout
+        for o, a, b in ((t, 0, 12), (r, 12, 28), (s, 28, 40)):
+            self.trs[slots, o:o + b - a] = v[:, a:b]
+
+    def get(self, slots):
+        return np.concatenate([np.ascontiguousarray(f).view(np.float32) for f in self._floats(slots)], axis=1)
+
+    def desc(self):
+        return TableInputs(self.trs.ctypes.data, self.ticks.ctypes.data)
+
+
+def host_table_inputs(capacities, layout=BEVY_TRANSFORM_LAYOUT, tick_fill=0, byte_fill=0xFF, pad=64):
+    """Input columns over ONE plain numpy buffer, beside host_tables' (same page rules).  Returns (inputs, buffer)."""
+    stride = int(layout[0])
+    al = lambda b: (b + pad - 1) // pad * pad
+    page = 4096
+    total = sum(al(c * stride) + al(c * 4) for c in capacities)
+    buf = np.zeros((total + 2 * page - 1) // page * page + page, np.uint8)
+    o, out = (-buf.ctypes.data) % page, []
+    for c in capacities:
+        trs = buf[o:o + c * stride].reshape(c, stride); o += al(c * stride)
+        ticks = buf[o:o + c * 4].view(np.uint32); o += al(c * 4)
+        trs[:] = byte_fill; ticks[:] = tick_fill
+        out.append(HostInputs(trs, ticks, layout))
+    return out, buf
+
+
 class ShadowItem(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("light_row", C.c_uint32), ("range", C.c_float), ("range_view_index", C.c_int32),
                 ("layer_mask", C.c_uint64), ("frusta", C.c_float * 144)]
@@ -179,6 +239,8 @@ _SIGNATURES = {
     "b200vis_set_tables": (C.c_int32, [_vp, C.c_uint32, _vp]),
     "b200vis_set_table_rows": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32, _vp]),
     "b200vis_writeback_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "b200vis_set_tables_ex": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, _P(TransformLayout)]),
+    "b200vis_read_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
     "b200vis_host_plan_summary": (C.c_int32, [C.c_uint32, _vp, _P(C.c_uint32)]),
     "b200vis_host_tile_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp]),
     "b200vis_host_warp_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp, _vp, _vp]),
@@ -833,6 +895,23 @@ class Context:
 
     def writeback_tables(self, which=WB_GLOBAL_TRANSFORM | WB_VIEW_VISIBILITY, gt_tick=0, vv_tick=0):
         self._check(self._lib.b200vis_writeback_tables(self._h, which, gt_tick, vv_tick))
+
+    def set_tables_ex(self, tables, inputs=None, layout=None):
+        """b200vis_set_tables_ex: `inputs` (None, or one HostInputs / TableInputs / None per table) and `layout`
+        (a TransformLayout or a (stride, translation, rotation, scale) tuple; None = NULL)."""
+        descs = [t.desc() if isinstance(t, HostTable) else t for t in tables]
+        arr = (Table * max(len(descs), 1))(*descs)
+        ins = None
+        if inputs is not None:
+            if len(inputs) != len(descs):                     # the library reads inputs[n_tables]
+                raise ValueError(f"set_tables_ex: {len(inputs)} inputs for {len(descs)} tables")
+            ins = (TableInputs * max(len(inputs), 1))(*[
+                i.desc() if isinstance(i, HostInputs) else (TableInputs() if i is None else i) for i in inputs])
+        lay = None if layout is None else (layout if isinstance(layout, TransformLayout) else TransformLayout(*layout))
+        self._check(self._lib.b200vis_set_tables_ex(self._h, len(descs), arr, ins, None if lay is None else C.byref(lay)))
+
+    def read_tables(self, which=RD_TRANSFORM | RD_GLOBAL_TRANSFORM, last_run=0, this_run=0):
+        self._check(self._lib.b200vis_read_tables(self._h, which, last_run & 0xFFFFFFFF, this_run & 0xFFFFFFFF))
 
     def p2p_export(self):
         """CUDA IPC handle (64 bytes) of this rank's gathered buffer."""

@@ -173,6 +173,7 @@ struct b200vis_ctx {
     // device) and its inverse, and the host-memory registrations the library owns
     bool tables_set = false;
     std::vector<b200vis_table> h_tabs; std::vector<uint32_t> tab_off;   // tab_off[t] = table t's first map entry
+    std::vector<b200vis_table_inputs> h_tab_in; b200vis_transform_layout tab_layout{};   // b200vis_set_tables_ex's input columns
     std::vector<uint32_t> h_tab_map, row_slot;                           // row_slot[row] = the row's map entry, or kNoParent
     std::vector<std::pair<uintptr_t, size_t>> host_regs;
     DevTable *d_tabs = nullptr; uint32_t *d_tab_chunks = nullptr; uint32_t tab_chunks_cap = 0, n_tab_chunks = 0;
@@ -3012,29 +3013,61 @@ static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_t
 }
 
 extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables) {
+    return b200vis_set_tables_ex(ctx, n_tables, tables, nullptr, nullptr);
+}
+
+extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables,
+                                         const b200vis_table_inputs *inputs, const b200vis_transform_layout *layout) {
     CHECK_CTX_JOIN();
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_tables: world_size > 1");
     if (n_tables && !tables) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: null tables");
     if (n_tables > B200VIS_MAX_TABLES) return fail(ctx, B200VIS_ERR_CAPACITY, "set_tables: %u tables > %u", n_tables, B200VIS_MAX_TABLES);
+    const b200vis_table_inputs no_inputs{nullptr, nullptr};
+    auto input = [&](uint32_t t) -> const b200vis_table_inputs & { return inputs ? inputs[t] : no_inputs; };
     uint64_t total = 0, chunks = 0;
+    bool any_transforms = false;
     for (uint32_t t = 0; t < n_tables; ++t) {
         if (tables[t].len > tables[t].capacity)
             return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u has len %u > capacity %u", t, tables[t].len, tables[t].capacity);
         // the kernel stores float4 matrices and u32 ticks
         if ((uintptr_t)tables[t].global_transforms % 16u || (uintptr_t)tables[t].gt_changed_ticks % 4u || (uintptr_t)tables[t].vv_changed_ticks % 4u)
             return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u: GlobalTransform needs 16-byte, tick columns 4-byte alignment", t);
+        const b200vis_table_inputs &in = input(t);
+        if ((in.transforms == nullptr) != (in.transform_changed_ticks == nullptr))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u: transforms and transform_changed_ticks must both be NULL or both be set", t);
+        // the kernel reads f32 fields and u32 ticks
+        if ((uintptr_t)in.transforms % 4u || (uintptr_t)in.transform_changed_ticks % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: table %u: input columns need 4-byte alignment", t);
+        any_transforms |= in.transforms != nullptr;
         total += tables[t].capacity;
         chunks += (tables[t].len + 127u) / 128u;
     }
+    if (any_transforms) {
+        if (!layout) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: a table has transforms but no layout was given");
+        const uint64_t lo[3] = {layout->translation, layout->rotation, layout->scale}, sz[3] = {12, 16, 12};
+        if (layout->stride % 4u || lo[0] % 4u || lo[1] % 4u || lo[2] % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: Transform layout fields and stride need 4-byte alignment");
+        for (int i = 0; i < 3; ++i) {
+            if (lo[i] + sz[i] > layout->stride)
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: Transform field at %llu runs past stride %u", (unsigned long long)lo[i], layout->stride);
+            for (int j = 0; j < i; ++j)
+                if (lo[i] < lo[j] + sz[j] && lo[j] < lo[i] + sz[i])
+                    return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_tables: Transform fields at %llu and %llu overlap", (unsigned long long)lo[j], (unsigned long long)lo[i]);
+        }
+    }
+    const b200vis_transform_layout lay = any_transforms ? *layout : b200vis_transform_layout{0, 0, 0, 0};
     if (total > (1ull << 31)) return fail(ctx, B200VIS_ERR_CAPACITY, "set_tables: %llu slots in all > 2^31", (unsigned long long)total);
-    CU(cudaStreamSynchronize(ctx->stream));   // no write-back in flight reads the old registry or registrations
+    CU(cudaStreamSynchronize(ctx->stream));   // no write-back or read in flight reads the old registry or registrations
     { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }   // queued entries index the current layout
     const uint32_t n_old = (uint32_t)ctx->h_tabs.size();
     auto moved = [&](uint32_t t) {            // table t's memory is not what it was (or t is new or gone)
         if (t >= n_old || t >= n_tables) return true;
         const b200vis_table &a = ctx->h_tabs[t], &b = tables[t];
+        const b200vis_table_inputs &ai = ctx->h_tab_in[t], &bi = input(t);
         return a.global_transforms != b.global_transforms || a.gt_changed_ticks != b.gt_changed_ticks ||
-               a.view_visibility != b.view_visibility || a.vv_changed_ticks != b.vv_changed_ticks || a.capacity != b.capacity;
+               a.view_visibility != b.view_visibility || a.vv_changed_ticks != b.vv_changed_ticks || a.capacity != b.capacity ||
+               ai.transforms != bi.transforms || ai.transform_changed_ticks != bi.transform_changed_ticks ||
+               (ai.transforms && ctx->tab_layout.stride != lay.stride);
     };
     // ---- the new maps: the entries below both capacities carry over ----
     std::vector<uint32_t> off(n_tables), map((size_t)total, kUnmapped), reset;
@@ -3055,15 +3088,16 @@ extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const
         for (const auto &r : ctx->host_regs) if (p >= r.first && p < r.first + r.second) return true;
         return false;
     };
-    auto columns = [](const b200vis_table &tb, auto &&fn) {
+    auto columns = [](const b200vis_table &tb, const b200vis_table_inputs &in, uint32_t stride, auto &&fn) {
         const size_t cap = tb.capacity;
         fn((void *)tb.global_transforms, cap * 64); fn((void *)tb.gt_changed_ticks, cap * 4);
         fn((void *)tb.view_visibility, cap); fn((void *)tb.vv_changed_ticks, cap * 4);
+        fn((void *)in.transforms, cap * stride); fn((void *)in.transform_changed_ticks, cap * 4);
     };
     auto rounded = [&](void *p, size_t bytes) { const uintptr_t a = (uintptr_t)p; return Range{a & ~(page - 1), (a + bytes + page - 1) & ~(page - 1)}; };
     std::vector<Range> need, changed;
     for (uint32_t t = 0; t < n_tables; ++t)
-        columns(tables[t], [&](void *p, size_t bytes) {
+        columns(tables[t], input(t), lay.stride, [&](void *p, size_t bytes) {
             if (!p || !bytes) return;
             if (moved(t)) changed.push_back(rounded(p, bytes));
             void *d = nullptr;
@@ -3072,7 +3106,9 @@ extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const
             need.push_back(rounded(p, bytes));
         });
     for (uint32_t t = 0; t < n_old; ++t)
-        if (moved(t)) columns(ctx->h_tabs[t], [&](void *p, size_t bytes) { if (p && bytes) changed.push_back(rounded(p, bytes)); });
+        if (moved(t))
+            columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride,
+                    [&](void *p, size_t bytes) { if (p && bytes) changed.push_back(rounded(p, bytes)); });
     std::sort(need.begin(), need.end());
     std::vector<Range> merged;
     for (const Range &r : need) {
@@ -3097,7 +3133,7 @@ extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const
             cudaGetLastError();
             for (const auto &q : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(q.first));
             cudaGetLastError();
-            ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
+            ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->h_tab_in.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
             std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
             ctx->n_tab_chunks = 0;
             return fail(ctx, B200VIS_ERR_CUDA, "set_tables: cudaHostRegister of %zu bytes at %p failed: %s", (size_t)(r.second - r.first),
@@ -3110,10 +3146,14 @@ extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const
     std::vector<uint32_t> chunk_table((size_t)chunks);
     for (uint32_t t = 0, c = 0; t < n_tables; ++t) {
         const b200vis_table &tb = tables[t];
-        void *alias[4] = {tb.global_transforms, tb.gt_changed_ticks, tb.view_visibility, tb.vv_changed_ticks};
+        const b200vis_table_inputs &in = input(t);
+        void *alias[6] = {tb.global_transforms, tb.gt_changed_ticks, tb.view_visibility, tb.vv_changed_ticks,
+                          const_cast<void *>(in.transforms), const_cast<uint32_t *>(in.transform_changed_ticks)};
         for (void *&p : alias) if (p && tb.capacity) { void *d = nullptr; CU(cudaHostGetDevicePointer(&d, p, 0)); p = d; } else p = nullptr;
         dt[t] = DevTable{static_cast<float4 *>(alias[0]), static_cast<uint32_t *>(alias[1]), static_cast<uint8_t *>(alias[2]),
-                         static_cast<uint32_t *>(alias[3]), tb.len, off[t], c, 0};
+                         static_cast<uint32_t *>(alias[3]), tb.len, off[t], c, 0,
+                         static_cast<const uint8_t *>(alias[4]), static_cast<const uint32_t *>(alias[5]),
+                         lay.stride, lay.translation, lay.rotation, lay.scale};
         for (uint32_t k = 0; k < (tb.len + 127u) / 128u; ++k) chunk_table[c++] = t;
     }
     const size_t N = ctx->cfg.max_entities;
@@ -3141,6 +3181,9 @@ extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const
     CU(cudaStreamSynchronize(st));
     // ---- commit ----
     ctx->h_tabs.assign(tables, tables + n_tables);
+    ctx->h_tab_in.resize(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t) ctx->h_tab_in[t] = input(t);
+    ctx->tab_layout = lay;
     ctx->tab_off = std::move(off);
     ctx->h_tab_map = std::move(map);
     ctx->row_slot.assign(N, kUnmapped);
@@ -3193,6 +3236,24 @@ extern "C" int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, ui
     const TableBufs tb{ctx->d_tabs, ctx->d_tab_chunks, ctx->n_tab_chunks, ctx->d_tab_map, ctx->d_tvv_shadow};
     launch_writeback_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_WB_GLOBAL_TRANSFORM | B200VIS_WB_VIEW_VISIBILITY), gt_tick, vv_tick);
     CU(cudaGetLastError());
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_t last_run, uint32_t this_run) {
+    CHECK_CTX();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "read_tables: world_size > 1");
+    if (!ctx->tables_set || ctx->h_tabs.empty()) return fail(ctx, B200VIS_ERR_NOT_READY, "read_tables: no tables are registered");
+    which &= B200VIS_RD_TRANSFORM | B200VIS_RD_GLOBAL_TRANSFORM;
+    { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }
+    const TableBufs tb{ctx->d_tabs, ctx->d_tab_chunks, ctx->n_tab_chunks, ctx->d_tab_map, ctx->d_tvv_shadow};
+    launch_read_tables(ctx->stream, ctx->rows, tb, which, last_run, this_run);
+    CU(cudaGetLastError());
+    if (which & B200VIS_RD_GLOBAL_TRANSFORM) {
+        // whether a slot was newer is known only on the device: the next propagate takes the marked instantiation
+        bool gt_inputs = false;
+        for (const b200vis_table &t : ctx->h_tabs) gt_inputs |= t.global_transforms && t.gt_changed_ticks;
+        if (gt_inputs) { ctx->gt_ext_pending = true; ctx->gt_aos_valid = false; }
+    }
     return B200VIS_OK;
 }
 

@@ -264,14 +264,17 @@ struct RowEdit {
     float2 *range_se;
 };
 
-// b200vis_set_tables: one registered archetype table as k_writeback_tables sees it (device aliases of the caller's columns,
-// nullptr = not delivered)
+// b200vis_set_tables: one registered archetype table as k_writeback_tables and k_read_tables see it (device aliases of the
+// caller's columns, nullptr = not delivered)
 struct DevTable {
     float4 *gt; uint32_t *gt_ticks; uint8_t *vv; uint32_t *vv_ticks;
-    uint32_t len;            // slots [0, len) are written
+    uint32_t len;            // slots [0, len) are written / read
     uint32_t map_off;        // the table's slot -> row map starts at TableBufs::map[map_off]
     uint32_t chunk_begin;    // the table's first 128-slot chunk in the launch's chunk numbering
     uint32_t pad;
+    // b200vis_set_tables_ex: the Transform column and its ticks (nullptr = not read), and the Transform layout in bytes
+    const uint8_t *trs; const uint32_t *trs_ticks;
+    uint32_t stride, t_off, r_off, s_off;
 };
 struct TableBufs {
     const DevTable *tables;

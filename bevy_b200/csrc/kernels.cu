@@ -3127,6 +3127,70 @@ k_writeback_tables(Rows R, TableBufs tb, uint32_t which, uint32_t gt_tick, uint3
     }
 }
 
+// ---- table read: Changed<Transform> and outside-written GlobalTransforms straight from the caller's tables
+// (b200vis_read_tables).  The write-back's chunk walk, one warp per 128-slot chunk.  A chunk's ticks cross PCIe as 16-byte
+// loads into the warp's shared slab: a misaligned head moves the window back to the previous 16-byte boundary (still inside
+// the column's page, so inside what is registered).  Only slots whose tick is newer read their Transform or Affine3A.
+// Staging the tick columns through the copy engine instead was measured and lost: one copy per table per column costs
+// ~3 us, so it wins at 4 tables but loses from 64 tables on (DESIGN.md section 7).
+__device__ __forceinline__ bool tick_is_newer(uint32_t tick, uint32_t last_run, uint32_t this_run) {
+    constexpr uint32_t kMaxChangeAge = 0xFFFFFFFFu - (2u * 518400000u - 1u);   // change_detection/mod.rs
+    return min(this_run - last_run, kMaxChangeAge) > min(this_run - tick, kMaxChangeAge);   // Tick::is_newer_than
+}
+// slots [s0, s1) of a tick column (s1 - s0 <= 128) into s: the tick of slot s0 + i lands at s[head + i]; returns head
+__device__ __forceinline__ uint32_t stage_ticks(const uint32_t *col, uint32_t s0, uint32_t s1, uint32_t lane, uint4 *s) {
+    const uintptr_t a = reinterpret_cast<uintptr_t>(col + s0);
+    const uint32_t head = (uint32_t)(a & 15u) / 4u;
+    const uint4 *v = reinterpret_cast<const uint4 *>(a - head * 4u);
+    const uint32_t n4 = (head + (s1 - s0) + 3u) / 4u;          // <= 33 pieces
+    for (uint32_t k = lane; k < n4; k += 32u) s[k] = __ldg(v + k);
+    return head;
+}
+
+__global__ void __launch_bounds__(256)
+k_read_tables(Rows R, TableBufs tb, uint32_t which, uint32_t last_run, uint32_t this_run) {
+    __shared__ uint4 s_tk[8][2][33];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    const bool rt = which & 1u, rg = which & 2u;
+    for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
+        const DevTable T = tb.tables[tb.chunk_table[ch]];
+        const bool do_t = rt && T.trs != nullptr, do_g = rg && T.gt != nullptr && T.gt_ticks != nullptr;
+        if (!do_t && !do_g) continue;                         // the same for the whole warp
+        const uint32_t base = (ch - T.chunk_begin) * 128u, n = min(T.len - base, 128u);
+        const uint32_t ht = do_t ? stage_ticks(T.trs_ticks, base, base + n, lane, s_tk[warp][0]) : 0u;
+        const uint32_t hg = do_g ? stage_ticks(T.gt_ticks, base, base + n, lane, s_tk[warp][1]) : 0u;
+        __syncwarp();
+        const uint32_t *tt = reinterpret_cast<const uint32_t *>(s_tk[warp][0]) + ht;
+        const uint32_t *tg = reinterpret_cast<const uint32_t *>(s_tk[warp][1]) + hg;
+        for (uint32_t i = lane; i < n; i += 32u) {
+            const uint32_t slot = base + i;
+            const bool nt = do_t && tick_is_newer(tt[i], last_run, this_run);
+            const bool ng = do_g && tick_is_newer(tg[i], last_run, this_run);
+            if (!nt && !ng) continue;
+            const uint32_t row = tb.map[T.map_off + slot];
+            if (row == kNoParent) continue;
+            if (nt) {                                         // what k_scatter_trs does with the packed 10 floats
+                const uint8_t *p = T.trs + (size_t)slot * T.stride;
+                const float *t = reinterpret_cast<const float *>(p + T.t_off), *q = reinterpret_cast<const float *>(p + T.r_off);
+                const float *s = reinterpret_cast<const float *>(p + T.s_off);
+                R.trsA[row] = make_float4(t[0], t[1], t[2], s[0]);
+                R.trsB[row] = make_float4(q[0], q[1], q[2], q[3]);
+                R.trsC[row] = make_float2(s[1], s[2]);
+                R.flags[row] = (uint8_t)(R.flags[row] | F_TCHANGED);
+            }
+            if (ng) {                                         // what k_write_gt_scattered does with lanes 0-2 of each Vec3A
+                const float4 *g = T.gt + (size_t)slot * 4u;
+                const float4 x = g[0], y = g[1], z = g[2], w = g[3];
+                R.gt0[row] = make_float4(x.x, y.x, z.x, w.x);
+                R.gt1[row] = make_float4(x.y, y.y, z.y, w.y);
+                R.gt2[row] = make_float4(x.z, y.z, z.z, w.z);
+                R.state[row] = (uint8_t)(R.state[row] | S_GT_EXT);
+            }
+        }
+        __syncwarp();                                         // the slab is the warp's next chunk's
+    }
+}
+
 __global__ void __launch_bounds__(256) k_update_table_map(uint32_t *__restrict__ map, const uint2 *__restrict__ set, uint32_t n_set,
                                                           uint8_t *__restrict__ vv_shadow, const uint32_t *__restrict__ reset,
                                                           uint32_t n_reset) {
@@ -3990,6 +4054,11 @@ void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb
     if (!tb.n_chunks) return;
     const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
     ++g_launches; k_writeback_tables<<<grid, 256, 0, st>>>(R, tb, which, gt_tick, vv_tick);
+}
+void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t last_run, uint32_t this_run) {
+    if (!tb.n_chunks || !which) return;
+    const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
+    ++g_launches; k_read_tables<<<grid, 256, 0, st>>>(R, tb, which, last_run, this_run);
 }
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
                              uint32_t n_reset) {

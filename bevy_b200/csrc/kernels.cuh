@@ -48,6 +48,8 @@ void launch_snapshot_lights(cudaStream_t st, const Rows &R, const Lights &L, flo
 void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, uint32_t stride, uint32_t *host_gt_bits, uint8_t *host_vv,
                               uint32_t *host_vv_bits, uint8_t *vv_shadow);
 void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
+// b200vis_read_tables: which = B200VIS_RD_* bits, slots newer by Tick::is_newer_than(last_run, this_run)
+void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t last_run, uint32_t this_run);
 // set_table_rows / set_tables / edit_topology: map[set[i].x] = set[i].y, then vv_shadow[reset[i]] = 0xFF
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
                              uint32_t n_reset);

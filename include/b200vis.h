@@ -513,6 +513,44 @@ B200VIS_API int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uin
  * UNSUPPORTED (world_size > 1). */
 B200VIS_API int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
 
+/* ---- reading Transform and outside-written GlobalTransform straight from the same tables ----------------------------------
+ * The device finds Changed<Transform> and Changed<GlobalTransform> itself: it reads every slot's tick over PCIe, and the
+ * Transform or Affine3A of the slots whose tick is newer, through the same slot -> row maps as the write-back.
+ * Transform is repr(Rust), so its layout is passed in (size_of::<Transform>() and offset_of! of its three fields). */
+typedef struct b200vis_transform_layout {
+    uint32_t stride;                          /* bytes per slot */
+    uint32_t translation, rotation, scale;    /* byte offsets of Vec3, Quat (x, y, z, w), Vec3 */
+} b200vis_transform_layout;
+typedef struct b200vis_table_inputs {
+    const void     *transforms;               /* [capacity] Transform; NULL = the table is not read for Transform */
+    const uint32_t *transform_changed_ticks;  /* [capacity] Transform's changed_ticks; NULL exactly when transforms is */
+} b200vis_table_inputs;
+/* b200vis_set_tables with input columns: inputs == NULL or inputs[n_tables].  The input columns are registered, kept and
+ * released with the output columns (the page rules above apply to them too).  b200vis_set_tables(ctx, n, t) is
+ * b200vis_set_tables_ex(ctx, n, t, NULL, NULL).  Errors, besides those of b200vis_set_tables: INVALID_ARG (a layout field
+ * that is not 4-byte aligned, a field past stride, overlapping fields, no layout while some table has transforms, only one
+ * of a table's two input pointers NULL, a misaligned input pointer); nothing changes then. */
+B200VIS_API int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables,
+                                          const b200vis_table_inputs *inputs, const b200vis_transform_layout *layout);
+/* Enqueues the read of `which` on the context's stream, in call order with every other upload; queued map changes are
+ * sent first.  A slot is read when it is below len, mapped to a live row, and its tick is newer by Bevy's
+ * Tick::is_newer_than(last_run, this_run) (change_detection/tick.rs): this_run - tick < this_run - last_run in wrapping
+ * u32 arithmetic, both ages clamped to MAX_CHANGE_AGE = 0xFFFFFFFF - (2 * 518400000 - 1).  Pass the reading system's
+ * SystemChangeTick pair: ticks that system's own write-back stamped last frame equal last_run and are not read.
+ *   B200VIS_RD_TRANSFORM         Transform, as b200vis_upload_transforms_scattered would upload it for the row (bits copied,
+ *                                the row marked Changed<Transform>)
+ *   B200VIS_RD_GLOBAL_TRANSFORM  global_transforms / gt_changed_ticks of b200vis_table (tables lacking either are skipped),
+ *                                as b200vis_write_global_transforms_scattered would write lanes 0-2 of the four Vec3A.
+ *                                Without a synchronisation the host cannot know whether any slot was newer, so the next
+ *                                run with PROPAGATE takes the marked tile-kernel instantiation (and an experiment tile
+ *                                kernel returns UNSUPPORTED) whenever some table has both columns.
+ * The frame is then b200vis_read_tables, b200vis_step(ctx, 0, NULL, NULL, ...) (or the runs), the write-back, one
+ * b200vis_synchronize.  The caller leaves the columns alone until that synchronize.  Errors: NOT_READY (no tables
+ * registered), UNSUPPORTED (world_size > 1). */
+#define B200VIS_RD_TRANSFORM        0x1u
+#define B200VIS_RD_GLOBAL_TRANSFORM 0x2u
+B200VIS_API int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_t last_run, uint32_t this_run);
+
 /* ---- SURVEY.md 8(f) N1: the render world's visible-entity diff ---------------------------------------------
  * RenderVisibleEntitiesClass::update_cpu_culled_entities (crates/bevy_render/src/view/visibility/mod.rs:194-249)
  * marches over last frame's and this frame's sorted list to find the newly added and newly removed entities.  With

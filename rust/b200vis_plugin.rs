@@ -15,10 +15,11 @@
 //! byte) composing correctly (SURVEY.md 8b).  With a three-line patch that makes those two systems removable, the device's
 //! ViewVisibility bytes + change bits can be written straight into the column instead (`forked-bevy` feature below).
 //!
-//! Data flow (INTEGRATION.md section 2): ECS columns -> `upload_*` on change; results -> pinned host buffers the GPU
-//! writes itself (`b200vis_set_result_sink`, `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system;
-//! GlobalTransform (and, forked, ViewVisibility) with their change ticks straight into the archetype tables
-//! (`b200vis_set_tables`, `b200vis_writeback_tables`).
+//! Data flow (INTEGRATION.md section 2): Transform and other systems' GlobalTransforms read by the device straight from
+//! the archetype tables by their change ticks (`b200vis_set_tables_ex`, `b200vis_read_tables`); other ECS columns ->
+//! `upload_*` on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
+//! `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system; GlobalTransform (and, forked,
+//! ViewVisibility) with their change ticks straight into the archetype tables (`b200vis_writeback_tables`).
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
 use bevy::camera::primitives::{Aabb, Frustum, Sphere};
 use bevy::camera::visibility::*;
@@ -31,6 +32,7 @@ use bevy::prelude::*;
 use bevy::transform::{systems::*, TransformSystems};
 use core::any::TypeId;
 use core::ffi::c_char;
+use core::mem::{offset_of, size_of};
 
 // ---- FFI (mirrors include/b200vis.h, ABI version 2) -----------------------------------------------------------------------
 #[repr(C)] pub struct b200vis_ctx { _p: [u8; 0] }
@@ -56,6 +58,9 @@ pub struct b200vis_cluster_feedback { has_farthest_z: u32, farthest_z: f32, has_
 #[repr(C)] #[derive(Clone, Copy, PartialEq)]
 pub struct b200vis_table { global_transforms: *mut GlobalTransform, gt_changed_ticks: *mut Tick, view_visibility: *mut ViewVisibility,
     vv_changed_ticks: *mut Tick, len: u32, capacity: u32 }
+#[repr(C)] pub struct b200vis_transform_layout { stride: u32, translation: u32, rotation: u32, scale: u32 }
+#[repr(C)] #[derive(Clone, Copy, PartialEq)]
+pub struct b200vis_table_inputs { transforms: *const Transform, transform_changed_ticks: *const Tick }
 
 #[link(name = "b200vis")]
 extern "C" {
@@ -66,9 +71,7 @@ extern "C" {
     fn b200vis_set_topology(ctx: *mut b200vis_ctx, n: u32, parent_row: *const u32, entity_bits: *const u64) -> i32;
     fn b200vis_plan_row_order(n: u32, parent_row: *const u32, new_to_old: *mut u32) -> i32;
     fn b200vis_upload_transforms(ctx: *mut b200vis_ctx, first: u32, count: u32, trs: *const f32) -> i32;
-    fn b200vis_upload_transforms_scattered(ctx: *mut b200vis_ctx, count: u32, rows: *const u32, trs: *const f32) -> i32;
     fn b200vis_upload_global_transforms(ctx: *mut b200vis_ctx, first: u32, count: u32, gt: *const f32) -> i32;
-    fn b200vis_write_global_transforms_scattered(ctx: *mut b200vis_ctx, count: u32, rows: *const u32, gt: *const f32) -> i32;
     fn b200vis_upload_bounds(ctx: *mut b200vis_ctx, first: u32, count: u32, bounds: *const f32, flags: *const u8, class_mask: *const u8,
                              layer_mask: *const u64, range_mask: *const u32) -> i32;
     fn b200vis_upload_view_visibility(ctx: *mut b200vis_ctx, first: u32, count: u32, vv: *const u8) -> i32;
@@ -84,13 +87,16 @@ extern "C" {
     fn b200vis_set_view_stats_sink(ctx: *mut b200vis_ctx, per_view: *mut [u32; 4]) -> i32;
     fn b200vis_set_column_sinks(ctx: *mut b200vis_ctx, sinks: *const b200vis_column_sinks) -> i32;
     fn b200vis_writeback_columns_ex(ctx: *mut b200vis_ctx, which: u32) -> i32;
-    fn b200vis_set_tables(ctx: *mut b200vis_ctx, n: u32, tables: *const b200vis_table) -> i32;
     fn b200vis_set_table_rows(ctx: *mut b200vis_ctx, table: u32, first_slot: u32, count: u32, rows: *const u32) -> i32;
     fn b200vis_writeback_tables(ctx: *mut b200vis_ctx, which: u32, gt_tick: u32, vv_tick: u32) -> i32;
+    fn b200vis_set_tables_ex(ctx: *mut b200vis_ctx, n: u32, tables: *const b200vis_table, inputs: *const b200vis_table_inputs,
+                             layout: *const b200vis_transform_layout) -> i32;
+    fn b200vis_read_tables(ctx: *mut b200vis_ctx, which: u32, last_run: u32, this_run: u32) -> i32;
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
 const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2; const UNMAPPED: u32 = 0xFFFF_FFFF;
+const RD_TRANSFORM: u32 = 1; const RD_GLOBAL_TRANSFORM: u32 = 2;
 const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04; const F_NO_FRUSTUM: u8 = 0x08;
 const F_RANGE: u8 = 0x10; const F_SPHERE_FROM_GT: u8 = 0x40;
 const VIEW_ACTIVE: u8 = 1; const VIEW_NO_CPU_CULLING: u8 = 2;
@@ -120,9 +126,10 @@ pub struct B200Vis {
     vv_col: Vec<u8>, vv_bits: Vec<u32>,
     visible_rows: Vec<u32>, visible_classes: Vec<u8>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
     planes_scratch: Vec<f32>,
-    // the archetype tables registered with b200vis_set_tables (one entry per table holding GlobalTransform, with its
-    // ViewVisibility column in the forked build), the entities each slot map was built from, and the rows epoch of the maps
-    tables: Vec<b200vis_table>, table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
+    // the archetype tables registered with b200vis_set_tables_ex (one entry per table holding GlobalTransform, with its
+    // Transform column and in the forked build its ViewVisibility column), the entities each slot map was built from, and
+    // the rows epoch of the maps
+    tables: Vec<b200vis_table>, table_inputs: Vec<b200vis_table_inputs>, table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -164,7 +171,8 @@ impl Plugin for B200VisibilityPlugin {
             stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, vv_col: vec![0; n],
             vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; max_views * n], visible_classes: vec![0; max_views * n],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
-            planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_entities: Vec::new(), maps_epoch: u64::MAX,
+            planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_entities: Vec::new(),
+            maps_epoch: u64::MAX,
         };
         let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: vis.visible_rows.as_mut_ptr(), visible_capacity: n as u32,
             visible_classes: vis.visible_classes.as_mut_ptr(), cluster_offsets: vis.cluster_offsets.as_mut_ptr(),
@@ -214,7 +222,8 @@ fn pack_gt12(g: &GlobalTransform, out: &mut Vec<f32>) {
 fn b200_propagate(
     this_run: SystemChangeTick,
     mut vis: ResMut<B200Vis>,
-    mut q: Query<(Entity, Ref<Transform>, &mut GlobalTransform, Option<&Children>, Option<&ChildOf>)>,
+    // write access to GlobalTransform: the GPU writes the tables' columns while this system runs
+    q: Query<(Entity, Ref<Transform>, &mut GlobalTransform, Option<&Children>, Option<&ChildOf>)>,
     structure_changed: Query<(), Or<(Added<GlobalTransform>, Changed<ChildOf>)>>,
     mut orphaned: RemovedComponents<ChildOf>,
     mut despawned: RemovedComponents<GlobalTransform>,
@@ -251,24 +260,12 @@ fn b200_propagate(
         vis.n = n;
         vis.columns_epoch += 1;
     } else {
-        // ---- steady state: only rows matching Changed<Transform> cross PCIe ----
-        let (mut rows, mut trs) = (Vec::new(), Vec::new());
-        for (e, t, _, _, _) in q.iter() {
-            if t.is_changed() { rows.push(vis.row_of[&e]); pack_trs(&t, &mut trs); }
-        }
-        if !rows.is_empty() {
-            vis.check(unsafe { b200vis_upload_transforms_scattered(vis.ctx, rows.len() as u32, rows.as_ptr(), trs.as_ptr()) })?;
-        }
-        // Changed<GlobalTransform> as this system sees it (systems.rs:709-710): exactly the writes of other systems, because
-        // this system's own write-back of its last run is not newer than its last_run.  Read through `q` (is_changed() on
-        // the `Mut` does not stamp a tick): a second query on GlobalTransform would conflict with q's mutable access.
-        let (mut grows, mut gts) = (Vec::new(), Vec::new());
-        for (e, _, g, _, _) in q.iter_mut() {
-            if g.is_changed() { grows.push(vis.row_of[&e]); pack_gt12(&g, &mut gts); }
-        }
-        if !grows.is_empty() {
-            vis.check(unsafe { b200vis_write_global_transforms_scattered(vis.ctx, grows.len() as u32, grows.as_ptr(), gts.as_ptr()) })?;
-        }
+        // ---- steady state: the device finds Changed<Transform> and Changed<GlobalTransform> in the tables itself and
+        // reads only those slots: no entity loop here.  Changed<GlobalTransform> as this system sees it (systems.rs:709-710)
+        // is exactly the writes of other systems, because this system's own write-back of its last run is not newer than
+        // its last_run (Tick::is_newer_than, the rule the device applies to every slot).
+        vis.check(unsafe { b200vis_read_tables(vis.ctx, RD_TRANSFORM | RD_GLOBAL_TRANSFORM, this_run.last_run().get(),
+                                               this_run.this_run().get()) })?;
     }
     // the registry b200_sync_tables left is current for this frame's tables; a rebuild above renumbered the rows and
     // b200vis_set_topology unmapped every slot, so the maps are sent again
@@ -293,13 +290,17 @@ fn b200_propagate(
 /// len) or the rows were renumbered.  Bevy never removes a table, so a table keeps its index in the registry.
 fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     let Some(gt_id) = world.component_id::<GlobalTransform>() else { return Ok(()) };
+    let t_id = world.component_id::<Transform>();
+    // Transform is repr(Rust): its layout is whatever this build of rustc chose
+    let layout = b200vis_transform_layout { stride: size_of::<Transform>() as u32, translation: offset_of!(Transform, translation) as u32,
+                                            rotation: offset_of!(Transform, rotation) as u32, scale: offset_of!(Transform, scale) as u32 };
     #[cfg(feature = "forked-bevy")]
     let vv_id = world.component_id::<ViewVisibility>();
     #[cfg(not(feature = "forked-bevy"))]
     let vv_id: Option<bevy::ecs::component::ComponentId> = None;
     world.resource_scope(|world, mut vis: Mut<B200Vis>| {
         let vis = &mut *vis;
-        let (mut descs, mut entities) = (Vec::new(), Vec::new());
+        let (mut descs, mut inputs, mut entities) = (Vec::new(), Vec::new(), Vec::new());
         for table in world.storages().tables.iter() {
             if !table.has_column(gt_id) { continue; }
             // SAFETY: the columns hold GlobalTransform / ViewVisibility.  Only raw pointers are kept; the GPU writes through
@@ -314,11 +315,19 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             descs.push(b200vis_table { global_transforms: gt.as_ptr() as *mut GlobalTransform, gt_changed_ticks: gt_ticks.as_ptr() as *mut Tick,
                                        view_visibility: vv, vv_changed_ticks: vv_ticks, len: table.entity_count(),
                                        capacity: table.capacity() as u32 });
+            // the Transform column and its ticks, which b200vis_read_tables reads (a table without Transform is not read)
+            inputs.push(match t_id.filter(|id| table.has_column(*id)) {
+                Some(id) => b200vis_table_inputs {
+                    transforms: unsafe { table.get_data_slice_for::<Transform>(id) }.unwrap().as_ptr() as *const Transform,
+                    transform_changed_ticks: table.get_changed_ticks_slice_for(id).unwrap().as_ptr() as *const Tick },
+                None => b200vis_table_inputs { transforms: core::ptr::null(), transform_changed_ticks: core::ptr::null() },
+            });
             entities.push(table.entities());
         }
-        if descs != vis.tables {
-            vis.check(unsafe { b200vis_set_tables(vis.ctx, descs.len() as u32, descs.as_ptr()) })?;
+        if descs != vis.tables || inputs != vis.table_inputs {
+            vis.check(unsafe { b200vis_set_tables_ex(vis.ctx, descs.len() as u32, descs.as_ptr(), inputs.as_ptr(), &layout) })?;
             vis.tables = descs;
+            vis.table_inputs = inputs;
         }
         let renumbered = vis.maps_epoch != vis.columns_epoch;
         let stale: Vec<bool> = entities.iter().enumerate()
