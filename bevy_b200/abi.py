@@ -136,7 +136,7 @@ def host_tables(capacities, lengths=None, gt_fill=np.nan, tick_fill=0, vv_fill=0
     return out, buf
 
 
-RD_TRANSFORM, RD_GLOBAL_TRANSFORM = 0x1, 0x2
+RD_TRANSFORM, RD_GLOBAL_TRANSFORM, RD_CULL_INPUTS = 0x1, 0x2, 0x4
 
 
 class TransformLayout(C.Structure):
@@ -196,6 +196,87 @@ def host_table_inputs(capacities, layout=BEVY_TRANSFORM_LAYOUT, tick_fill=0, byt
     return out, buf
 
 
+class BoundsLayout(C.Structure):
+    """b200vis_bounds_layout: bytes per slot and byte offsets of Aabb's center / half_extents and Sphere's center / radius."""
+    _fields_ = [("aabb_stride", C.c_uint32), ("aabb_center", C.c_uint32), ("aabb_half_extents", C.c_uint32),
+                ("sphere_stride", C.c_uint32), ("sphere_center", C.c_uint32), ("sphere_radius", C.c_uint32)]
+
+
+# Aabb = two Vec3A (16-byte aligned, 32 bytes); Sphere = Vec3A + f32, padded to 32 bytes: center @ 0 in both
+BEVY_BOUNDS_LAYOUT = (32, 0, 16, 32, 0, 16)
+
+
+class TableCullInputs(C.Structure):
+    """b200vis_table_cull_inputs: a table's Aabb, Sphere and InheritedVisibility columns with their ticks, and its
+    per-archetype flags."""
+    _fields_ = [("aabbs", C.c_void_p), ("aabb_changed_ticks", C.c_void_p), ("spheres", C.c_void_p),
+                ("sphere_changed_ticks", C.c_void_p), ("inherited_visibility", C.c_void_p), ("iv_changed_ticks", C.c_void_p),
+                ("flags", C.c_uint32)]
+
+
+class HostCull:
+    """A table's cull-input columns: Aabb and Sphere as raw bytes [capacity, stride] in `layout`, InheritedVisibility
+    bytes [capacity], each with ticks [capacity] uint32.  `has` names the columns desc() passes ("aabb", "sphere", "iv"),
+    `flags` the per-archetype bits."""
+
+    def __init__(self, aabb, aabb_ticks, sphere, sphere_ticks, iv, iv_ticks, layout, has=("aabb", "iv"), flags=0):
+        self.aabb, self.aabb_ticks, self.sphere, self.sphere_ticks = aabb, aabb_ticks, sphere, sphere_ticks
+        self.iv, self.iv_ticks, self.layout = iv, iv_ticks, tuple(layout)
+        self.has, self.flags = tuple(has), int(flags)
+
+    def _put(self, col, slots, fields):
+        slots = np.asarray(slots, np.int64)
+        for off, vals in fields:
+            v = np.ascontiguousarray(vals, np.float32).reshape(len(slots), -1)
+            col[slots, off:off + 4 * v.shape[1]] = v.view(np.uint8)
+
+    def put_aabb(self, slots, center, half_extents):
+        _, c, h = self.layout[:3]
+        self._put(self.aabb, slots, ((c, center), (h, half_extents)))
+
+    def put_sphere(self, slots, center, radius):
+        _, c, r = self.layout[3:]
+        self._put(self.sphere, slots, ((c, center), (r, np.asarray(radius, np.float32).reshape(-1, 1))))
+
+    def get_aabb(self, slots):
+        """[k, 6] float32: center.xyz, half_extents.xyz."""
+        _, c, h = self.layout[:3]
+        b = self.aabb[np.asarray(slots, np.int64)]
+        return np.concatenate([np.ascontiguousarray(b[:, o:o + 12]).view(np.float32) for o in (c, h)], axis=1)
+
+    def get_sphere(self, slots):
+        """[k, 4] float32: center.xyz, radius."""
+        _, c, r = self.layout[3:]
+        b = self.sphere[np.asarray(slots, np.int64)]
+        return np.concatenate([np.ascontiguousarray(b[:, c:c + 12]).view(np.float32),
+                               np.ascontiguousarray(b[:, r:r + 4]).view(np.float32)], axis=1)
+
+    def desc(self):
+        ptr = lambda name, a: a.ctypes.data if name in self.has else None
+        return TableCullInputs(ptr("aabb", self.aabb), ptr("aabb", self.aabb_ticks), ptr("sphere", self.sphere),
+                               ptr("sphere", self.sphere_ticks), ptr("iv", self.iv), ptr("iv", self.iv_ticks), self.flags)
+
+
+def host_table_cull_inputs(capacities, layout=BEVY_BOUNDS_LAYOUT, tick_fill=0, byte_fill=0xFF, pad=64):
+    """Cull-input columns (all three, each with ticks) over ONE plain numpy buffer, beside host_tables' (same page
+    rules).  Returns (inputs, buffer); set each HostCull's `has` and `flags` before passing it."""
+    sa, ss = int(layout[0]), int(layout[3])
+    al = lambda b: (b + pad - 1) // pad * pad
+    page = 4096
+    total = sum(al(c * sa) + al(c * ss) + al(c) + 3 * al(c * 4) for c in capacities)
+    buf = np.zeros((total + 2 * page - 1) // page * page + page, np.uint8)
+    o, out = (-buf.ctypes.data) % page, []
+    for c in capacities:
+        cols = []
+        for width, dtype in ((sa, None), (4, np.uint32), (ss, None), (4, np.uint32), (1, None), (4, np.uint32)):
+            a = buf[o:o + c * width]; o += al(c * width)
+            a = a.view(dtype) if dtype is not None else (a.reshape(c, width) if width > 1 else a)
+            a[:] = tick_fill if dtype is not None else byte_fill
+            cols.append(a)
+        out.append(HostCull(*cols, layout))
+    return out, buf
+
+
 class ShadowItem(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("light_row", C.c_uint32), ("range", C.c_float), ("range_view_index", C.c_int32),
                 ("layer_mask", C.c_uint64), ("frusta", C.c_float * 144)]
@@ -241,6 +322,7 @@ _SIGNATURES = {
     "b200vis_writeback_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
     "b200vis_set_tables_ex": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, _P(TransformLayout)]),
     "b200vis_read_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "b200vis_set_table_cull_inputs": (C.c_int32, [_vp, C.c_uint32, _vp, _P(BoundsLayout)]),
     "b200vis_host_plan_summary": (C.c_int32, [C.c_uint32, _vp, _P(C.c_uint32)]),
     "b200vis_host_tile_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp]),
     "b200vis_host_warp_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp, _vp, _vp]),
@@ -912,6 +994,17 @@ class Context:
 
     def read_tables(self, which=RD_TRANSFORM | RD_GLOBAL_TRANSFORM, last_run=0, this_run=0):
         self._check(self._lib.b200vis_read_tables(self._h, which, last_run & 0xFFFFFFFF, this_run & 0xFFFFFFFF))
+
+    def set_table_cull_inputs(self, inputs, layout=BEVY_BOUNDS_LAYOUT, n_tables=None):
+        """b200vis_set_table_cull_inputs: `inputs` = one HostCull / TableCullInputs / None (not read) per registered
+        table; `layout` a BoundsLayout, a 6-tuple or None (NULL).  n_tables overrides the count passed (argument tests)."""
+        descs = [i.desc() if isinstance(i, HostCull) else (TableCullInputs() if i is None else i) for i in inputs]
+        arr = (TableCullInputs * max(len(descs), 1))(*descs)
+        lay = None if layout is None else (layout if isinstance(layout, BoundsLayout) else BoundsLayout(*layout))
+        n = len(descs) if n_tables is None else n_tables
+        if n > len(descs):                                   # the library reads inputs[n_tables]
+            raise ValueError(f"set_table_cull_inputs: n_tables {n} > {len(descs)} entries")
+        self._check(self._lib.b200vis_set_table_cull_inputs(self._h, n, arr, None if lay is None else C.byref(lay)))
 
     def p2p_export(self):
         """CUDA IPC handle (64 bytes) of this rank's gathered buffer."""

@@ -182,6 +182,11 @@ struct b200vis_ctx {
     uint8_t *d_tab_upd = nullptr; size_t tab_upd_cap = 0;   // map updates on their way to k_update_table_map
     std::vector<uint32_t> pend_touched, pend_reset;          // queued map entries / shadow resets, sent by flush_table_updates
     uint8_t *h_tab_stage = nullptr; size_t h_tab_stage_cap = 0; cudaEvent_t ev_tab = nullptr;   // pinned staging of a batch
+    // b200vis_set_table_cull_inputs: the entries of the last call (kept across b200vis_set_tables, which only detaches them),
+    // whether they are attached, their device form, and per map entry the "read in full" mark k_read_table_cull clears
+    std::vector<b200vis_table_cull_inputs> h_tab_cull; b200vis_bounds_layout cull_layout{}; bool cull_attached = false;
+    DevTableCull *d_tab_cull = nullptr; uint8_t *d_tab_fresh = nullptr;
+    bool cull_fresh_pending = false;    // slots (re)mapped or tables (re)attached since the last RD_CULL_INPUTS read
     double step_t[6] = {0, 0, 0, 0, 0, 0}; uint64_t step_n = 0;   // B200VIS_STEP_TRACE: host time per phase of b200vis_step
     void *nccl_comm = nullptr;          // b200vis_comm_init
     uint32_t *d_gather = nullptr;       // [world][slab] when the library owns the exchange
@@ -242,7 +247,8 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_range_se, ctx->d_range_ua, ctx->d_range_views, ctx->d_visibility, ctx->d_iv_changed,
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
                    ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
-                   ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd};
+                   ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
+                   ctx->d_tab_cull, ctx->d_tab_fresh};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -2967,7 +2973,7 @@ static int32_t flush_table_updates(b200vis_ctx *ctx) {
     if (n_reset) memcpy(ctx->h_tab_stage + set_bytes, reset.data(), n_reset * 4);
     CU(cudaMemcpyAsync(ctx->d_tab_upd, ctx->h_tab_stage, bytes, cudaMemcpyHostToDevice, ctx->stream));
     launch_update_table_map(ctx->stream, ctx->d_tab_map, reinterpret_cast<const uint2 *>(ctx->d_tab_upd), (uint32_t)n_set, ctx->d_tvv_shadow,
-                            reinterpret_cast<const uint32_t *>(ctx->d_tab_upd + set_bytes), (uint32_t)n_reset);
+                            reinterpret_cast<const uint32_t *>(ctx->d_tab_upd + set_bytes), (uint32_t)n_reset, ctx->d_tab_fresh);
     CU(cudaGetLastError());
     CU(cudaEventRecord(ctx->ev_tab, ctx->stream));
     touched.clear(); reset.clear();
@@ -3010,6 +3016,101 @@ static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_t
         r = old_to_new[r];
         ctx->row_slot[r] = (uint32_t)i;
     }
+}
+
+// ---- registrations of the caller's columns: page-rounded ranges, overlapping ones merged; stale ones released before new
+// ones are made ----
+using Range = std::pair<uintptr_t, uintptr_t>;
+struct ColumnRanges { std::vector<Range> need, changed; };   // changed = memory that may have been reallocated
+
+static Range page_range(const void *p, size_t bytes) {
+    const uintptr_t page = (uintptr_t)sysconf(_SC_PAGESIZE), a = (uintptr_t)p;
+    return Range{a & ~(page - 1), (a + bytes + page - 1) & ~(page - 1)};
+}
+template <typename Fn>
+static void cull_columns(size_t cap, const b200vis_table_cull_inputs &cu, const b200vis_bounds_layout &bl, Fn &&fn) {
+    fn(cu.aabbs, cap * bl.aabb_stride); fn(cu.aabb_changed_ticks, cap * 4);
+    fn(cu.spheres, cap * bl.sphere_stride); fn(cu.sphere_changed_ticks, cap * 4);
+    fn(cu.inherited_visibility, cap); fn(cu.iv_changed_ticks, cap * 4);
+}
+// every column of a table: the outputs, the Transform input and the cull inputs, as (pointer, bytes)
+template <typename Fn>
+static void table_columns(const b200vis_table &tb, const b200vis_table_inputs &in, uint32_t trs_stride, const b200vis_table_cull_inputs &cu,
+                          const b200vis_bounds_layout &bl, Fn &&fn) {
+    const size_t cap = tb.capacity;
+    fn(tb.global_transforms, cap * 64); fn(tb.gt_changed_ticks, cap * 4);
+    fn(tb.view_visibility, cap); fn(tb.vv_changed_ticks, cap * 4);
+    fn(in.transforms, cap * trs_stride); fn(in.transform_changed_ticks, cap * 4);
+    cull_columns(cap, cu, bl, fn);
+}
+// a column the registry uses: registered by the library unless its owner pinned it
+static void need_column(b200vis_ctx *ctx, const void *p, size_t bytes, bool changed, ColumnRanges &cr) {
+    if (!p || !bytes) return;
+    if (changed) cr.changed.push_back(page_range(p, bytes));
+    bool ours = false;
+    for (const auto &r : ctx->host_regs) ours |= (uintptr_t)p >= r.first && (uintptr_t)p < r.first + r.second;
+    void *d = nullptr;
+    if (!ours && cudaHostGetDevicePointer(&d, const_cast<void *>(p), 0) == cudaSuccess) return;   // pinned by its owner
+    cudaGetLastError();
+    cr.need.push_back(page_range(p, bytes));
+}
+// A registered table as the kernels see it: the device aliases of its columns (NULL = not delivered).  The aliases are
+// derived again whenever registrations may have moved.
+static cudaError_t dev_table(const b200vis_table &tb, const b200vis_table_inputs &in, const b200vis_transform_layout &lay, uint32_t map_off,
+                             uint32_t chunk_begin, DevTable &out) {
+    void *alias[6] = {tb.global_transforms, tb.gt_changed_ticks, tb.view_visibility, tb.vv_changed_ticks,
+                      const_cast<void *>(in.transforms), const_cast<uint32_t *>(in.transform_changed_ticks)};
+    for (void *&p : alias) {
+        if (!p || !tb.capacity) { p = nullptr; continue; }
+        void *d = nullptr;
+        const cudaError_t e = cudaHostGetDevicePointer(&d, p, 0);
+        if (e != cudaSuccess) return e;
+        p = d;
+    }
+    out = DevTable{static_cast<float4 *>(alias[0]), static_cast<uint32_t *>(alias[1]), static_cast<uint8_t *>(alias[2]),
+                   static_cast<uint32_t *>(alias[3]), tb.len, map_off, chunk_begin, 0,
+                   static_cast<const uint8_t *>(alias[4]), static_cast<const uint32_t *>(alias[5]),
+                   lay.stride, lay.translation, lay.rotation, lay.scale};
+    return cudaSuccess;
+}
+
+// Releases the registrations no range of cr.need is and those overlapping cr.changed, then registers what is missing.
+// No table read or write-back may be in flight.  On failure every registration is released and the registry emptied.
+static int32_t register_columns(b200vis_ctx *ctx, ColumnRanges &cr, const char *who) {
+    std::sort(cr.need.begin(), cr.need.end());
+    std::vector<Range> merged;
+    for (const Range &r : cr.need) {
+        if (!merged.empty() && r.first < merged.back().second) merged.back().second = std::max(merged.back().second, r.second);
+        else merged.push_back(r);
+    }
+    std::vector<std::pair<uintptr_t, size_t>> regs;
+    ctx->n_tab_chunks = 0;   // until the caller commits its registry, no write-back or read reaches a released range
+    for (const auto &r : ctx->host_regs) {
+        const uintptr_t lo = r.first, hi = r.first + r.second;
+        bool stale = std::find(merged.begin(), merged.end(), Range{lo, hi}) == merged.end();
+        for (const Range &c : cr.changed) stale |= c.first < hi && lo < c.second;
+        if (stale) cudaHostUnregister(reinterpret_cast<void *>(lo));
+        else regs.push_back(r);
+    }
+    cudaGetLastError();
+    ctx->host_regs = regs;
+    for (const Range &r : merged) {
+        if (std::find(regs.begin(), regs.end(), std::make_pair(r.first, (size_t)(r.second - r.first))) != regs.end()) continue;
+        const cudaError_t e = cudaHostRegister(reinterpret_cast<void *>(r.first), r.second - r.first, cudaHostRegisterMapped | cudaHostRegisterPortable);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            for (const auto &q : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(q.first));
+            cudaGetLastError();
+            ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->h_tab_in.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
+            ctx->h_tab_cull.clear(); ctx->cull_attached = false;
+            std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
+            ctx->n_tab_chunks = 0;
+            return fail(ctx, B200VIS_ERR_CUDA, "%s: cudaHostRegister of %zu bytes at %p failed: %s", who, (size_t)(r.second - r.first),
+                        reinterpret_cast<void *>(r.first), cudaGetErrorString(e));
+        }
+        ctx->host_regs.emplace_back(r.first, (size_t)(r.second - r.first));
+    }
+    return B200VIS_OK;
 }
 
 extern "C" int32_t b200vis_set_tables(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table *tables) {
@@ -3081,80 +3182,27 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
         if (tables[t].view_visibility != ctx->h_tabs[t].view_visibility)   // a new column: its bytes are sent again
             for (uint32_t s = 0; s < keep; ++s) if (map[o + s] != kUnmapped) reset.push_back(map[o + s]);
     }
-    // ---- registrations: page-rounded column ranges, overlapping ones merged; stale ones released before new ones ----
-    using Range = std::pair<uintptr_t, uintptr_t>;
-    const uintptr_t page = (uintptr_t)sysconf(_SC_PAGESIZE);
-    auto ours = [&](uintptr_t p) {
-        for (const auto &r : ctx->host_regs) if (p >= r.first && p < r.first + r.second) return true;
-        return false;
+    // ---- registrations: every current column, plus the cull inputs of tables that stay (kept until they are attached
+    // again); the columns of moved tables, old and new, are memory that may have been reallocated ----
+    const b200vis_table_cull_inputs no_cull{};
+    auto kept_cull = [&](uint32_t t) -> const b200vis_table_cull_inputs & {
+        return t < n_old && t < ctx->h_tab_cull.size() && !moved(t) ? ctx->h_tab_cull[t] : no_cull;
     };
-    auto columns = [](const b200vis_table &tb, const b200vis_table_inputs &in, uint32_t stride, auto &&fn) {
-        const size_t cap = tb.capacity;
-        fn((void *)tb.global_transforms, cap * 64); fn((void *)tb.gt_changed_ticks, cap * 4);
-        fn((void *)tb.view_visibility, cap); fn((void *)tb.vv_changed_ticks, cap * 4);
-        fn((void *)in.transforms, cap * stride); fn((void *)in.transform_changed_ticks, cap * 4);
-    };
-    auto rounded = [&](void *p, size_t bytes) { const uintptr_t a = (uintptr_t)p; return Range{a & ~(page - 1), (a + bytes + page - 1) & ~(page - 1)}; };
-    std::vector<Range> need, changed;
+    ColumnRanges cr;
     for (uint32_t t = 0; t < n_tables; ++t)
-        columns(tables[t], input(t), lay.stride, [&](void *p, size_t bytes) {
-            if (!p || !bytes) return;
-            if (moved(t)) changed.push_back(rounded(p, bytes));
-            void *d = nullptr;
-            if (!ours((uintptr_t)p) && cudaHostGetDevicePointer(&d, p, 0) == cudaSuccess) return;   // pinned by its owner
-            cudaGetLastError();
-            need.push_back(rounded(p, bytes));
-        });
+        table_columns(tables[t], input(t), lay.stride, kept_cull(t), ctx->cull_layout,
+                      [&](const void *p, size_t bytes) { need_column(ctx, p, bytes, moved(t), cr); });
     for (uint32_t t = 0; t < n_old; ++t)
         if (moved(t))
-            columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride,
-                    [&](void *p, size_t bytes) { if (p && bytes) changed.push_back(rounded(p, bytes)); });
-    std::sort(need.begin(), need.end());
-    std::vector<Range> merged;
-    for (const Range &r : need) {
-        if (!merged.empty() && r.first < merged.back().second) merged.back().second = std::max(merged.back().second, r.second);
-        else merged.push_back(r);
-    }
-    std::vector<std::pair<uintptr_t, size_t>> regs;
-    ctx->n_tab_chunks = 0;   // until the new registry is committed, no write-back reaches a released range
-    for (const auto &r : ctx->host_regs) {
-        const uintptr_t lo = r.first, hi = r.first + r.second;
-        bool stale = std::find(merged.begin(), merged.end(), Range{lo, hi}) == merged.end();
-        for (const Range &c : changed) stale |= c.first < hi && lo < c.second;
-        if (stale) cudaHostUnregister(reinterpret_cast<void *>(lo));
-        else regs.push_back(r);
-    }
-    cudaGetLastError();
-    ctx->host_regs = regs;
-    for (const Range &r : merged) {
-        if (std::find(regs.begin(), regs.end(), std::make_pair(r.first, (size_t)(r.second - r.first))) != regs.end()) continue;
-        const cudaError_t e = cudaHostRegister(reinterpret_cast<void *>(r.first), r.second - r.first, cudaHostRegisterMapped | cudaHostRegisterPortable);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            for (const auto &q : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(q.first));
-            cudaGetLastError();
-            ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->h_tab_in.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
-            std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
-            ctx->n_tab_chunks = 0;
-            return fail(ctx, B200VIS_ERR_CUDA, "set_tables: cudaHostRegister of %zu bytes at %p failed: %s", (size_t)(r.second - r.first),
-                        reinterpret_cast<void *>(r.first), cudaGetErrorString(e));
-        }
-        ctx->host_regs.emplace_back(r.first, (size_t)(r.second - r.first));
-    }
+            table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, t < ctx->h_tab_cull.size() ? ctx->h_tab_cull[t] : no_cull,
+                          ctx->cull_layout, [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); });
+    { const int32_t rrc = register_columns(ctx, cr, "set_tables"); if (rrc) return rrc; }
     // ---- the device registry: table descriptors, chunk -> table, and the maps when their layout changed ----
     std::vector<DevTable> dt(n_tables);
     std::vector<uint32_t> chunk_table((size_t)chunks);
     for (uint32_t t = 0, c = 0; t < n_tables; ++t) {
-        const b200vis_table &tb = tables[t];
-        const b200vis_table_inputs &in = input(t);
-        void *alias[6] = {tb.global_transforms, tb.gt_changed_ticks, tb.view_visibility, tb.vv_changed_ticks,
-                          const_cast<void *>(in.transforms), const_cast<uint32_t *>(in.transform_changed_ticks)};
-        for (void *&p : alias) if (p && tb.capacity) { void *d = nullptr; CU(cudaHostGetDevicePointer(&d, p, 0)); p = d; } else p = nullptr;
-        dt[t] = DevTable{static_cast<float4 *>(alias[0]), static_cast<uint32_t *>(alias[1]), static_cast<uint8_t *>(alias[2]),
-                         static_cast<uint32_t *>(alias[3]), tb.len, off[t], c, 0,
-                         static_cast<const uint8_t *>(alias[4]), static_cast<const uint32_t *>(alias[5]),
-                         lay.stride, lay.translation, lay.rotation, lay.scale};
-        for (uint32_t k = 0; k < (tb.len + 127u) / 128u; ++k) chunk_table[c++] = t;
+        CU(dev_table(tables[t], input(t), lay, off[t], c, dt[t]));
+        for (uint32_t k = 0; k < (tables[t].len + 127u) / 128u; ++k) chunk_table[c++] = t;
     }
     const size_t N = ctx->cfg.max_entities;
     if (!ctx->d_tabs) CU(dalloc(&ctx->d_tabs, B200VIS_MAX_TABLES));
@@ -3178,8 +3226,22 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
     if (chunks) CU(cudaMemcpyAsync(ctx->d_tab_chunks, chunk_table.data(), (size_t)chunks * 4, cudaMemcpyHostToDevice, st));
     if (!same_layout && total) CU(cudaMemcpyAsync(ctx->d_tab_map, map.data(), (size_t)total * 4, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync(ctx->d_tab_total, &total32, 4, cudaMemcpyHostToDevice, st));
+    uint8_t *old_fresh = nullptr;
+    if (!same_layout || !ctx->d_tab_fresh) {
+        // the "read in full" marks move with the map entries that carry over (the cull inputs of a table that stays
+        // are attached again without a full read)
+        old_fresh = ctx->d_tab_fresh; ctx->d_tab_fresh = nullptr;
+        CU(dalloc(&ctx->d_tab_fresh, std::max<size_t>(ctx->tab_map_cap, 1)));
+        for (uint32_t t = 0; old_fresh && t < std::min(n_old, n_tables); ++t) {
+            const uint32_t keep = std::min(tables[t].capacity, ctx->h_tabs[t].capacity);
+            if (keep) CU(cudaMemcpyAsync(ctx->d_tab_fresh + off[t], old_fresh + ctx->tab_off[t], keep, cudaMemcpyDeviceToDevice, st));
+        }
+    }
     CU(cudaStreamSynchronize(st));
+    if (old_fresh) cudaFree(old_fresh);
     // ---- commit ----
+    // slots that come below len may hold "read in full" marks a cull read skipped while they were past it
+    for (uint32_t t = 0; t < n_tables; ++t) ctx->cull_fresh_pending |= tables[t].len > (t < n_old ? ctx->h_tabs[t].len : 0u);
     ctx->h_tabs.assign(tables, tables + n_tables);
     ctx->h_tab_in.resize(n_tables);
     for (uint32_t t = 0; t < n_tables; ++t) ctx->h_tab_in[t] = input(t);
@@ -3190,6 +3252,7 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
     for (size_t i = 0; i < ctx->h_tab_map.size(); ++i) if (ctx->h_tab_map[i] != kUnmapped) ctx->row_slot[ctx->h_tab_map[i]] = (uint32_t)i;
     ctx->n_tab_chunks = (uint32_t)chunks;
     ctx->tables_set = true;
+    ctx->cull_attached = false;              // the cull inputs are attached again by b200vis_set_table_cull_inputs
     queue_table_updates(ctx, {}, reset);
     return B200VIS_OK;
 }
@@ -3223,7 +3286,156 @@ extern "C" int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uint
         ctx->h_tab_map[e] = r;
         touched.push_back(e);
     }
+    ctx->cull_fresh_pending |= !touched.empty();
     queue_table_updates(ctx, touched, reset);
+    return B200VIS_OK;
+}
+
+static bool cull_reads(const b200vis_table_cull_inputs &c) {
+    return c.aabbs || c.spheres || c.inherited_visibility || c.flags;
+}
+// the same columns, flags and used layout fields: the table needs no full read
+static bool cull_same(const b200vis_table_cull_inputs &a, const b200vis_bounds_layout &la, const b200vis_table_cull_inputs &b,
+                      const b200vis_bounds_layout &lb) {
+    return a.aabbs == b.aabbs && a.aabb_changed_ticks == b.aabb_changed_ticks && a.spheres == b.spheres &&
+           a.sphere_changed_ticks == b.sphere_changed_ticks && a.inherited_visibility == b.inherited_visibility &&
+           a.iv_changed_ticks == b.iv_changed_ticks && a.flags == b.flags &&
+           (!a.aabbs || (la.aabb_stride == lb.aabb_stride && la.aabb_center == lb.aabb_center && la.aabb_half_extents == lb.aabb_half_extents)) &&
+           (!a.spheres || a.aabbs || (la.sphere_stride == lb.sphere_stride && la.sphere_center == lb.sphere_center && la.sphere_radius == lb.sphere_radius));
+}
+
+extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_cull_inputs *inputs,
+                                                 const b200vis_bounds_layout *layout) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_table_cull_inputs: world_size > 1");
+    if (!ctx->tables_set || ctx->h_tabs.empty()) return fail(ctx, B200VIS_ERR_NOT_READY, "set_table_cull_inputs: no tables are registered");
+    if (n_tables != ctx->h_tabs.size())
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: %u entries for %zu registered tables", n_tables, ctx->h_tabs.size());
+    if (!inputs) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: null inputs");
+    constexpr uint32_t kArchetypeBits = B200VIS_F_NO_FRUSTUM_CULLING | B200VIS_F_HAS_VIS_RANGE | B200VIS_F_NO_CPU_CULLING | B200VIS_F_SPHERE_FROM_GT;
+    bool any_aabb = false, any_sphere = false;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const b200vis_table_cull_inputs &c = inputs[t];
+        if ((c.aabbs == nullptr) != (c.aabb_changed_ticks == nullptr) || (c.spheres == nullptr) != (c.sphere_changed_ticks == nullptr) ||
+            (c.inherited_visibility == nullptr) != (c.iv_changed_ticks == nullptr))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: table %u: a column and its ticks must both be NULL or both be set", t);
+        // the kernel reads f32 fields and u32 ticks
+        if ((uintptr_t)c.aabbs % 4u || (uintptr_t)c.spheres % 4u || (uintptr_t)c.aabb_changed_ticks % 4u ||
+            (uintptr_t)c.sphere_changed_ticks % 4u || (uintptr_t)c.iv_changed_ticks % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: table %u: columns need 4-byte alignment", t);
+        if (c.flags & ~kArchetypeBits)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: table %u: flags 0x%x has bits other than the per-archetype ones", t, c.flags);
+        any_aabb |= c.aabbs != nullptr; any_sphere |= c.spheres != nullptr;
+    }
+    if ((any_aabb || any_sphere) && !layout)
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: a table has aabbs or spheres but no layout was given");
+    auto check_struct = [&](const char *name, uint32_t stride, const uint64_t (&lo)[2], const uint64_t (&sz)[2]) -> int32_t {
+        if (stride % 4u || lo[0] % 4u || lo[1] % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: %s layout fields and stride need 4-byte alignment", name);
+        for (int i = 0; i < 2; ++i)
+            if (lo[i] + sz[i] > stride)
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: %s field at %llu runs past stride %u", name, (unsigned long long)lo[i], stride);
+        if (lo[0] < lo[1] + sz[1] && lo[1] < lo[0] + sz[0])
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: %s fields at %llu and %llu overlap", name,
+                        (unsigned long long)lo[0], (unsigned long long)lo[1]);
+        return B200VIS_OK;
+    };
+    if (any_aabb) {
+        const int32_t rc = check_struct("Aabb", layout->aabb_stride, {layout->aabb_center, layout->aabb_half_extents}, {12, 12});
+        if (rc) return rc;
+    }
+    if (any_sphere) {
+        const int32_t rc = check_struct("Sphere", layout->sphere_stride, {layout->sphere_center, layout->sphere_radius}, {12, 4});
+        if (rc) return rc;
+    }
+    b200vis_bounds_layout lay{};
+    if (any_aabb) { lay.aabb_stride = layout->aabb_stride; lay.aabb_center = layout->aabb_center; lay.aabb_half_extents = layout->aabb_half_extents; }
+    if (any_sphere) { lay.sphere_stride = layout->sphere_stride; lay.sphere_center = layout->sphere_center; lay.sphere_radius = layout->sphere_radius; }
+    CU(cudaStreamSynchronize(ctx->stream));   // no read in flight reads the old cull columns or registrations
+    const b200vis_table_cull_inputs none{};
+    auto prev = [&](uint32_t t) -> const b200vis_table_cull_inputs & { return t < ctx->h_tab_cull.size() ? ctx->h_tab_cull[t] : none; };
+    std::vector<bool> full(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t) full[t] = cull_reads(inputs[t]) && !cull_same(inputs[t], lay, prev(t), ctx->cull_layout);
+    // ---- registrations: every table's columns with the new cull inputs; cull columns that changed may be reallocated ----
+    const uint32_t chunks = ctx->n_tab_chunks;
+    ColumnRanges cr;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const bool moved = !cull_same(inputs[t], lay, prev(t), ctx->cull_layout);
+        table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, inputs[t], lay,
+                      [&](const void *p, size_t bytes) { need_column(ctx, p, bytes, false, cr); });
+        if (moved) {
+            auto changed = [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); };
+            cull_columns(ctx->h_tabs[t].capacity, inputs[t], lay, changed);
+            cull_columns(ctx->h_tabs[t].capacity, prev(t), ctx->cull_layout, changed);
+        }
+    }
+    { const int32_t rrc = register_columns(ctx, cr, "set_table_cull_inputs"); if (rrc) return rrc; }
+    ctx->n_tab_chunks = chunks;
+    // From here on registrations may have moved: a failure detaches the cull inputs (nothing reads them until the next
+    // call, which reads every table it attaches in full) instead of leaving the device pointed at released ranges.
+    auto detach = [&](cudaError_t e, const char *what, uint32_t t) {
+        ctx->cull_attached = false;
+        ctx->h_tab_cull.clear();
+        return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA,
+                    "set_table_cull_inputs: table %u: %s: %s", t, what, cudaGetErrorString(e));
+    };
+    // ---- the registry's descriptors again: an output or Transform column sharing a page with a cull column may have
+    // been registered anew, and its device alias is derived from the registration ----
+    std::vector<DevTable> dt(n_tables);
+    for (uint32_t t = 0, c = 0; t < n_tables; ++t) {
+        const cudaError_t e = dev_table(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout, ctx->tab_off[t], c, dt[t]);
+        if (e != cudaSuccess) return detach(e, "no device alias for a registered column", t);
+        c += (ctx->h_tabs[t].len + 127u) / 128u;
+    }
+    // ---- the device form of the cull inputs, and the full-read marks of the tables attached anew ----
+    std::vector<DevTableCull> dc(n_tables);
+    bool any = false;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const b200vis_table_cull_inputs &c = inputs[t];
+        const uint32_t cap = ctx->h_tabs[t].capacity;
+        cudaError_t lost = cudaSuccess;
+        auto alias = [&](const void *p) -> const void * {
+            void *d = nullptr;
+            if (!p || !cap) return nullptr;
+            const cudaError_t e = cudaHostGetDevicePointer(&d, const_cast<void *>(p), 0);
+            if (e != cudaSuccess) lost = e;
+            return d;
+        };
+        const bool aabb = c.aabbs != nullptr;
+        DevTableCull &d = dc[t];
+        d.bnd = static_cast<const uint8_t *>(alias(aabb ? c.aabbs : c.spheres));
+        d.bnd_ticks = static_cast<const uint32_t *>(alias(aabb ? c.aabb_changed_ticks : c.sphere_changed_ticks));
+        d.iv = static_cast<const uint8_t *>(alias(c.inherited_visibility));
+        d.iv_ticks = static_cast<const uint32_t *>(alias(c.iv_changed_ticks));
+        if (lost != cudaSuccess) return detach(lost, "no device alias for a registered column", t);
+        d.flags = c.flags | (aabb ? B200VIS_F_HAS_AABB : c.spheres ? B200VIS_F_HAS_SPHERE : 0u);
+        d.read = cull_reads(c) && cap ? 1u : 0u;
+        d.stride = aabb ? lay.aabb_stride : lay.sphere_stride;
+        d.c_off = aabb ? lay.aabb_center : lay.sphere_center;
+        d.e_off = aabb ? lay.aabb_half_extents : lay.sphere_radius;
+        d.is_aabb = aabb;
+        any |= d.read != 0;
+    }
+    cudaStream_t st = ctx->stream;
+    cudaError_t e = cudaSuccess;
+    if (!ctx->d_tab_cull && (e = dalloc(&ctx->d_tab_cull, B200VIS_MAX_TABLES)) != cudaSuccess) return detach(e, "cudaMalloc", 0);
+    if ((e = cudaMemcpyAsync(ctx->d_tabs, dt.data(), dt.size() * sizeof(DevTable), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+        return detach(e, "table descriptors", 0);
+    if ((e = cudaMemcpyAsync(ctx->d_tab_cull, dc.data(), dc.size() * sizeof(DevTableCull), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+        return detach(e, "cull descriptors", 0);
+    bool pending = false;
+    for (uint32_t t = 0; t < n_tables; ++t)
+        if (full[t] && ctx->h_tabs[t].capacity) {
+            if ((e = cudaMemsetAsync(ctx->d_tab_fresh + ctx->tab_off[t], 1, ctx->h_tabs[t].capacity, st)) != cudaSuccess)
+                return detach(e, "full-read marks", t);
+            pending = true;
+        }
+    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return detach(e, "cudaStreamSynchronize", 0);
+    // ---- commit ----
+    ctx->cull_fresh_pending |= pending;
+    ctx->h_tab_cull.assign(inputs, inputs + n_tables);
+    ctx->cull_layout = lay;
+    ctx->cull_attached = any;
     return B200VIS_OK;
 }
 
@@ -3243,11 +3455,18 @@ extern "C" int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_
     CHECK_CTX();
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "read_tables: world_size > 1");
     if (!ctx->tables_set || ctx->h_tabs.empty()) return fail(ctx, B200VIS_ERR_NOT_READY, "read_tables: no tables are registered");
-    which &= B200VIS_RD_TRANSFORM | B200VIS_RD_GLOBAL_TRANSFORM;
     { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }
     const TableBufs tb{ctx->d_tabs, ctx->d_tab_chunks, ctx->n_tab_chunks, ctx->d_tab_map, ctx->d_tvv_shadow};
-    launch_read_tables(ctx->stream, ctx->rows, tb, which, last_run, this_run);
+    launch_read_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_RD_TRANSFORM | B200VIS_RD_GLOBAL_TRANSFORM), last_run, this_run);
     CU(cudaGetLastError());
+    if ((which & B200VIS_RD_CULL_INPUTS) && ctx->cull_attached) {
+        launch_read_table_cull(ctx->stream, ctx->rows, tb, ctx->d_tab_cull, ctx->d_tab_fresh, last_run, this_run);
+        CU(cudaGetLastError());
+        ctx->bounds_set = true;
+        // F_SPHERE_FROM_GT and HAS_AABB change on full reads only, and the host queued every one of them: the light rows
+        // are verified again only then, so a steady-state read adds no synchronisation
+        if (ctx->cull_fresh_pending) { ctx->lights_tag_dirty = true; ctx->cull_fresh_pending = false; }
+    }
     if (which & B200VIS_RD_GLOBAL_TRANSFORM) {
         // whether a slot was newer is known only on the device: the next propagate takes the marked instantiation
         bool gt_inputs = false;

@@ -283,6 +283,16 @@ struct TableBufs {
     const uint32_t *map;           // slot -> row of every table, 0xFFFFFFFF = unmapped
     uint8_t *vv_shadow;            // per row: the ViewVisibility byte its slot holds (0xFF = unknown)
 };
+// b200vis_set_table_cull_inputs: one table's cull inputs as k_read_table_cull sees them (device aliases, nullptr = absent).
+// bnd is the Aabb column, or the Sphere column of a table without Aabb.
+struct DevTableCull {
+    const uint8_t *bnd; const uint32_t *bnd_ticks;
+    const uint8_t *iv; const uint32_t *iv_ticks;
+    uint32_t flags;          // the table's per-archetype bits | HAS_AABB / HAS_SPHERE
+    uint32_t read;           // 0 = the table is not read
+    uint32_t stride, c_off, e_off;   // bytes per slot, center, half_extents (Aabb) or radius (Sphere)
+    uint32_t is_aabb;
+};
 
 // b200vis_compact_topology: row-valued lists (list l = rows[l * stride .. + count[l * count_step]))
 struct RowLists {

@@ -3191,11 +3191,57 @@ k_read_tables(Rows R, TableBufs tb, uint32_t which, uint32_t last_run, uint32_t 
     }
 }
 
+// ---- table read of the cull inputs (b200vis_read_tables with RD_CULL_INPUTS): the chunk walk of k_read_tables over the
+// Aabb / Sphere ticks and the InheritedVisibility ticks.  fresh[entry] marks a slot (re)mapped or a table (re)attached
+// since the last such read: that slot is read in full (flags rebuilt from the table's) and its mark cleared.  Otherwise
+// only newer columns are read, so only newer or fresh slots touch their map entry and their 4 to 32 bytes of payload.
+__global__ void __launch_bounds__(256)
+k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, uint8_t *__restrict__ fresh, uint32_t last_run,
+                  uint32_t this_run) {
+    __shared__ uint4 s_tk[8][2][33];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
+        const uint32_t t = tb.chunk_table[ch];
+        const DevTableCull C = cull[t];
+        if (!C.read) continue;                                // the same for the whole warp
+        const DevTable &T = tb.tables[t];
+        const uint32_t len = T.len, map_off = T.map_off;
+        const uint32_t base = (ch - T.chunk_begin) * 128u, n = min(len - base, 128u);
+        const uint32_t hb = C.bnd ? stage_ticks(C.bnd_ticks, base, base + n, lane, s_tk[warp][0]) : 0u;
+        const uint32_t hi = C.iv ? stage_ticks(C.iv_ticks, base, base + n, lane, s_tk[warp][1]) : 0u;
+        __syncwarp();
+        const uint32_t *tbnd = reinterpret_cast<const uint32_t *>(s_tk[warp][0]) + hb;
+        const uint32_t *tiv = reinterpret_cast<const uint32_t *>(s_tk[warp][1]) + hi;
+        for (uint32_t i = lane; i < n; i += 32u) {
+            const uint32_t slot = base + i, e = map_off + slot;
+            const bool full = fresh[e] != 0;
+            const bool nb = C.bnd && tick_is_newer(tbnd[i], last_run, this_run);
+            const bool ni = C.iv && tick_is_newer(tiv[i], last_run, this_run);
+            if (!full && !nb && !ni) continue;
+            if (full) fresh[e] = 0;
+            const uint32_t row = tb.map[e];
+            if (row == kNoParent) continue;
+            if (C.bnd && (full || nb)) {                      // what k_unpack_bounds stores; no Aabb / Sphere: bounds kept
+                const uint8_t *p = C.bnd + (size_t)slot * C.stride;
+                const float *c = reinterpret_cast<const float *>(p + C.c_off), *x = reinterpret_cast<const float *>(p + C.e_off);
+                R.bndA[row] = make_float4(c[0], c[1], c[2], x[0]);
+                R.bndB[row] = C.is_aabb ? make_float2(x[1], x[2]) : make_float2(0.0f, 0.0f);
+            }
+            if (full || ni) {
+                const uint32_t iv = C.iv && C.iv[slot] ? (uint32_t)F_INHERITED : 0u;
+                const uint32_t f = R.flags[row];
+                R.flags[row] = (uint8_t)(full ? (C.flags | iv | (f & F_TCHANGED)) : ((f & ~(uint32_t)F_INHERITED) | iv));
+            }
+        }
+        __syncwarp();                                         // the slab is the warp's next chunk's
+    }
+}
+
 __global__ void __launch_bounds__(256) k_update_table_map(uint32_t *__restrict__ map, const uint2 *__restrict__ set, uint32_t n_set,
                                                           uint8_t *__restrict__ vv_shadow, const uint32_t *__restrict__ reset,
-                                                          uint32_t n_reset) {
+                                                          uint32_t n_reset, uint8_t *__restrict__ fresh) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n_set) map[set[i].x] = set[i].y;
+    if (i < n_set) { map[set[i].x] = set[i].y; fresh[set[i].x] = 1; }
     if (i < n_reset) vv_shadow[reset[i]] = 0xFF;
 }
 
@@ -4060,10 +4106,16 @@ void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uin
     const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
     ++g_launches; k_read_tables<<<grid, 256, 0, st>>>(R, tb, which, last_run, this_run);
 }
+void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
+                            uint32_t last_run, uint32_t this_run) {
+    if (!tb.n_chunks) return;
+    const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
+    ++g_launches; k_read_table_cull<<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run);
+}
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
-                             uint32_t n_reset) {
+                             uint32_t n_reset, uint8_t *fresh) {
     const uint32_t n = std::max(n_set, n_reset);
-    if (n) { ++g_launches; k_update_table_map<<<cdiv(n, 256), 256, 0, st>>>(map, set, n_set, vv_shadow, reset, n_reset); }
+    if (n) { ++g_launches; k_update_table_map<<<cdiv(n, 256), 256, 0, st>>>(map, set, n_set, vv_shadow, reset, n_reset, fresh); }
 }
 void launch_record_push(cudaStream_t st, const uint32_t *block, uint32_t block_words, const ClusterBufs &cb) {
     ++g_launches; k_record_push<<<cb.world, 256, 0, st>>>(block, block_words, cb);

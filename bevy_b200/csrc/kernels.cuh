@@ -50,9 +50,12 @@ void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, ui
 void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
 // b200vis_read_tables: which = B200VIS_RD_* bits, slots newer by Tick::is_newer_than(last_run, this_run)
 void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t last_run, uint32_t this_run);
-// set_table_rows / set_tables / edit_topology: map[set[i].x] = set[i].y, then vv_shadow[reset[i]] = 0xFF
+// b200vis_read_tables with RD_CULL_INPUTS: cull[t] = table t's cull inputs, fresh[entry] = read the slot in full (cleared)
+void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
+                            uint32_t last_run, uint32_t this_run);
+// set_table_rows / set_tables / edit_topology: map[set[i].x] = set[i].y and fresh[set[i].x] = 1, then vv_shadow[reset[i]] = 0xFF
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
-                             uint32_t n_reset);
+                             uint32_t n_reset, uint8_t *fresh);
 void launch_record_push(cudaStream_t st, const uint32_t *block, uint32_t block_words, const ClusterBufs &cb);
 void launch_slab_push(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, uint32_t *done, uint32_t max_views);
 void launch_cluster_lists(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, DevStats *stats, uint32_t max_views);

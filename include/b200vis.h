@@ -549,7 +549,59 @@ B200VIS_API int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, c
  * registered), UNSUPPORTED (world_size > 1). */
 #define B200VIS_RD_TRANSFORM        0x1u
 #define B200VIS_RD_GLOBAL_TRANSFORM 0x2u
+#define B200VIS_RD_CULL_INPUTS      0x4u   /* b200vis_set_table_cull_inputs' columns, see below */
 B200VIS_API int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_t last_run, uint32_t this_run);
+
+/* ---- reading the cull inputs (Aabb, Sphere, InheritedVisibility) straight from the same tables ------------------------------
+ * Aabb (primitives.rs:65) and Sphere (primitives.rs:199) are repr(Rust): their layouts are passed in (size_of and offset_of!
+ * of their fields).  Every field is f32: center and half_extents are lanes 0-2 of a Vec3A, radius one float.
+ * The other inputs of check_visibility_cpu_culling (Has<NoFrustumCulling>, Has<VisibilityRange>, Without<NoCpuCulling>, a
+ * point light's Sphere rebuilt from its GlobalTransform) are fixed for an archetype, so they are given once per table in
+ * `flags`.  VisibilityClass, RenderLayers and the VisibleEntityRanges mask are not read: b200vis_upload_bounds carries them. */
+typedef struct b200vis_bounds_layout {
+    uint32_t aabb_stride, aabb_center, aabb_half_extents;   /* bytes; each field is 3 floats */
+    uint32_t sphere_stride, sphere_center, sphere_radius;   /* center 3 floats, radius 1 float */
+} b200vis_bounds_layout;
+typedef struct b200vis_table_cull_inputs {
+    const void     *aabbs;                 /* [capacity] Aabb; NULL = the archetype has no Aabb */
+    const uint32_t *aabb_changed_ticks;    /* [capacity]; NULL exactly when aabbs is */
+    const void     *spheres;               /* [capacity] Sphere; NULL = no Sphere */
+    const uint32_t *sphere_changed_ticks;  /* [capacity]; NULL exactly when spheres is */
+    const uint8_t  *inherited_visibility;  /* [capacity] InheritedVisibility (bool); NULL = not in the visibility query */
+    const uint32_t *iv_changed_ticks;      /* [capacity]; NULL exactly when inherited_visibility is */
+    uint32_t        flags;                 /* per-archetype bits only: B200VIS_F_NO_FRUSTUM_CULLING | _HAS_VIS_RANGE |
+                                              _NO_CPU_CULLING | _SPHERE_FROM_GT */
+} b200vis_table_cull_inputs;
+/* inputs[t] belongs to table t of the current registry: n_tables must equal its size.  The call replaces the previous
+ * cull inputs.  An entry with every pointer NULL and flags 0 leaves its table unread.  b200vis_set_tables / _ex replace
+ * the registry and drop all cull inputs (nothing is read for them until this call attaches them again); the columns of a
+ * table whose registry entry did not change stay registered until then.
+ * The columns are registered, merged with the output and input columns, kept and released by the code of
+ * b200vis_set_tables_ex, and the page rules above apply to them.
+ * When table t's entry (its pointers, its flags, or the part of the layout it uses) differs from entry t of the previous
+ * call, every slot of the table is read in full at the next RD_CULL_INPUTS read: a reallocated table, a table that had no
+ * cull inputs before.
+ * B200VIS_RD_CULL_INPUTS gives each row the device state b200vis_upload_bounds gives it for the row's bounds and flags
+ * (class mask, RenderLayers and the range mask stay as they are).  A slot is considered when it is below len, is mapped
+ * to a live row and its table is read.  It is read in full when it was (re)mapped by b200vis_set_table_rows since the
+ * last RD_CULL_INPUTS read, or its table was (re)attached as above; otherwise each column is read only where its tick is
+ * newer by the Tick::is_newer_than rule of b200vis_read_tables.
+ *   flags    (full read) the table's flags, | HAS_AABB if it has aabbs, | HAS_SPHERE if it has spheres and no aabbs
+ *            (Aabb takes precedence, visibility/mod.rs:824-843), | INHERITED_VISIBLE if the byte is nonzero; the row's
+ *            Changed<Transform> mark is kept
+ *   Aabb     (full read or newer tick) bounds = center.xyz, half_extents.xyz
+ *   Sphere   (a table without aabbs; full read or newer tick) bounds = center.xyz, radius, 0, 0
+ *   InheritedVisibility (newer tick) bit INHERITED_VISIBLE of the flags only
+ * A table with neither Aabb nor Sphere leaves the rows' bounds as they are.  Rows in no read table keep what
+ * b200vis_upload_bounds gave them.  The maps' "(re)mapped" marks survive an RD_TRANSFORM read and
+ * b200vis_compact_topology; b200vis_set_topology unmaps every slot, so the rows mapped again are read in full.
+ * Errors: INVALID_ARG (n_tables differs from the registry's size, only one pointer of a column pair NULL, a pointer not
+ * 4-byte aligned, a layout field not 4-byte aligned, overlapping or past its stride, no layout while some table has aabbs
+ * or spheres, flags other than the four per-archetype bits), NOT_READY (no tables registered), UNSUPPORTED
+ * (world_size > 1); nothing changes then.  On B200VIS_ERR_CUDA the registry is left empty when cudaHostRegister refused
+ * the memory, and otherwise every cull input is detached (the next call reads every table it attaches in full). */
+B200VIS_API int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_cull_inputs *inputs,
+                                                  const b200vis_bounds_layout *layout);
 
 /* ---- SURVEY.md 8(f) N1: the render world's visible-entity diff ---------------------------------------------
  * RenderVisibleEntitiesClass::update_cpu_culled_entities (crates/bevy_render/src/view/visibility/mod.rs:194-249)

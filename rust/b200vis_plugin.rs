@@ -15,9 +15,10 @@
 //! byte) composing correctly (SURVEY.md 8b).  With a three-line patch that makes those two systems removable, the device's
 //! ViewVisibility bytes + change bits can be written straight into the column instead (`forked-bevy` feature below).
 //!
-//! Data flow (INTEGRATION.md section 2): Transform and other systems' GlobalTransforms read by the device straight from
-//! the archetype tables by their change ticks (`b200vis_set_tables_ex`, `b200vis_read_tables`); other ECS columns ->
-//! `upload_*` on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
+//! Data flow (INTEGRATION.md section 2): Transform, other systems' GlobalTransforms, and the cull inputs Aabb, Sphere and
+//! InheritedVisibility read by the device straight from the archetype tables by their change ticks
+//! (`b200vis_set_tables_ex`, `b200vis_set_table_cull_inputs`, `b200vis_read_tables`); VisibilityClass, RenderLayers and
+//! the VisibleEntityRanges masks -> `upload_bounds` on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
 //! `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system; GlobalTransform (and, forked,
 //! ViewVisibility) with their change ticks straight into the archetype tables (`b200vis_writeback_tables`).
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
@@ -61,6 +62,11 @@ pub struct b200vis_table { global_transforms: *mut GlobalTransform, gt_changed_t
 #[repr(C)] pub struct b200vis_transform_layout { stride: u32, translation: u32, rotation: u32, scale: u32 }
 #[repr(C)] #[derive(Clone, Copy, PartialEq)]
 pub struct b200vis_table_inputs { transforms: *const Transform, transform_changed_ticks: *const Tick }
+#[repr(C)] pub struct b200vis_bounds_layout { aabb_stride: u32, aabb_center: u32, aabb_half_extents: u32, sphere_stride: u32,
+                                             sphere_center: u32, sphere_radius: u32 }
+#[repr(C)] #[derive(Clone, Copy, PartialEq)]
+pub struct b200vis_table_cull_inputs { aabbs: *const Aabb, aabb_changed_ticks: *const Tick, spheres: *const Sphere,
+    sphere_changed_ticks: *const Tick, inherited_visibility: *const InheritedVisibility, iv_changed_ticks: *const Tick, flags: u32 }
 
 #[link(name = "b200vis")]
 extern "C" {
@@ -92,13 +98,15 @@ extern "C" {
     fn b200vis_set_tables_ex(ctx: *mut b200vis_ctx, n: u32, tables: *const b200vis_table, inputs: *const b200vis_table_inputs,
                              layout: *const b200vis_transform_layout) -> i32;
     fn b200vis_read_tables(ctx: *mut b200vis_ctx, which: u32, last_run: u32, this_run: u32) -> i32;
+    fn b200vis_set_table_cull_inputs(ctx: *mut b200vis_ctx, n: u32, inputs: *const b200vis_table_cull_inputs,
+                                     layout: *const b200vis_bounds_layout) -> i32;
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
 const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2; const UNMAPPED: u32 = 0xFFFF_FFFF;
-const RD_TRANSFORM: u32 = 1; const RD_GLOBAL_TRANSFORM: u32 = 2;
+const RD_TRANSFORM: u32 = 1; const RD_GLOBAL_TRANSFORM: u32 = 2; const RD_CULL_INPUTS: u32 = 4;
 const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04; const F_NO_FRUSTUM: u8 = 0x08;
-const F_RANGE: u8 = 0x10; const F_SPHERE_FROM_GT: u8 = 0x40;
+const F_RANGE: u8 = 0x10; const F_NO_CPU_CULLING: u8 = 0x20; const F_SPHERE_FROM_GT: u8 = 0x40;
 const VIEW_ACTIVE: u8 = 1; const VIEW_NO_CPU_CULLING: u8 = 2;
 const ERR_HIERARCHY_CYCLE: i32 = 4;
 const MAX_CAMERAS: usize = 32; const MAX_CLUSTERS: usize = 4096;
@@ -127,9 +135,10 @@ pub struct B200Vis {
     visible_rows: Vec<u32>, visible_classes: Vec<u8>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
     planes_scratch: Vec<f32>,
     // the archetype tables registered with b200vis_set_tables_ex (one entry per table holding GlobalTransform, with its
-    // Transform column and in the forked build its ViewVisibility column), the entities each slot map was built from, and
-    // the rows epoch of the maps
-    tables: Vec<b200vis_table>, table_inputs: Vec<b200vis_table_inputs>, table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
+    // Transform column and in the forked build its ViewVisibility column), their cull inputs, the entities each slot map
+    // was built from, and the rows epoch of the maps
+    tables: Vec<b200vis_table>, table_inputs: Vec<b200vis_table_inputs>, table_cull: Vec<b200vis_table_cull_inputs>,
+    table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -171,7 +180,7 @@ impl Plugin for B200VisibilityPlugin {
             stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, vv_col: vec![0; n],
             vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; max_views * n], visible_classes: vec![0; max_views * n],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
-            planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_entities: Vec::new(),
+            planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_cull: Vec::new(), table_entities: Vec::new(),
             maps_epoch: u64::MAX,
         };
         let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: vis.visible_rows.as_mut_ptr(), visible_capacity: n as u32,
@@ -294,13 +303,23 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     // Transform is repr(Rust): its layout is whatever this build of rustc chose
     let layout = b200vis_transform_layout { stride: size_of::<Transform>() as u32, translation: offset_of!(Transform, translation) as u32,
                                             rotation: offset_of!(Transform, rotation) as u32, scale: offset_of!(Transform, scale) as u32 };
+    // Aabb and Sphere are repr(Rust) too
+    let bounds_layout = b200vis_bounds_layout { aabb_stride: size_of::<Aabb>() as u32, aabb_center: offset_of!(Aabb, center) as u32,
+        aabb_half_extents: offset_of!(Aabb, half_extents) as u32, sphere_stride: size_of::<Sphere>() as u32,
+        sphere_center: offset_of!(Sphere, center) as u32, sphere_radius: offset_of!(Sphere, radius) as u32 };
+    let (aabb_id, sphere_id) = (world.component_id::<Aabb>(), world.component_id::<Sphere>());
+    let (iv_id, vis_vv_id) = (world.component_id::<InheritedVisibility>(), world.component_id::<ViewVisibility>());
+    // per-archetype bits of check_visibility_cpu_culling's query (visibility/mod.rs:758-772), fixed for a whole table
+    let markers = [(world.component_id::<NoFrustumCulling>(), F_NO_FRUSTUM), (world.component_id::<VisibilityRange>(), F_RANGE),
+                   (world.component_id::<NoCpuCulling>(), F_NO_CPU_CULLING)];
+    let light_id = world.component_id::<PointLight>();
     #[cfg(feature = "forked-bevy")]
     let vv_id = world.component_id::<ViewVisibility>();
     #[cfg(not(feature = "forked-bevy"))]
     let vv_id: Option<bevy::ecs::component::ComponentId> = None;
     world.resource_scope(|world, mut vis: Mut<B200Vis>| {
         let vis = &mut *vis;
-        let (mut descs, mut inputs, mut entities) = (Vec::new(), Vec::new(), Vec::new());
+        let (mut descs, mut inputs, mut culls, mut entities) = (Vec::new(), Vec::new(), Vec::new(), Vec::new());
         for table in world.storages().tables.iter() {
             if !table.has_column(gt_id) { continue; }
             // SAFETY: the columns hold GlobalTransform / ViewVisibility.  Only raw pointers are kept; the GPU writes through
@@ -322,12 +341,32 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
                     transform_changed_ticks: table.get_changed_ticks_slice_for(id).unwrap().as_ptr() as *const Tick },
                 None => b200vis_table_inputs { transforms: core::ptr::null(), transform_changed_ticks: core::ptr::null() },
             });
+            // the cull inputs b200vis_read_tables(RD_CULL_INPUTS) reads: Aabb, Sphere and InheritedVisibility with their ticks,
+            // and the bits the archetype fixes.  A table outside visible_aabb_query (NoCpuCulling, or no InheritedVisibility /
+            // ViewVisibility) is NO_CPU_CULLING: the cull never looks at its rows.
+            let has = |c: Option<bevy::ecs::component::ComponentId>| c.is_some_and(|c| table.has_column(c));
+            let (aabb, aabb_t) = column::<Aabb>(table, aabb_id);
+            let (sphere, sphere_t) = column::<Sphere>(table, sphere_id);
+            let in_query = has(iv_id) && has(vis_vv_id) && !has(markers[2].0);
+            let (iv, iv_t) = if in_query { column::<InheritedVisibility>(table, iv_id) } else { (core::ptr::null(), core::ptr::null()) };
+            let mut flags = markers.iter().fold(0u8, |f, (c, bit)| if has(*c) { f | bit } else { f });
+            if !in_query { flags |= F_NO_CPU_CULLING; }
+            // a point light's Sphere is rebuilt from its GlobalTransform every frame (point_light.rs:195-209)
+            if has(light_id) && aabb.is_null() && !sphere.is_null() { flags |= F_SPHERE_FROM_GT; }
+            culls.push(b200vis_table_cull_inputs { aabbs: aabb, aabb_changed_ticks: aabb_t, spheres: sphere, sphere_changed_ticks: sphere_t,
+                                                   inherited_visibility: iv, iv_changed_ticks: iv_t, flags: flags as u32 });
             entities.push(table.entities());
         }
-        if descs != vis.tables || inputs != vis.table_inputs {
+        let registry_changed = descs != vis.tables || inputs != vis.table_inputs;
+        if registry_changed {
             vis.check(unsafe { b200vis_set_tables_ex(vis.ctx, descs.len() as u32, descs.as_ptr(), inputs.as_ptr(), &layout) })?;
             vis.tables = descs;
             vis.table_inputs = inputs;
+        }
+        // b200vis_set_tables_ex drops the cull inputs: attach them again (a table whose entry is unchanged is not read in full)
+        if registry_changed || culls != vis.table_cull {
+            vis.check(unsafe { b200vis_set_table_cull_inputs(vis.ctx, culls.len() as u32, culls.as_ptr(), &bounds_layout) })?;
+            vis.table_cull = culls;
         }
         let renumbered = vis.maps_epoch != vis.columns_epoch;
         let stale: Vec<bool> = entities.iter().enumerate()
@@ -335,6 +374,17 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
         vis.table_entities = entities.iter().map(|e| e.to_vec()).collect();
         send_table_maps(vis, Some(&stale))
     })
+}
+
+/// A table's column of T and its changed ticks as raw pointers, or two NULLs when the table has no such column.
+fn column<T: Component>(table: &bevy::ecs::storage::Table, id: Option<bevy::ecs::component::ComponentId>) -> (*const T, *const Tick) {
+    match id.filter(|c| table.has_column(*c)) {
+        // SAFETY: the column holds T.  Only raw pointers are kept; the GPU reads through them inside the systems that
+        // call b200vis_read_tables, while no other system can write the column.
+        Some(c) => (unsafe { table.get_data_slice_for::<T>(c) }.unwrap().as_ptr() as *const T,
+                    table.get_changed_ticks_slice_for(c).unwrap().as_ptr() as *const Tick),
+        None => (core::ptr::null(), core::ptr::null()),
+    }
 }
 
 /// b200vis_set_table_rows for every table (`only` = None) or the tables marked in `only`: slot s -> the row of the entity
@@ -350,8 +400,8 @@ fn send_table_maps(vis: &mut B200Vis, only: Option<&[bool]>) -> Result<(), BevyE
     Ok(())
 }
 
-/// cull: the parameter list of check_visibility_cpu_culling (visibility/mod.rs:748-774); `Ref` instead of `&` where the shim
-/// needs change detection for its column mirror.
+/// cull: the parameter list of check_visibility_cpu_culling (visibility/mod.rs:748-774), plus the rows whose VisibilityClass
+/// or RenderLayers changed, which the device cannot read from the tables.
 fn b200_check_visibility(
     this_run: SystemChangeTick,
     mut vis: ResMut<B200Vis>,
@@ -360,6 +410,8 @@ fn b200_check_visibility(
                                    Option<Ref<Aabb>>, Option<Ref<Sphere>>, &GlobalTransform, Has<NoFrustumCulling>, Has<VisibilityRange>,
                                    Has<PointLight>), Without<NoCpuCulling>>,
     visible_entity_ranges: Option<Res<VisibleEntityRanges>>,
+    dirty_query: Query<Entity, (Without<NoCpuCulling>, Or<(Changed<VisibilityClass>, Changed<RenderLayers>, With<VisibilityRange>)>)>,
+    mut removed_layers: RemovedComponents<RenderLayers>,
 ) -> Result<(), BevyError> {
     let vis = &mut *vis;
     // ---- views: half spaces copied verbatim from `Frustum` (bit-identical by construction) ----
@@ -376,45 +428,50 @@ fn b200_check_visibility(
         if views.len() == vis.max_views { break; }
     }
     vis.check(unsafe { b200vis_set_views(vis.ctx, views.len() as u32, views.as_ptr()) })?;
-    // ---- row columns: everything after a renumbering, otherwise the rows whose components changed, as contiguous ranges ----
+    // ---- VisibilityClass, RenderLayers and the VisibleEntityRanges masks (which the device cannot read from the tables):
+    // every row after a renumbering, otherwise only the rows whose class or layers changed and the rows with a
+    // VisibilityRange (VisibleEntityRanges is rebuilt by check_visibility_ranges every frame), as contiguous ranges.
+    // upload_bounds also takes the rows' current bounds and flags; the table read below, enqueued after it, then brings
+    // every row's Aabb / Sphere / InheritedVisibility up to date by their change ticks.  No loop over every entity. ----
     let all = vis.bounds_epoch != vis.columns_epoch;
-    let mut dirty: Vec<u32> = Vec::new();
     let n = vis.n;
-    let (mut bounds, mut flags, mut class, mut layer, mut range) = (vec![0f32; n * 6], vec![0u8; n], vec![0u8; n], vec![1u64; n], vec![0u32; n]);
-    for (e, inherited, _, vclass, layers, aabb, sphere, _, no_frustum, has_range, is_light) in visible_aabb_query.iter() {
-        let Some(&r) = vis.row_of.get(&e) else { continue };
-        // (VisibleEntityRanges is rebuilt by check_visibility_ranges every frame: rows with a VisibilityRange are always refreshed)
-        let changed = all || has_range || inherited.is_changed() || vclass.as_ref().is_some_and(|c| c.is_changed()) || layers.as_ref().is_some_and(|c| c.is_changed())
-            || aabb.as_ref().is_some_and(|c| c.is_changed()) || sphere.as_ref().is_some_and(|c| c.is_changed());
-        if !changed { continue; }
-        let r = r as usize;
+    let mut dirty: Vec<u32> = if all { (0..n as u32).collect() } else {
+        dirty_query.iter().chain(removed_layers.read()).filter_map(|e| vis.row_of.get(&e).copied()).collect()
+    };
+    dirty.sort_unstable();
+    dirty.dedup();
+    let k = dirty.len();
+    let (mut bounds, mut flags, mut class, mut layer, mut range) = (vec![0f32; k * 6], vec![F_NO_CPU_CULLING; k], vec![0u8; k], vec![1u64; k], vec![0u32; k]);
+    for (i, &r) in dirty.iter().enumerate() {
+        let e = vis.entity_of[r as usize];
+        // a row outside visible_aabb_query stays NO_CPU_CULLING, as its table's cull inputs say
+        let Ok((_, inherited, _, vclass, layers, aabb, sphere, _, no_frustum, has_range, is_light)) = visible_aabb_query.get(e) else { continue };
         let mut f = if inherited.get() { F_INHERITED } else { 0 } | if no_frustum { F_NO_FRUSTUM } else { 0 } | if has_range { F_RANGE } else { 0 };
-        if let Some(a) = &aabb { f |= F_AABB; bounds[r * 6..r * 6 + 6].copy_from_slice(&[a.center.x, a.center.y, a.center.z, a.half_extents.x, a.half_extents.y, a.half_extents.z]); }
+        if let Some(a) = &aabb { f |= F_AABB; bounds[i * 6..i * 6 + 6].copy_from_slice(&[a.center.x, a.center.y, a.center.z, a.half_extents.x, a.half_extents.y, a.half_extents.z]); }
         else if let Some(s) = &sphere {
-            // a point light's Sphere is rebuilt from its GlobalTransform every frame (point_light.rs:195-209): the device does the
-            // same from the row's own translation (F_SPHERE_FROM_GT) and only needs the radius
             f |= F_SPHERE | if is_light { F_SPHERE_FROM_GT } else { 0 };
-            bounds[r * 6..r * 6 + 4].copy_from_slice(&[s.center.x, s.center.y, s.center.z, s.radius]);
+            bounds[i * 6..i * 6 + 4].copy_from_slice(&[s.center.x, s.center.y, s.center.z, s.radius]);
         }
-        flags[r] = f;
-        class[r] = vclass.as_ref().map_or(0, |c| c.iter().fold(0u8, |m, id| m | vis.class_bit(*id)));
-        layer[r] = layers.as_ref().map_or(1, |l| l.bits()[0]);
-        range[r] = match (&visible_entity_ranges, has_range) {       // entity_is_in_range_of_view (visibility/range.rs:214-222)
+        flags[i] = f;
+        class[i] = vclass.as_ref().map_or(0, |c| c.iter().fold(0u8, |m, id| m | vis.class_bit(*id)));
+        layer[i] = layers.as_ref().map_or(1, |l| l.bits()[0]);
+        range[i] = match (&visible_entity_ranges, has_range) {       // entity_is_in_range_of_view (visibility/range.rs:214-222)
             (Some(vr), true) => vis.view_entities.iter().enumerate().fold(0u32, |m, (v, view)| m | ((vr.entity_is_in_range_of_view(e, *view) as u32) << v)),
             _ => 0,
         };
-        dirty.push(r as u32);
     }
-    dirty.sort_unstable();
     let mut i = 0;
-    while i < dirty.len() {                                     // coalesce into [first, first + count) ranges
-        let first = dirty[i] as usize;
+    while i < k {                                               // coalesce into [first, first + count) ranges
         let mut j = i + 1;
-        while j < dirty.len() && dirty[j] == dirty[j - 1] + 1 { j += 1; }
-        let c = j - i;
-        vis.check(unsafe { b200vis_upload_bounds(vis.ctx, first as u32, c as u32, bounds[first * 6..].as_ptr(), flags[first..].as_ptr(),
-            class[first..].as_ptr(), layer[first..].as_ptr(), if visible_entity_ranges.is_some() { range[first..].as_ptr() } else { core::ptr::null() }) })?;
+        while j < k && dirty[j] == dirty[j - 1] + 1 { j += 1; }
+        vis.check(unsafe { b200vis_upload_bounds(vis.ctx, dirty[i], (j - i) as u32, bounds[i * 6..].as_ptr(), flags[i..].as_ptr(),
+            class[i..].as_ptr(), layer[i..].as_ptr(), if visible_entity_ranges.is_some() { range[i..].as_ptr() } else { core::ptr::null() }) })?;
         i = j;
+    }
+    // Aabb, Sphere and InheritedVisibility straight from the tables, by this system's own change ticks; rows (re)mapped
+    // since the last read (archetype moves, a renumbering) are read in full, their per-archetype flags with them
+    if !vis.tables.is_empty() {
+        vis.check(unsafe { b200vis_read_tables(vis.ctx, RD_CULL_INPUTS, this_run.last_run().get(), this_run.this_run().get()) })?;
     }
     if all {
         #[cfg(feature = "forked-bevy")]
