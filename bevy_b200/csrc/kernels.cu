@@ -452,6 +452,12 @@ __device__ __forceinline__ void bulk_s2g(void *dst, const void *src, uint32_t by
     asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes) : "memory");
 }
 
+__device__ __forceinline__ void cp_async_16(void *dst, const void *src) {
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
+__device__ __forceinline__ void cp_async_8(void *dst, const void *src) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
+}
 template <bool PROP, bool CULL>
 __device__ __forceinline__ void issue_tile_loads(const Rows &R, const Tile &t, TileStage &S, unsigned long long *bar) {
     const uint32_t a = t.base & ~15u;
@@ -468,14 +474,29 @@ __device__ __forceinline__ void issue_tile_loads(const Rows &R, const Tile &t, T
 }
 
 #ifdef B200VIS_TILE_TIMING
-// debug build only (tools/tile_timing.py): per-CTA phase timestamps of the tile kernel, read back through
-// b200vis_debug_tile_timing; not compiled into the product library
+// debug build only (tools/tile_timing.py), not compiled into the product library.  Kernel 1f: per-CTA phase timestamps, read
+// back through b200vis_debug_tile_timing
 __device__ unsigned long long g_tile_timing[8192 * 16];
 #define TT(slot) do { if (lr == 0 && blockIdx.x < 8192u) g_tile_timing[blockIdx.x * 16u + (slot)] = clock64(); } while (0)
 #define TTW(slot) do { if (lr == 224u && blockIdx.x < 8192u) g_tile_timing[blockIdx.x * 16u + (slot)] = clock64(); } while (0)
+// kernel 1b: thread 0's clock64 cycles per phase, summed over every tile of the CTA (slots 1..15; slot 0 counts the tiles) and
+// over its tiles after the first (slots 17..31, slot 16).  The sums live in shared memory while the CTA runs (a global
+// read-modify-write per mark would put an L2 round trip into every phase it measures) and are stored when the CTA ends: the
+// last launch wins.
+__device__ unsigned long long g_tile_phase[8192 * 32];
+#define TP_BEGIN() __shared__ unsigned long long tp_acc_[32]; unsigned long long tp_prev_ = clock64(); uint32_t tp_n_ = 0; \
+    if (lr == 0) for (int k_ = 0; k_ < 32; ++k_) tp_acc_[k_] = 0ull
+#define TP(ph) do { if (lr == 0) { const unsigned long long now_ = clock64(); \
+    if ((ph) == 0) { ++tp_n_; tp_acc_[0] += 1ull; if (tp_n_ > 1u) tp_acc_[16] += 1ull; } \
+    else { tp_acc_[(ph)] += now_ - tp_prev_; if (tp_n_ > 1u) tp_acc_[16 + (ph)] += now_ - tp_prev_; } \
+    tp_prev_ = now_; } } while (0)
+#define TP_END() do { if (lr == 0 && blockIdx.x < 8192u) for (int k_ = 0; k_ < 32; ++k_) g_tile_phase[blockIdx.x * 32u + k_] = tp_acc_[k_]; } while (0)
 #else
 #define TT(slot) do { } while (0)
 #define TTW(slot) do { } while (0)
+#define TP_BEGIN() do { } while (0)
+#define TP(ph) do { } while (0)
+#define TP_END() do { } while (0)
 #endif
 #define B200VIS_TILE_1B k_propagate_cull_tma
 #define B200VIS_TILE_1B_EXT false
@@ -4394,5 +4415,9 @@ void launch_permute_rows(cudaStream_t st, const RowPermute &p) {
 extern "C" __attribute__((visibility("default"))) int b200vis_debug_tile_timing(unsigned long long *out, unsigned n_ctas) {
     if (n_ctas > 8192u) n_ctas = 8192u;
     return (int)cudaMemcpyFromSymbol(out, b200vis::g_tile_timing, (size_t)n_ctas * 16 * sizeof(unsigned long long));
+}
+extern "C" __attribute__((visibility("default"))) int b200vis_debug_tile_phases(unsigned long long *out, unsigned n_ctas) {
+    if (n_ctas > 8192u) n_ctas = 8192u;
+    return (int)cudaMemcpyFromSymbol(out, b200vis::g_tile_phase, (size_t)n_ctas * 32 * sizeof(unsigned long long));
 }
 #endif

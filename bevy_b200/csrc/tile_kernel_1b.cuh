@@ -22,10 +22,9 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+    TP_BEGIN();
     // launched with programmatic stream serialization: everything above overlapped the previous kernel's tail
-    TT(0);
     asm volatile("griddepcontrol.wait;" ::: "memory");
-    TT(1);
     uint32_t t = blockIdx.x;
     if (lr == 0 && t < n_tiles) issue_tile_loads<PROP, CULL>(R, tiles[t], s.st[0], &s.bar[0]);
     uint32_t n_gt_total = 0, n_vv_total = 0;
@@ -34,10 +33,12 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
     // ceil(n/g) tiles running next to finished neighbours with floor(n/g) -- a fifth of the pass at 3.3 tiles per CTA.  The
     // ticket counter is never reset: every launch draws exactly n_tiles tickets, and the host passes the running base.
     for (uint32_t it = 0; t < n_tiles; ++it) {
+        TP(0);
         const uint32_t sidx = it & 1u;
         const Tile tile = tiles[t];
+        TP(1);
         mbar_wait(&s.bar[sidx], (it >> 1) & 1u);
-        if (it == 1) { TT(2); }
+        TP(2);
         TileStage &S = s.st[sidx];
         const uint32_t off = tile.base & 15u;
         const uint32_t li = off + lr;                 // index into the staged window
@@ -45,10 +46,10 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         const uint32_t row = tile.base + lr;
         const uint32_t f = active ? S.flags[li] : 0u;
         const uint32_t st8 = active ? S.state[li] : 0u;
-        // bounds are only needed after the hierarchy walk: plain coalesced loads issued now, consumed in phase 3
-        // (keeping them out of the staged window lets a fourth CTA fit in shared memory)
+        // bounds are only needed after the hierarchy walk (keeping them out of the staged window lets a fourth CTA fit in shared
+        // memory).  Without a walk: plain coalesced loads issued now, consumed in phase 3.
         float4 bA = make_float4(0, 0, 0, 0); float2 bB = make_float2(0, 0);
-        if (CULL && active) { bA = R.bndA[row]; bB = R.bndB[row]; }
+        if (!PROP && CULL && active) { bA = R.bndA[row]; bB = R.bndB[row]; }
 
         bool visited = false, changed = false;
         const bool ext_mark = EXT && (st8 & S_GT_EXT);
@@ -78,8 +79,12 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 __syncthreads();
                 dirty = s.dirty[lr];
             }
-            if (it == 1) { TT(3); }    // dirty phase done
+            TP(3);
             const Aff l = affine_from_trs(S.trsA[li], S.trsB[li], S.trsC[li]);
+            // With a walk, the row's bounds come in by cp.async into its own Transform slots, which nothing reads again in this
+            // tile: the loads run under the walk without holding six registers through it (at the 64-register budget those
+            // registers were spilled in the hot loop), and the cull reads them back from shared memory
+            if (CULL && active) { cp_async_16(&S.trsA[li], R.bndA + row); cp_async_8(&S.trsC[li], R.bndB + row); }
             const uint32_t my_level = (active && !(topo & T_DETACHED)) ? depth : 0xFFFFFFFFu;
             if (active && (topo & T_DETACHED) && has_children) s.pst[lr] = 0;
             if (my_level == 0) {
@@ -99,7 +104,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 if (changed) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
                 if (has_children) s.pst[lr] = (uint8_t)((visited ? 1u : 0u) | ((changed || (visited && ext_mark)) ? 2u : 0u));
             }
-            if (it == 1) { TT(4); }    // local affine + level 0 done
+            TP(4);
             // one level of the walk for this thread's row: the parent's rows are the tile's own (in-place) GlobalTransform entries
             auto walk_row = [&]() {
                 const uint32_t pst = s.pst[plocal];
@@ -144,12 +149,11 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 for (uint32_t lvl = 1; lvl < tile.n_levels; ++lvl) {
                     if (lvl < 32u && ((tile.warp_sync_mask >> lvl) & 1u)) __syncwarp(); else __syncthreads();
                     if (my_level == lvl) walk_row();
-                    if (it == 1 && lvl <= 7) { TT(4 + lvl); }   // thread 0 after the level's barrier and (for level-lvl rows) work
                 }
             }
             if (active && tchanged) R.flags[row] = (uint8_t)(f & ~F_TCHANGED);
         }
-        if (it == 1) { TT(12); }   // walk done
+        TP(5);
         // Prefetch the NEXT tile into the other stage.  That stage was last read by the previous tile's bulk store,
         // issued most of an iteration ago, so the wait below is (almost always) already satisfied: putting the
         // prefetch here instead of at the top of the loop keeps the store drain off every warp's critical path.
@@ -157,10 +161,12 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
             const uint32_t tn = ticket ? gridDim.x + (atomicAdd(ticket, 1u) - ticket_base) : t + gridDim.x;
             if (tn < n_tiles) {
                 asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
+                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stage's generic writes (bounds) -> TMA loads
                 issue_tile_loads<PROP, CULL>(R, tiles[tn], s.st[sidx ^ 1u], &s.bar[sidx ^ 1u]);
             }
             s.next_tile[sidx] = tn;      // read by everybody behind the tile's closing barrier
         }
+        TP(6);
         uint32_t out = st8 & (S_VV | S_HAS_CLASS);     // (drops S_GT_EXT: the pass consumes the marks)
         if (PROP) out |= (changed ? S_GT_CHANGED : 0u) | (visited ? S_VISITED : 0u);
         else out |= st8 & (S_GT_CHANGED | S_VISITED);
@@ -168,6 +174,10 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
 
         bool vv_changed = false;
         if (CULL) {
+            if (PROP) {      // this thread's bounds copies (above) have landed
+                asm volatile("cp.async.wait_all;" ::: "memory");
+                if (active) { bA = S.trsA[li]; bB = S.trsC[li]; }
+            }
             Aff g; g.r0 = S.gt0[li]; g.r1 = S.gt1[li]; g.r2 = S.gt2[li];   // own row: written by this thread or untouched
             const bool in_query = active && !(f & F_NO_CPU_CULL);
             const bool base = in_query && (f & F_INHERITED);
@@ -251,8 +261,10 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 }
             }
             if (my_ballot) {
-                uint32_t *mask = vb.mask + (size_t)lane * vb.words_stride;
-                uint32_t *cc = vb.chunk_count + ((size_t)parity * kMaxViews + lane) * vb.chunks_stride;
+                uint32_t vl = lane;
+                asm volatile("" : "+r"(vl));     // keeps the two row offsets below out of registers held through the tile loop
+                uint32_t *mask = vb.mask + (size_t)vl * vb.words_stride;
+                uint32_t *cc = vb.chunk_count + ((size_t)parity * kMaxViews + vl) * vb.chunks_stride;
                 const uint32_t row0 = row - lane, w0 = row0 >> 5, sh = row0 & 31u;
                 const uint32_t lo = my_ballot << sh, hi = sh ? (my_ballot >> (32u - sh)) : 0u;
                 if (lo) { atomicOr(mask + w0, lo); atomicAdd(cc + (w0 / kChunkWords), __popc(lo)); }
@@ -277,9 +289,9 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         // end of tile: everybody is done with this stage; count changes; write the tile's matrices back
         n_gt_total += (PROP && changed) ? 1u : 0u;      // per-thread tallies, reduced once at the end of the kernel
         n_vv_total += vv_changed ? 1u : 0u;
-        if (it == 1) { TT(13); }   // cull done
+        TP(7);
         const int any_gt = __syncthreads_or(PROP && changed);
-        if (it == 1) { TT(15); }
+        TP(8);
         t = s.next_tile[sidx];
         if (lr == 0) {
             if (PROP && any_gt) {
@@ -290,9 +302,10 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 asm volatile("cp.async.bulk.commit_group;" ::: "memory");
             }
         }
+        TP(9);
     }
+    TP_END();
     if (lr == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    TT(14);
     // block-reduce the per-thread tallies (warp shuffle, then one shared-memory atomic per warp)
     __shared__ uint32_t s_cnt[2];
     if (lr < 2) s_cnt[lr] = 0;
