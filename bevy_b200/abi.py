@@ -90,6 +90,7 @@ class ColumnSinks(C.Structure):
 
 
 WB_GLOBAL_TRANSFORM, WB_VIEW_VISIBILITY = 0x1, 0x2
+WB_SET_VISIBLE = 0x4      # set_visible() over the bytes the tables hold (b200vis_writeback_tables)
 MAX_TABLES = 4096
 UNMAPPED = 0xFFFFFFFF
 
@@ -282,6 +283,10 @@ class ShadowItem(C.Structure):
                 ("layer_mask", C.c_uint64), ("frusta", C.c_float * 144)]
 
 
+class VisibleEntitiesSink(C.Structure):
+    _fields_ = [("entities", C.c_void_p), ("capacity", C.c_uint32), ("offsets", C.c_void_p)]
+
+
 class ResultSink(C.Structure):
     _fields_ = [("stats", C.POINTER(FrameStats)), ("visible_rows", C.c_void_p), ("visible_capacity", C.c_uint32),
                 ("visible_classes", C.c_void_p), ("cluster_offsets", C.c_void_p), ("cluster_indices", C.c_void_p), ("cluster_capacity", C.c_uint32)]
@@ -350,6 +355,7 @@ _SIGNATURES = {
     "b200vis_download_frame_stats": (C.c_int32, [_vp, _P(FrameStats)]),
     "b200vis_download_view_stats": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp]),
     "b200vis_set_view_stats_sink": (C.c_int32, [_vp, _vp]),
+    "b200vis_set_visible_entities_sink": (C.c_int32, [_vp, _P(VisibleEntitiesSink)]),
     "b200vis_download_global_transforms": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, C.c_uint32, _vp]),
     "b200vis_download_view_visibility": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "b200vis_download_visible": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
@@ -943,6 +949,19 @@ class Context:
         s.cluster_capacity = 0 if cluster_indices is None else cluster_indices.shape[1]
         self._sink = (s, visible_rows, cluster_offsets, cluster_indices, visible_classes)
         self._check(self._lib.b200vis_set_result_sink(self._h, C.byref(s)))
+
+    def set_visible_entities_sink(self, entities, offsets):
+        """b200vis_set_visible_entities_sink: pinned (or registrable) host numpy arrays entities [max_views, capacity] uint64
+        (Entity::to_bits(), each view's class lists back to back) and offsets [max_views, 9] uint32 (class k of view v is
+        entities[v, offsets[v, k]:offsets[v, k + 1]]).  (None, None) removes the sink."""
+        if entities is None and offsets is None:
+            self._check(self._lib.b200vis_set_visible_entities_sink(self._h, None))
+            self._ent_sink = None
+            return
+        s = VisibleEntitiesSink(entities.ctypes.data, entities.shape[-1] if entities.ndim else 0,
+                                None if offsets is None else offsets.ctypes.data)
+        self._check(self._lib.b200vis_set_visible_entities_sink(self._h, C.byref(s)))
+        self._ent_sink = (entities, offsets)
 
     def set_column_sinks(self, gt=None, gt_changed_bits=None, view_visibility=None, vv_changed_bits=None):
         """b200vis_set_column_sinks: numpy arrays over (ideally pinned) host memory; gt is [n, 12] or [n, 16] float32.

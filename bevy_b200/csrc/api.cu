@@ -161,6 +161,9 @@ struct b200vis_ctx {
     uint32_t *sink_rows_d = nullptr, *sink_off_d = nullptr, *sink_idx_d = nullptr, *sink_stats_d = nullptr;
     uint8_t *sink_cls_d = nullptr; uint8_t *d_cls = nullptr;   // VisibilityClass masks: sink alias, per-row column
     uint32_t *view_stats_sink = nullptr, *view_stats_d = nullptr;   // b200vis_set_view_stats_sink: [max_views][4], host and device alias
+    // b200vis_set_visible_entities_sink: device aliases, and the per (view, chunk, class) counts of the emit
+    uint64_t *ent_sink_d = nullptr; uint32_t *ent_off_d = nullptr; uint32_t ent_cap = 0;
+    uint32_t *d_ent_counts = nullptr; uint32_t ent_chunks = 0;
 
     b200vis_column_sinks colsink{}; bool have_colsink = false;          // b200vis_set_column_sinks (device aliases below)
     float *col_gt_d = nullptr; uint32_t *col_gt_bits_d = nullptr, *col_vv_bits_d = nullptr; uint8_t *col_vv_d = nullptr;
@@ -248,7 +251,7 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
                    ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
                    ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
-                   ctx->d_tab_cull, ctx->d_tab_fresh};
+                   ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -962,6 +965,7 @@ static int32_t plan_world(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, 
 
 // the slot -> row maps of b200vis_set_tables follow the row numbering
 static int32_t tables_unmap_all(b200vis_ctx *ctx);
+static int32_t make_keys_resident(b200vis_ctx *ctx);
 static int32_t tables_unmap_rows(b200vis_ctx *ctx, uint32_t n_rows, const uint32_t *rows);
 static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_to_new);
 static int32_t flush_table_updates(b200vis_ctx *ctx);
@@ -1032,7 +1036,20 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         ctx->keys_resident = false;
         ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
     }
+    if (ctx->ent_sink_d) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sink reads them
     return tables_unmap_all(ctx);
+}
+
+// The keys in rank order on the device (uploaded from the host copy if they are not there yet).  Once resident, the edits
+// and compactions keep them so.
+static int32_t make_keys_resident(b200vis_ctx *ctx) {
+    if (ctx->keys_resident) return B200VIS_OK;
+    if (!ctx->d_keys) CU(dalloc(&ctx->d_keys, ctx->cfg.max_entities));
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (!ctx->h_keys.empty()) CU(cudaMemcpy(ctx->d_keys, ctx->h_keys.data(), ctx->h_keys.size() * 8, cudaMemcpyHostToDevice));
+    ctx->keys_resident = true;
+    std::vector<uint64_t>().swap(ctx->h_keys);
+    return B200VIS_OK;
 }
 
 static int32_t grow_edit_staging(b200vis_ctx *ctx, size_t bytes) {
@@ -2377,6 +2394,9 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
         if (ctx->diff_on && ctx->diff_sink_rows_d)
             launch_publish_visible_diff(tail, vb, ctx->diff, ctx->diff_sink_rows_d, ctx->diff_sink_cap, ctx->diff_sink_counts_d,
                                         active_consts(ctx).n_views, ctx->cfg.max_views);
+        if (ctx->ent_sink_d)
+            launch_emit_visible_entities(tail, vb, R.rank, ctx->d_keys, fc, ctx->d_stats, ctx->n, ctx->cfg.max_views, ctx->d_ent_counts,
+                                         ctx->ent_chunks, ctx->ent_sink_d, ctx->ent_cap, ctx->ent_off_d);
     }
     if (do_cull && ctx->have_sink && ctx->sink_rows_d) {
         // posting ~1 MB of visible rows over PCIe takes tens of microseconds: in the serial (non-pipelined) case do it on the
@@ -2873,6 +2893,33 @@ extern "C" int32_t b200vis_set_view_stats_sink(b200vis_ctx *ctx, uint32_t *per_v
     if (!per_view) return B200VIS_OK;
     const int32_t rc = map_host(ctx, per_view, (size_t)ctx->cfg.max_views * 16, &ctx->view_stats_d); if (rc) return rc;
     ctx->view_stats_sink = per_view;
+    return B200VIS_OK;
+}
+
+extern "C" int32_t b200vis_set_visible_entities_sink(b200vis_ctx *ctx, const b200vis_visible_entities_sink *sink) {
+    CHECK_CTX_JOIN();
+    if (sink) {
+        if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_visible_entities_sink: world_size > 1");
+        if (!sink->entities || !sink->offsets || !sink->capacity)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_visible_entities_sink: entities, offsets and a capacity go together");
+        if (reinterpret_cast<uintptr_t>(sink->entities) & 7u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_visible_entities_sink: entities is not 8-byte aligned");
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    ctx->ent_sink_d = nullptr; ctx->ent_off_d = nullptr; ctx->ent_cap = 0;
+    if (!sink) return B200VIS_OK;
+    const size_t V = ctx->cfg.max_views;
+    int32_t rc;
+    uint32_t *de = nullptr, *doff = nullptr;
+    if ((rc = map_host(ctx, sink->entities, V * sink->capacity * 8, &de))) return rc;
+    if ((rc = map_host(ctx, sink->offsets, V * 9 * 4, &doff))) return rc;
+    if (!ctx->d_ent_counts) {
+        const uint32_t chunks = visible_entity_chunks(ctx->cfg.max_entities);
+        CU(dalloc(&ctx->d_ent_counts, V * chunks * 8));
+        ctx->ent_chunks = chunks;
+    }
+    if ((rc = make_keys_resident(ctx))) return rc;
+    ctx->ent_sink_d = reinterpret_cast<uint64_t *>(de); ctx->ent_off_d = doff; ctx->ent_cap = sink->capacity;
     return B200VIS_OK;
 }
 
@@ -3443,10 +3490,15 @@ extern "C" int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, ui
     CHECK_CTX();
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "writeback_tables: world_size > 1");
     if (!ctx->tables_set) return fail(ctx, B200VIS_ERR_NOT_READY, "writeback_tables: call b200vis_set_tables first");
+    const bool set_visible = which & B200VIS_WB_SET_VISIBLE;
+    if (set_visible && (which & B200VIS_WB_VIEW_VISIBILITY))
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "writeback_tables: WB_SET_VISIBLE and WB_VIEW_VISIBILITY exclude each other");
     { const int32_t frc = flush_table_updates(ctx); if (frc) return frc; }
     // on the main stream, right behind the tile pass, like the column write-back
     const TableBufs tb{ctx->d_tabs, ctx->d_tab_chunks, ctx->n_tab_chunks, ctx->d_tab_map, ctx->d_tvv_shadow};
-    launch_writeback_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_WB_GLOBAL_TRANSFORM | B200VIS_WB_VIEW_VISIBILITY), gt_tick, vv_tick);
+    if (!set_visible || (which & B200VIS_WB_GLOBAL_TRANSFORM))
+        launch_writeback_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_WB_GLOBAL_TRANSFORM | B200VIS_WB_VIEW_VISIBILITY), gt_tick, vv_tick);
+    if (set_visible) launch_set_visible_tables(ctx->stream, ctx->rows, tb, vv_tick);
     CU(cudaGetLastError());
     return B200VIS_OK;
 }

@@ -3266,6 +3266,144 @@ __global__ void __launch_bounds__(256) k_update_table_map(uint32_t *__restrict__
     if (i < n_reset) vv_shadow[reset[i]] = 0xFF;
 }
 
+// ---- table write-back of SetViewVisibility::set_visible (B200VIS_WB_SET_VISIBLE): the chunk walk of k_writeback_tables.
+// Each lane gathers the rows of its four slots and their device state; a chunk none of whose slots is visible costs no
+// PCIe traffic.  Otherwise the chunk's ViewVisibility bytes cross PCIe as 16-byte loads into the warp's slab (the head
+// rule of stage_ticks), and only the bytes that lack bit 0 are rewritten.  The byte is read, not inferred: other systems
+// of CheckVisibility may have set bit 0 already, and the 2-bit state is the CPU's in this mode.
+__global__ void __launch_bounds__(256)
+k_set_visible_tables(Rows R, TableBufs tb, uint32_t vv_tick) {
+    __shared__ uint4 s_vv[8][9];
+    const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
+        const DevTable T = tb.tables[tb.chunk_table[ch]];
+        if (T.vv == nullptr) continue;                        // the same for the whole warp
+        const uint32_t base = (ch - T.chunk_begin) * 128u, n = min(T.len - base, 128u);
+        uint32_t vis = 0;                                     // bit j: slot base + j * 32 + lane is visible
+#pragma unroll
+        for (uint32_t j = 0; j < 4u; ++j) {
+            const uint32_t i = j * 32u + lane;
+            const uint32_t row = i < n ? tb.map[T.map_off + base + i] : kNoParent;
+            if (row == kNoParent) continue;
+            if (tb.vv_shadow[row] != 0xFF) tb.vv_shadow[row] = 0xFF;   // the slot's byte is the CPU's from here on
+            if (R.state[row] & 1u) vis |= 1u << j;
+        }
+        if (!__any_sync(0xFFFFFFFFu, vis != 0)) continue;
+        const uintptr_t a = reinterpret_cast<uintptr_t>(T.vv + base);
+        const uint32_t head = (uint32_t)(a & 15u);
+        const uint4 *src = reinterpret_cast<const uint4 *>(a - head);
+        if (lane < (head + n + 15u) / 16u) s_vv[warp][lane] = src[lane];   // <= 9 pieces, inside the column's pages
+        __syncwarp();
+        const uint8_t *b = reinterpret_cast<const uint8_t *>(s_vv[warp]) + head;
+#pragma unroll
+        for (uint32_t j = 0; j < 4u; ++j) {
+            const uint32_t i = j * 32u + lane;
+            if (!((vis >> j) & 1u)) continue;
+            const uint32_t v = b[i];
+            if (v & 1u) continue;
+            T.vv[base + i] = (uint8_t)(v | 1u);
+            if (!(v & 2u) && T.vv_ticks != nullptr) T.vv_ticks[base + i] = vv_tick;
+        }
+        __syncwarp();                                         // the slab is the warp's next chunk's
+    }
+}
+
+// ---- VisibleEntities as Entity lists (b200vis_set_visible_entities_sink) -----------------------------------------------
+// Two launches over the frame's expanded lists: per (view, chunk) class counts, then an ordered emit whose positions are
+// the counts of the earlier chunks and of the lower classes.  A chunk is kEntChunk list entries, 512 per warp.
+constexpr uint32_t kEntChunk = 4096;
+
+// the class counts of list entries [w0, min(w0 + 512, count)), one ballot per class bit
+__device__ __forceinline__ void count_classes(const uint8_t *__restrict__ cls, uint32_t w0, uint32_t count, uint32_t lane,
+                                              uint32_t cnt[8]) {
+    const uint32_t end = min(w0 + 512u, count);
+    for (uint32_t i = w0; i < end; i += 32u) {
+        const uint32_t c = i + lane < end ? cls[i + lane] : 0u;
+#pragma unroll
+        for (int k = 0; k < 8; ++k) cnt[k] += __popc(__ballot_sync(0xFFFFFFFFu, (c >> k) & 1u));
+    }
+}
+
+__device__ __forceinline__ bool entity_view_written(const FrameConsts *fc, uint32_t v) {
+    return v < fc->n_views && (fc->views[v].flags & 1u);      // an inactive view keeps its lists (mod.rs:780-782)
+}
+
+// counts[v][chunk][k] = entries of class k in the chunk
+__global__ void __launch_bounds__(256)
+k_count_visible_classes(VisibleBufs vb, const FrameConsts *__restrict__ fc, const DevStats *__restrict__ stats,
+                        uint32_t *__restrict__ counts, uint32_t chunks_stride) {
+    __shared__ uint32_t s[8];
+    const uint32_t v = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    if (!entity_view_written(fc, v)) return;
+    if (threadIdx.x < 8u) s[threadIdx.x] = 0;
+    __syncthreads();
+    uint32_t cnt[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    count_classes(vb.classes + (size_t)v * vb.list_stride, chunk * kEntChunk + warp * 512u, stats->visible_count[v], lane, cnt);
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) if (cnt[k]) atomicAdd(&s[k], cnt[k]);
+    }
+    __syncthreads();
+    if (threadIdx.x < 8u) counts[((size_t)v * chunks_stride + chunk) * 8u + threadIdx.x] = s[threadIdx.x];
+}
+
+// the ordered emit: lanes store 8 bytes each, consecutive lanes of one class to consecutive entries of the mapped sink
+__global__ void __launch_bounds__(256)
+k_emit_visible_entities(VisibleBufs vb, const uint32_t *__restrict__ rank, const uint64_t *__restrict__ keys,
+                        const FrameConsts *__restrict__ fc, const DevStats *__restrict__ stats, const uint32_t *__restrict__ counts,
+                        uint32_t chunks_stride, uint64_t *__restrict__ host_entities, uint32_t capacity, uint32_t *__restrict__ host_offsets) {
+    __shared__ uint32_t s_tot[8], s_part[8], s_w[8][8];
+    const uint32_t v = blockIdx.y, chunk = blockIdx.x, lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
+    if (!entity_view_written(fc, v)) return;
+    const uint32_t count = stats->visible_count[v];
+    {   // warp k: class k's total over the view's chunks, and its part in the chunks before this one
+        const uint32_t *c = counts + (size_t)v * chunks_stride * 8u + warp;
+        uint32_t part = 0, tot = 0;
+        for (uint32_t i = lane; i < gridDim.x; i += 32u) { const uint32_t x = c[(size_t)i * 8u]; tot += x; if (i < chunk) part += x; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) { part += __shfl_xor_sync(0xFFFFFFFFu, part, o); tot += __shfl_xor_sync(0xFFFFFFFFu, tot, o); }
+        if (lane == 0) { s_tot[warp] = tot; s_part[warp] = part; }
+    }
+    const uint8_t *cls = vb.classes + (size_t)v * vb.list_stride;
+    const uint32_t w0 = chunk * kEntChunk + warp * 512u;
+    uint32_t pos[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+    count_classes(cls, w0, count, lane, pos);
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) s_w[warp][k] = pos[k];
+    }
+    __syncthreads();
+    if (chunk == 0 && threadIdx.x <= 8u) {                    // offsets[k] = the totals of the classes below k
+        uint32_t o = 0;
+        for (uint32_t k = 0; k < threadIdx.x; ++k) o += s_tot[k];
+        host_offsets[(size_t)v * 9u + threadIdx.x] = o;
+    }
+    if (w0 >= count) return;
+    uint32_t below = 0;                                       // entries of the lower classes
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        uint32_t p = below + s_part[k];
+        for (uint32_t w = 0; w < warp; ++w) p += s_w[w][k];
+        pos[k] = p;
+        below += s_tot[k];
+    }
+    const uint32_t *lst = vb.lists + (size_t)v * vb.list_stride;
+    uint64_t *out = host_entities + (size_t)v * capacity;
+    const uint32_t lt = (1u << lane) - 1u, end = min(w0 + 512u, count);
+    for (uint32_t i = w0; i < end; i += 32u) {
+        const uint32_t j = i + lane;
+        const uint32_t c = j < end ? cls[j] : 0u;
+        uint64_t key = 0;
+        if (c) { const uint32_t r = lst[j]; key = keys[rank ? rank[r] : r]; }
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            const uint32_t b = __ballot_sync(0xFFFFFFFFu, (c >> k) & 1u);
+            if ((c >> k) & 1u) { const uint32_t p = pos[k] + __popc(b & lt); if (p < capacity) out[p] = key; }
+            pos[k] += __popc(b);
+        }
+    }
+}
+
 // zero this rank's slab for the next frame's assign kernel (only the words in use)
 __global__ void k_cluster_clear(const FrameConsts *__restrict__ fc, ClusterBufs cb) {
     const uint32_t v = blockIdx.y;
@@ -4132,6 +4270,19 @@ void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb,
     if (!tb.n_chunks) return;
     const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
     ++g_launches; k_read_table_cull<<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run);
+}
+void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick) {
+    if (!tb.n_chunks) return;
+    const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
+    ++g_launches; k_set_visible_tables<<<grid, 256, 0, st>>>(R, tb, vv_tick);
+}
+uint32_t visible_entity_chunks(uint32_t max_rows) { return std::max(cdiv(max_rows, kEntChunk), 1u); }
+void launch_emit_visible_entities(cudaStream_t st, const VisibleBufs &vb, const uint32_t *rank, const uint64_t *keys, const FrameConsts *fc,
+                                  const DevStats *stats, uint32_t n_rows, uint32_t max_views, uint32_t *counts, uint32_t chunks_stride,
+                                  uint64_t *host_entities, uint32_t capacity, uint32_t *host_offsets) {
+    const dim3 grid(visible_entity_chunks(n_rows), max_views);
+    ++g_launches; k_count_visible_classes<<<grid, 256, 0, st>>>(vb, fc, stats, counts, chunks_stride);
+    ++g_launches; k_emit_visible_entities<<<grid, 256, 0, st>>>(vb, rank, keys, fc, stats, counts, chunks_stride, host_entities, capacity, host_offsets);
 }
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
                              uint32_t n_reset, uint8_t *fresh) {

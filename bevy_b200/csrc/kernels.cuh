@@ -53,6 +53,13 @@ void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uin
 // b200vis_read_tables with RD_CULL_INPUTS: cull[t] = table t's cull inputs, fresh[entry] = read the slot in full (cleared)
 void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
                             uint32_t last_run, uint32_t this_run);
+// b200vis_writeback_tables with WB_SET_VISIBLE: set_visible() over the bytes the table slots hold, vv_shadow marked unknown
+void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick);
+// b200vis_set_visible_entities_sink: counts = [max_views][chunks_stride][8] scratch, chunks_stride >= visible_entity_chunks(n_rows)
+uint32_t visible_entity_chunks(uint32_t max_rows);
+void launch_emit_visible_entities(cudaStream_t st, const VisibleBufs &vb, const uint32_t *rank, const uint64_t *keys, const FrameConsts *fc,
+                                  const DevStats *stats, uint32_t n_rows, uint32_t max_views, uint32_t *counts, uint32_t chunks_stride,
+                                  uint64_t *host_entities, uint32_t capacity, uint32_t *host_offsets);
 // set_table_rows / set_tables / edit_topology: map[set[i].x] = set[i].y and fresh[set[i].x] = 1, then vv_shadow[reset[i]] = 0xFF
 void launch_update_table_map(cudaStream_t st, uint32_t *map, const uint2 *set, uint32_t n_set, uint8_t *vv_shadow, const uint32_t *reset,
                              uint32_t n_reset, uint8_t *fresh);

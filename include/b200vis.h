@@ -431,6 +431,28 @@ B200VIS_API int32_t b200vis_set_result_sink(b200vis_ctx *ctx, const b200vis_resu
  * synchronisation): per_view[max_views][4] = visible_count, cluster_index_count, cluster_farthest_z (float bits),
  * cluster_index_overflow.  Needs a result sink to be published.  Pinned or registered like the result sink; NULL removes it. */
 B200VIS_API int32_t b200vis_set_view_stats_sink(b200vis_ctx *ctx, uint32_t *per_view);
+/* VisibleEntities as Entity values, one sorted list per VisibilityClass (visibility/mod.rs:344-347, 852-874).  Entity is
+ * repr(C, align(8)) and equivalent to a u64 (crates/bevy_ecs/src/entity/mod.rs:423-432), so each entry is
+ * Entity::to_bits() as given to b200vis_set_topology / b200vis_edit_topology and the shim extends each class's Vec<Entity>
+ * with one slice:
+ *   entities [max_views][capacity]  a view's class lists back to back, class 0 first
+ *   offsets  [max_views][9]         class k of view v is entities[v*capacity + offsets[v*9+k] .. offsets[v*9+k+1])
+ * For every active view below the frame's view count, class k's list is the view's b200vis_download_visible list filtered
+ * to the rows whose b200vis_download_visible_classes mask has bit k, mapped through the entity bits: ascending by
+ * to_bits(), an entity with several classes in each of their lists.  offsets[v*9+8] is the true total even when it
+ * exceeds capacity; positions at or past capacity are not written.  An inactive view, and a view at or past the frame's
+ * view count, has neither its region nor its offsets written (an inactive view keeps its lists, :780-782).
+ * Written by the GPU on the frame's tail right behind the list expansion, wherever the CULL stage runs (pipelined
+ * STAGE_ALL, B200VIS_PIPELINE=0, b200vis_step, more than eight views, after edits and compactions); the frame is readable
+ * after the next b200vis_synchronize.  Pinned or registered like the result sink.  While the sink is set the entity keys
+ * stay resident on the device (8 bytes per max_entities row).  NULL removes the sink.
+ * Errors: INVALID_ARG (capacity 0, entities or offsets NULL, entities not 8-byte aligned), UNSUPPORTED (world_size > 1). */
+typedef struct b200vis_visible_entities_sink {
+    uint64_t *entities;
+    uint32_t  capacity;           /* entries per view */
+    uint32_t *offsets;
+} b200vis_visible_entities_sink;
+B200VIS_API int32_t b200vis_set_visible_entities_sink(b200vis_ctx *ctx, const b200vis_visible_entities_sink *sink);
 
 /* ---- write-back of the frame's column results into the caller's ECS columns -------------------------------------------
  * The reference systems leave their results IN the ECS: GlobalTransform (+ Changed<GlobalTransform>) and ViewVisibility
@@ -509,8 +531,18 @@ B200VIS_API int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uin
                                            const uint32_t *rows);
 /* Enqueues the write-back of `which` (B200VIS_WB_*) on the context's stream, behind the frame's tile pass, like
  * b200vis_writeback_columns_ex; the results are complete after b200vis_synchronize.  gt_tick / vv_tick = the tick stamped
- * into the changed_ticks columns (the writing system's this_run).  Errors: NOT_READY (no b200vis_set_tables yet),
- * UNSUPPORTED (world_size > 1). */
+ * into the changed_ticks columns (the writing system's this_run).
+ *   B200VIS_WB_SET_VISIBLE  SetViewVisibility::set_visible (crates/bevy_camera/src/visibility/mod.rs:290-306) applied to the
+ *                           bytes the caller's reset_view_visibility left, for builds where the device does not own the
+ *                           ViewVisibility state: every slot below len mapped to a row whose device ViewVisibility bit 0
+ *                           is set has its byte b READ; where b & 1 == 0 the slot gets b | 1, and where also b & 2 == 0
+ *                           vv_changed_ticks gets vv_tick.  Nothing else is written.  It neither uses nor updates what the
+ *                           ViewVisibility write-back knows a slot holds: every mapped slot it covers is marked unknown, so
+ *                           a later B200VIS_WB_VIEW_VISIBILITY sends every byte again.  Tables without view_visibility are
+ *                           skipped.
+ * Errors: NOT_READY (no b200vis_set_tables yet), UNSUPPORTED (world_size > 1), INVALID_ARG (B200VIS_WB_SET_VISIBLE with
+ * B200VIS_WB_VIEW_VISIBILITY; nothing is enqueued then). */
+#define B200VIS_WB_SET_VISIBLE 0x4u
 B200VIS_API int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
 
 /* ---- reading Transform and outside-written GlobalTransform straight from the same tables ----------------------------------

@@ -10,17 +10,19 @@
 //!   cluster    <- assign_objects_to_clusters   (crates/bevy_light/src/cluster/assign.rs:137; the only member of
 //!                 SimulationLightSystems::AssignLightsToClusters, crates/bevy_light/src/lib.rs:187-191)
 //! `reset_view_visibility` and `mark_newly_hidden_entities_invisible` are private and share their sets with systems that
-//! must stay, so in an UNFORKED Bevy they keep running on the CPU: the cull system below turns the device's "visible in
-//! >= 1 view" bit into `set_visible()` calls, which is also what keeps the light-visibility systems (they OR into the same
-//! byte) composing correctly (SURVEY.md 8b).  With a three-line patch that makes those two systems removable, the device's
-//! ViewVisibility bytes + change bits can be written straight into the column instead (`forked-bevy` feature below).
+//! must stay, so in an UNFORKED Bevy they keep running on the CPU: the device applies `set_visible()` to the ViewVisibility
+//! byte of every slot whose entity is visible in >= 1 view, straight in the archetype tables (`B200VIS_WB_SET_VISIBLE`),
+//! reading the byte so that the light-visibility systems (they OR into the same byte) compose correctly (SURVEY.md 8b).
+//! With a three-line patch that makes those two systems removable, the device's ViewVisibility bytes + change ticks are
+//! written into the tables instead (`forked-bevy` feature below).
 //!
 //! Data flow (INTEGRATION.md section 2): Transform, other systems' GlobalTransforms, and the cull inputs Aabb, Sphere and
 //! InheritedVisibility read by the device straight from the archetype tables by their change ticks
 //! (`b200vis_set_tables_ex`, `b200vis_set_table_cull_inputs`, `b200vis_read_tables`); VisibilityClass, RenderLayers and
 //! the VisibleEntityRanges masks -> `upload_bounds` on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
-//! `b200vis_set_column_sinks`), read after one `b200vis_synchronize` per system; GlobalTransform (and, forked,
-//! ViewVisibility) with their change ticks straight into the archetype tables (`b200vis_writeback_tables`).
+//! and VisibleEntities as per-class Entity lists through `b200vis_set_visible_entities_sink`), read after one
+//! `b200vis_synchronize` per system; GlobalTransform and ViewVisibility with their change ticks straight into the archetype
+//! tables (`b200vis_writeback_tables`).
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
 use bevy::camera::primitives::{Aabb, Frustum, Sphere};
 use bevy::camera::visibility::*;
@@ -54,8 +56,7 @@ pub struct b200vis_frame_stats { visible_count: [u32; 8], cluster_index_count: [
 pub struct b200vis_cluster_feedback { has_farthest_z: u32, farthest_z: f32, has_index_count: u32, index_count: u32 }
 #[repr(C)] pub struct b200vis_result_sink { stats: *mut b200vis_frame_stats, visible_rows: *mut u32, visible_capacity: u32,
     visible_classes: *mut u8, cluster_offsets: *mut u32, cluster_indices: *mut u32, cluster_capacity: u32 }
-#[repr(C)] pub struct b200vis_column_sinks { global_transforms: *mut f32, gt_stride_floats: u32, gt_changed_bits: *mut u32,
-    view_visibility: *mut u8, vv_changed_bits: *mut u32 }
+#[repr(C)] pub struct b200vis_visible_entities_sink { entities: *mut u64, capacity: u32, offsets: *mut [u32; 9] }
 #[repr(C)] #[derive(Clone, Copy, PartialEq)]
 pub struct b200vis_table { global_transforms: *mut GlobalTransform, gt_changed_ticks: *mut Tick, view_visibility: *mut ViewVisibility,
     vv_changed_ticks: *mut Tick, len: u32, capacity: u32 }
@@ -91,8 +92,7 @@ extern "C" {
     fn b200vis_run(ctx: *mut b200vis_ctx, stages: u32) -> i32;
     fn b200vis_set_result_sink(ctx: *mut b200vis_ctx, sink: *const b200vis_result_sink) -> i32;
     fn b200vis_set_view_stats_sink(ctx: *mut b200vis_ctx, per_view: *mut [u32; 4]) -> i32;
-    fn b200vis_set_column_sinks(ctx: *mut b200vis_ctx, sinks: *const b200vis_column_sinks) -> i32;
-    fn b200vis_writeback_columns_ex(ctx: *mut b200vis_ctx, which: u32) -> i32;
+    fn b200vis_set_visible_entities_sink(ctx: *mut b200vis_ctx, sink: *const b200vis_visible_entities_sink) -> i32;
     fn b200vis_set_table_rows(ctx: *mut b200vis_ctx, table: u32, first_slot: u32, count: u32, rows: *const u32) -> i32;
     fn b200vis_writeback_tables(ctx: *mut b200vis_ctx, which: u32, gt_tick: u32, vv_tick: u32) -> i32;
     fn b200vis_set_tables_ex(ctx: *mut b200vis_ctx, n: u32, tables: *const b200vis_table, inputs: *const b200vis_table_inputs,
@@ -103,7 +103,7 @@ extern "C" {
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
-const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2; const UNMAPPED: u32 = 0xFFFF_FFFF;
+const WB_GLOBAL_TRANSFORM: u32 = 1; const WB_VIEW_VISIBILITY: u32 = 2; const WB_SET_VISIBLE: u32 = 4; const UNMAPPED: u32 = 0xFFFF_FFFF;
 const RD_TRANSFORM: u32 = 1; const RD_GLOBAL_TRANSFORM: u32 = 2; const RD_CULL_INPUTS: u32 = 4;
 const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04; const F_NO_FRUSTUM: u8 = 0x08;
 const F_RANGE: u8 = 0x10; const F_NO_CPU_CULLING: u8 = 0x20; const F_SPHERE_FROM_GT: u8 = 0x40;
@@ -131,11 +131,11 @@ pub struct B200Vis {
     stats: Box<b200vis_frame_stats>,
     view_stats: Vec<[u32; 4]>,    // every view: visible_count, cluster_index_count, cluster_farthest_z bits, overflow
     max_views: usize,
-    vv_col: Vec<u8>, vv_bits: Vec<u32>,
-    visible_rows: Vec<u32>, visible_classes: Vec<u8>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
+    // VisibleEntities as Entity::to_bits(), every view's class lists back to back, and their offsets
+    visible_entities: Vec<u64>, entity_offsets: Vec<[u32; 9]>, cluster_offsets: Vec<u32>, cluster_indices: Vec<u32>, cluster_cap: usize,
     planes_scratch: Vec<f32>,
     // the archetype tables registered with b200vis_set_tables_ex (one entry per table holding GlobalTransform, with its
-    // Transform column and in the forked build its ViewVisibility column), their cull inputs, the entities each slot map
+    // Transform and ViewVisibility columns), their cull inputs, the entities each slot map
     // was built from, and the rows epoch of the maps
     tables: Vec<b200vis_table>, table_inputs: Vec<b200vis_table_inputs>, table_cull: Vec<b200vis_table_cull_inputs>,
     table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
@@ -161,7 +161,10 @@ impl B200Vis {
 }
 
 /// `max_cameras`: the most cameras (views) the app renders at once, 1..=32; views past the eighth cost one extra cull pass
-/// per eight views (DESIGN.md section 4), and the result buffers are sized by it.
+/// per eight views (DESIGN.md section 4), and the result buffers are sized by it.  The VisibleEntities sink holds
+/// `max_entities` entries per view: a view whose visible entities are in more than `max_entities` class lists in all (an
+/// entity counts once per VisibilityClass it carries) makes the cull system return an error, so an app whose entities
+/// carry several classes sets `max_entities` to cover that total.
 pub struct B200VisibilityPlugin { pub max_entities: u32, pub max_lights: u32, pub max_cameras: u32 }
 
 impl Plugin for B200VisibilityPlugin {
@@ -177,21 +180,21 @@ impl Plugin for B200VisibilityPlugin {
         let mut vis = B200Vis {
             ctx, max_entities: n, n: 0, row_of: Default::default(), entity_of: Vec::new(), columns_epoch: 0, bounds_epoch: u64::MAX,
             lights_epoch: u64::MAX, classes: Vec::new(), view_entities: Vec::new(), light_entities: Vec::new(),
-            stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, vv_col: vec![0; n],
-            vv_bits: vec![0; n.div_ceil(32)], visible_rows: vec![0; max_views * n], visible_classes: vec![0; max_views * n],
+            stats: Box::default(), view_stats: vec![[0; 4]; max_views], max_views, visible_entities: vec![0; max_views * n],
+            entity_offsets: vec![[0; 9]; max_views],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
             planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_cull: Vec::new(), table_entities: Vec::new(),
             maps_epoch: u64::MAX,
         };
-        let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: vis.visible_rows.as_mut_ptr(), visible_capacity: n as u32,
-            visible_classes: vis.visible_classes.as_mut_ptr(), cluster_offsets: vis.cluster_offsets.as_mut_ptr(),
+        // the sorted row lists stay on the device: VisibleEntities arrives as Entity values through the entities sink, and
+        // GlobalTransform and ViewVisibility go straight into the archetype tables (b200vis_set_tables)
+        let rs = b200vis_result_sink { stats: &mut *vis.stats, visible_rows: core::ptr::null_mut(), visible_capacity: 0,
+            visible_classes: core::ptr::null_mut(), cluster_offsets: vis.cluster_offsets.as_mut_ptr(),
             cluster_indices: vis.cluster_indices.as_mut_ptr(), cluster_capacity: cluster_cap as u32 };
-        // GlobalTransform goes straight into the archetype tables (b200vis_set_tables); the column sink carries the
-        // ViewVisibility bytes the unforked cull turns into set_visible() calls
-        let cs = b200vis_column_sinks { global_transforms: core::ptr::null_mut(), gt_stride_floats: 16,
-            gt_changed_bits: core::ptr::null_mut(), view_visibility: vis.vv_col.as_mut_ptr(), vv_changed_bits: vis.vv_bits.as_mut_ptr() };
+        let es = b200vis_visible_entities_sink { entities: vis.visible_entities.as_mut_ptr(), capacity: n as u32,
+                                                 offsets: vis.entity_offsets.as_mut_ptr() };
         unsafe {
-            assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_column_sinks(ctx, &cs), 0);
+            assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_visible_entities_sink(ctx, &es), 0);
             assert_eq!(b200vis_set_view_stats_sink(ctx, vis.view_stats.as_mut_ptr()), 0);   // per-view stats of every view
         }
         app.insert_resource(vis);
@@ -291,7 +294,7 @@ fn b200_propagate(
 }
 
 /// The table registry (INTEGRATION.md section 2): one entry per archetype table that holds GlobalTransform -- that column and
-/// its changed ticks, and in the forked build the table's ViewVisibility column and ticks -- read from
+/// its changed ticks, and the table's ViewVisibility column and ticks -- read from
 /// `World::storages().tables` with `Table::entity_count` / `Table::capacity` (storage/table/mod.rs).  Exclusive and chained
 /// right before each write-back system, so no table moves between the registration and the write-back that uses it.  The
 /// registry is replaced when a table's pointers, len or capacity changed; a table's slot -> row map is sent again when its
@@ -313,10 +316,6 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     let markers = [(world.component_id::<NoFrustumCulling>(), F_NO_FRUSTUM), (world.component_id::<VisibilityRange>(), F_RANGE),
                    (world.component_id::<NoCpuCulling>(), F_NO_CPU_CULLING)];
     let light_id = world.component_id::<PointLight>();
-    #[cfg(feature = "forked-bevy")]
-    let vv_id = world.component_id::<ViewVisibility>();
-    #[cfg(not(feature = "forked-bevy"))]
-    let vv_id: Option<bevy::ecs::component::ComponentId> = None;
     world.resource_scope(|world, mut vis: Mut<B200Vis>| {
         let vis = &mut *vis;
         let (mut descs, mut inputs, mut culls, mut entities) = (Vec::new(), Vec::new(), Vec::new(), Vec::new());
@@ -326,7 +325,7 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             // them inside the write-back systems, which hold the only access to those columns while they run.
             let gt = unsafe { table.get_data_slice_for::<GlobalTransform>(gt_id) }.unwrap();
             let gt_ticks = table.get_changed_ticks_slice_for(gt_id).unwrap();
-            let (vv, vv_ticks) = match vv_id.filter(|id| table.has_column(*id)) {
+            let (vv, vv_ticks) = match vis_vv_id.filter(|id| table.has_column(*id)) {
                 Some(id) => (unsafe { table.get_data_slice_for::<ViewVisibility>(id) }.unwrap().as_ptr() as *mut ViewVisibility,
                              table.get_changed_ticks_slice_for(id).unwrap().as_ptr() as *mut Tick),
                 None => (core::ptr::null_mut(), core::ptr::null_mut()),
@@ -406,7 +405,7 @@ fn b200_check_visibility(
     this_run: SystemChangeTick,
     mut vis: ResMut<B200Vis>,
     mut view_query: Query<(Entity, &mut VisibleEntities, &Frustum, Option<&RenderLayers>, &Camera, Has<NoCpuCulling>)>,
-    mut visible_aabb_query: Query<(Entity, Ref<InheritedVisibility>, &mut ViewVisibility, Option<Ref<VisibilityClass>>, Option<Ref<RenderLayers>>,
+    visible_aabb_query: Query<(Entity, Ref<InheritedVisibility>, &mut ViewVisibility, Option<Ref<VisibilityClass>>, Option<Ref<RenderLayers>>,
                                    Option<Ref<Aabb>>, Option<Ref<Sphere>>, &GlobalTransform, Has<NoFrustumCulling>, Has<VisibilityRange>,
                                    Has<PointLight>), Without<NoCpuCulling>>,
     visible_entity_ranges: Option<Res<VisibleEntityRanges>>,
@@ -479,37 +478,40 @@ fn b200_check_visibility(
           vis.check(unsafe { b200vis_upload_view_visibility(vis.ctx, 0, n as u32, vv.as_ptr()) })?; }
         vis.bounds_epoch = vis.columns_epoch;
     }
-    // forked: the tables b200_sync_tables registered carry the ViewVisibility columns too; they receive the bytes and, where
-    // Changed<ViewVisibility> fires, this run's tick
+    // ViewVisibility straight into the tables b200_sync_tables registered.  Unforked, the CPU's reset_view_visibility and
+    // mark_newly_hidden_entities_invisible own the 2-bit state: the device applies set_visible() to the byte each visible
+    // slot holds, with this run's tick where it goes from hidden to visible.  Forked, the device owns the state and writes
+    // the bytes, with the tick where Changed<ViewVisibility> fires.
     unsafe {
         vis.check(b200vis_run(vis.ctx, STAGE_CULL))?;
         #[cfg(not(feature = "forked-bevy"))]
-        vis.check(b200vis_writeback_columns_ex(vis.ctx, WB_VIEW_VISIBILITY))?;
+        vis.check(b200vis_writeback_tables(vis.ctx, WB_SET_VISIBLE, 0, this_run.this_run().get()))?;
         #[cfg(feature = "forked-bevy")]
         vis.check(b200vis_writeback_tables(vis.ctx, WB_VIEW_VISIBILITY, 0, this_run.this_run().get()))?;
-        vis.check(b200vis_synchronize(vis.ctx))?;       // stats, sorted lists + class masks, ViewVisibility bytes are in host memory now
+        vis.check(b200vis_synchronize(vis.ctx))?;       // stats, Entity lists and the tables' ViewVisibility are written now
     }
-    // ---- VisibleEntities: one sorted Vec per class; an entity is pushed once per class it carries (mod.rs:846-857).  The device
-    // list is already in Entity::to_bits() order, so every class list comes out sorted and the reference's sort_unstable
-    // (mod.rs:870-874) has nothing left to do ----
+    // ---- VisibleEntities: one sorted Vec per class (mod.rs:846-874), each filled with one slice of the device's Entity list:
+    // the device wrote every class list already split, in Entity::to_bits() order, so the reference's sort_unstable has
+    // nothing left to do.  No loop over entities. ----
+    // Entity is repr(C, align(8)) and "equivalent to a u64" (bevy_ecs/src/entity/mod.rs:423-432): its memory is to_bits()
+    const _: () = assert!(size_of::<Entity>() == size_of::<u64>() && core::mem::align_of::<Entity>() == core::mem::align_of::<u64>());
     for (v, view_entity) in vis.view_entities.iter().enumerate() {
         let Ok((_, mut visible_entities, _, _, camera, _)) = view_query.get_mut(*view_entity) else { continue };
         if !camera.is_active { continue; }                       // an inactive view keeps its lists (mod.rs:780-782)
         for list in visible_entities.entities.values_mut() { list.clear(); }
-        let count = vis.view_stats[v][0] as usize;
-        let (rows, masks) = (&vis.visible_rows[v * vis.max_entities..][..count], &vis.visible_classes[v * vis.max_entities..][..count]);
-        for (row, mask) in rows.iter().zip(masks) {
-            let entity = vis.entity_of[*row as usize];
-            let mut m = *mask;
-            while m != 0 { let k = m.trailing_zeros() as usize; m &= m - 1; visible_entities.get_mut(vis.classes[k]).push(entity); }
+        let off = vis.entity_offsets[v];
+        if off[8] as usize > vis.max_entities {
+            return Err(format!("view {v}: {} VisibleEntities entries exceed the sink's {} per view (entities in several \
+                                VisibilityClasses): raise max_entities", off[8], vis.max_entities).into());
+        }
+        let all = &vis.visible_entities[v * vis.max_entities..][..off[8] as usize];
+        // SAFETY: every entry is the to_bits() of a live Entity, given to b200vis_set_topology; layout asserted above
+        let all = unsafe { core::slice::from_raw_parts(all.as_ptr() as *const Entity, all.len()) };
+        for (k, id) in vis.classes.iter().enumerate() {
+            let list = &all[off[k] as usize..off[k + 1] as usize];
+            if !list.is_empty() { visible_entities.get_mut(*id).extend_from_slice(list); }
         }
     }
-    // ---- ViewVisibility ----
-    #[cfg(not(feature = "forked-bevy"))]
-    for (r, byte) in vis.vv_col[..n].iter().enumerate() {        // the CPU bracket systems own the 2-bit state machine and the ticks
-        if byte & 1 != 0 { if let Ok(mut q) = visible_aabb_query.get_mut(vis.entity_of[r]) { q.2.set_visible(); } }
-    }
-    // forked: nothing left to do -- the device owns the state machine and wrote bytes and ticks into the tables
     Ok(())
 }
 
