@@ -287,6 +287,11 @@ class VisibleEntitiesSink(C.Structure):
     _fields_ = [("entities", C.c_void_p), ("capacity", C.c_uint32), ("offsets", C.c_void_p)]
 
 
+class ShadowEntitiesSink(C.Structure):
+    _fields_ = [("entities", C.c_void_p), ("capacity", C.c_uint32), ("max_items", C.c_uint32), ("offsets", C.c_void_p),
+                ("active", C.c_void_p)]
+
+
 class ResultSink(C.Structure):
     _fields_ = [("stats", C.POINTER(FrameStats)), ("visible_rows", C.c_void_p), ("visible_capacity", C.c_uint32),
                 ("visible_classes", C.c_void_p), ("cluster_offsets", C.c_void_p), ("cluster_indices", C.c_void_p), ("cluster_capacity", C.c_uint32)]
@@ -328,6 +333,7 @@ _SIGNATURES = {
     "b200vis_set_tables_ex": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, _P(TransformLayout)]),
     "b200vis_read_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
     "b200vis_set_table_cull_inputs": (C.c_int32, [_vp, C.c_uint32, _vp, _P(BoundsLayout)]),
+    "b200vis_set_table_shadow_casters": (C.c_int32, [_vp, C.c_uint32, _vp]),
     "b200vis_host_plan_summary": (C.c_int32, [C.c_uint32, _vp, _P(C.c_uint32)]),
     "b200vis_host_tile_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp]),
     "b200vis_host_warp_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp, _vp, _vp]),
@@ -365,6 +371,7 @@ _SIGNATURES = {
     "b200vis_set_shadow_lights": (C.c_int32, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_int32, C.c_uint32]),
     "b200vis_run_shadow_culling": (C.c_int32, [_vp]),
     "b200vis_download_shadow_visible": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "b200vis_set_shadow_entities_sink": (C.c_int32, [_vp, _P(ShadowEntitiesSink)]),
     "b200vis_host_point_light_frusta": (None, [_vp, C.c_float, C.c_float, _vp]),
     "b200vis_upload_visibility_ranges": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "b200vis_set_visibility_range_views": (C.c_int32, [_vp, C.c_uint32, _vp]),
@@ -856,6 +863,25 @@ class Context:
         self._check(self._lib.b200vis_download_shadow_visible(self._h, shadow_light, face, _ptr(rows), len(rows), C.byref(cnt)))
         return rows[:cnt.value]
 
+    def set_shadow_entities_sink(self, entities, offsets, active, capacity=None, max_items=None):
+        """b200vis_set_shadow_entities_sink: pinned (or registrable) host numpy arrays entities [capacity] uint64 (every list
+        of the run back to back, Entity::to_bits()), offsets [max_items * 6 + 1] uint32 (list item * 6 + face is
+        entities[offsets[l]:offsets[l + 1]]) and active [max_items] uint8.  capacity / max_items override the counts passed
+        (argument tests).  All None removes the sink."""
+        if entities is None and offsets is None and active is None:
+            self._check(self._lib.b200vis_set_shadow_entities_sink(self._h, None))
+            self._shadow_sink = None
+            return
+        ptr = lambda a: None if a is None else a.ctypes.data
+        cap = (0 if entities is None else entities.size) if capacity is None else capacity
+        mi = (0 if active is None else active.size) if max_items is None else max_items
+        if entities is not None and cap > entities.size or offsets is not None and mi * 6 + 1 > offsets.size or \
+                active is not None and mi > active.size:
+            raise ValueError("set_shadow_entities_sink: the arrays are smaller than capacity / max_items say")
+        s = ShadowEntitiesSink(ptr(entities), cap, mi, ptr(offsets), ptr(active))
+        self._check(self._lib.b200vis_set_shadow_entities_sink(self._h, C.byref(s)))
+        self._shadow_sink = (entities, offsets, active)
+
     # ---- SURVEY 8(f) N4 ----
     def upload_visibility_ranges(self, first, start_end, use_aabb):
         se = np.ascontiguousarray(start_end, np.float32); ua = np.ascontiguousarray(use_aabb, np.uint8)
@@ -1024,6 +1050,18 @@ class Context:
         if n > len(descs):                                   # the library reads inputs[n_tables]
             raise ValueError(f"set_table_cull_inputs: n_tables {n} > {len(descs)} entries")
         self._check(self._lib.b200vis_set_table_cull_inputs(self._h, n, arr, None if lay is None else C.byref(lay)))
+
+    def set_table_shadow_casters(self, is_caster, n_tables=None):
+        """b200vis_set_table_shadow_casters: one byte per registered table (1 = its archetype is in the light systems'
+        visible_entity_query); None detaches.  n_tables overrides the count passed (argument tests)."""
+        if is_caster is None:
+            self._check(self._lib.b200vis_set_table_shadow_casters(self._h, 0 if n_tables is None else n_tables, None))
+            return
+        c = np.ascontiguousarray(is_caster, np.uint8)
+        n = len(c) if n_tables is None else n_tables
+        if n > len(c):                                       # the library reads is_caster[n_tables]
+            raise ValueError(f"set_table_shadow_casters: n_tables {n} > {len(c)} entries")
+        self._check(self._lib.b200vis_set_table_shadow_casters(self._h, n, _ptr(c)))
 
     def p2p_export(self):
         """CUDA IPC handle (64 bytes) of this rank's gathered buffer."""

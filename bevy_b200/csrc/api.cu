@@ -164,6 +164,8 @@ struct b200vis_ctx {
     // b200vis_set_visible_entities_sink: device aliases, and the per (view, chunk, class) counts of the emit
     uint64_t *ent_sink_d = nullptr; uint32_t *ent_off_d = nullptr; uint32_t ent_cap = 0;
     uint32_t *d_ent_counts = nullptr; uint32_t ent_chunks = 0;
+    // b200vis_set_shadow_entities_sink: device aliases (entities == nullptr: none), its max_items, and the device offsets
+    ShadowSink shsink{}; uint32_t shsink_max_items = 0; uint32_t *d_shadow_off = nullptr; size_t shadow_off_cap = 0;
 
     b200vis_column_sinks colsink{}; bool have_colsink = false;          // b200vis_set_column_sinks (device aliases below)
     float *col_gt_d = nullptr; uint32_t *col_gt_bits_d = nullptr, *col_vv_bits_d = nullptr; uint8_t *col_vv_d = nullptr;
@@ -189,6 +191,8 @@ struct b200vis_ctx {
     // whether they are attached, their device form, and per map entry the "read in full" mark k_read_table_cull clears
     std::vector<b200vis_table_cull_inputs> h_tab_cull; b200vis_bounds_layout cull_layout{}; bool cull_attached = false;
     DevTableCull *d_tab_cull = nullptr; uint8_t *d_tab_fresh = nullptr;
+    // b200vis_set_table_shadow_casters: the attached per-table caster bytes, and their device copy
+    std::vector<uint8_t> h_tab_caster; bool caster_attached = false; uint8_t *d_tab_caster = nullptr;
     bool cull_fresh_pending = false;    // slots (re)mapped or tables (re)attached since the last RD_CULL_INPUTS read
     double step_t[6] = {0, 0, 0, 0, 0, 0}; uint64_t step_n = 0;   // B200VIS_STEP_TRACE: host time per phase of b200vis_step
     void *nccl_comm = nullptr;          // b200vis_comm_init
@@ -251,7 +255,7 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
                    ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
                    ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
-                   ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts};
+                   ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -1036,7 +1040,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         ctx->keys_resident = false;
         ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
     }
-    if (ctx->ent_sink_d) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sink reads them
+    if (ctx->ent_sink_d || ctx->shsink.entities) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sinks read them
     return tables_unmap_all(ctx);
 }
 
@@ -2600,6 +2604,8 @@ extern "C" int32_t b200vis_set_shadow_lights(b200vis_ctx *ctx, uint32_t n_lights
     CHECK_CTX_JOIN();
     if (n_lights && (!light_ordinals || !frusta)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_lights: null");
     if (!ctx->d_caster) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_lights: upload the shadow-caster column first");
+    if (ctx->shsink.entities && n_lights > ctx->shsink_max_items)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_lights: %u items > the shadow entity sink's max_items %u", n_lights, ctx->shsink_max_items);
     for (uint32_t i = 0; i < n_lights; ++i)
         if (light_ordinals[i] >= ctx->lights.n) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_lights: light ordinal %u >= %u lights", light_ordinals[i], ctx->lights.n);
     ctx->h_shadow.resize(n_lights);
@@ -2617,6 +2623,8 @@ extern "C" int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, 
     CHECK_CTX_JOIN();
     if (n_items && !items) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items: null");
     if (!ctx->d_caster) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_items: upload the shadow-caster column first");
+    if (ctx->shsink.entities && n_items > ctx->shsink_max_items)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_items: %u items > the shadow entity sink's max_items %u", n_items, ctx->shsink_max_items);
     ctx->h_shadow.resize(n_items);
     for (uint32_t i = 0; i < n_items; ++i) {
         const b200vis_shadow_item &it = items[i];
@@ -2635,8 +2643,11 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     CHECK_CTX_JOIN();   // reads what the frame's CULL stage (incl. its tail on the side stream) left behind
     if (!ctx->d_caster || !ctx->diff.prev) return fail(ctx, B200VIS_ERR_NOT_READY, "run_shadow_culling: call b200vis_set_shadow_lights first");
     if (ctx->frame == 0) return fail(ctx, B200VIS_ERR_NOT_READY, "run_shadow_culling: run the CULL stage first");
-    if (!ctx->shadow.n_lights) return B200VIS_OK;
     cudaStream_t st = ctx->stream;
+    if (!ctx->shadow.n_lights) {                // the sink's one offset: a memset, no launch
+        if (ctx->shsink.entities) CU(cudaMemsetAsync(ctx->shsink.offsets, 0, 4, st));
+        return B200VIS_OK;
+    }
     Rows R = ctx->rows;
     R.layers = ctx->have_layers ? ctx->d_layers : nullptr;
     R.range = ctx->have_range ? ctx->d_range : nullptr;
@@ -2645,8 +2656,10 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     ShadowBufs sb = ctx->shadow;
     sb.has_ranges = ctx->have_range ? 1u : 0u;
     CU(cudaMemsetAsync(sb.chunk_count, 0, (size_t)sb.n_lights * 6 * ctx->vis.chunks_stride * 4, st));
+    ShadowSink sink = ctx->shsink;
+    sink.keys = ctx->d_keys;                    // a compaction swaps the key buffers
     launch_shadow_cull(st, R, sb, ctx->diff.prev, active_consts(ctx).n_views, ctx->vis.n_words, ctx->vis.n_chunks,
-                       ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u);
+                       ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u, sink);
     CU(cudaGetLastError());
     return B200VIS_OK;
 }
@@ -2666,6 +2679,42 @@ extern "C" int32_t b200vis_download_shadow_visible(b200vis_ctx *ctx, uint32_t sh
         if (c) CU(cudaMemcpyAsync(rows, ctx->shadow.lists + (size_t)list * ctx->shadow.list_cap, (size_t)c * 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
     }
+    return B200VIS_OK;
+}
+
+static int32_t map_host(b200vis_ctx *ctx, void *p, size_t bytes, uint32_t **dev);
+extern "C" int32_t b200vis_set_shadow_entities_sink(b200vis_ctx *ctx, const b200vis_shadow_entities_sink *sink) {
+    CHECK_CTX_JOIN();
+    if (sink) {
+        if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_shadow_entities_sink: world_size > 1");
+        if (!sink->entities || !sink->offsets || !sink->active || !sink->capacity)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_entities_sink: entities, offsets, active and a capacity go together");
+        if (reinterpret_cast<uintptr_t>(sink->entities) & 7u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_entities_sink: entities is not 8-byte aligned");
+        if (sink->max_items < ctx->shadow.n_lights)
+            return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_entities_sink: max_items %u < %u installed shadow items", sink->max_items,
+                        ctx->shadow.n_lights);
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    ctx->shsink = ShadowSink{}; ctx->shsink_max_items = 0;
+    if (!sink) return B200VIS_OK;
+    const size_t n_off = (size_t)sink->max_items * 6 + 1;
+    int32_t rc;
+    uint32_t *de = nullptr, *doff = nullptr, *dact = nullptr;
+    if ((rc = map_host(ctx, sink->entities, (size_t)sink->capacity * 8, &de))) return rc;
+    if ((rc = map_host(ctx, sink->offsets, n_off * 4, &doff))) return rc;
+    if ((rc = map_host(ctx, sink->active, std::max<size_t>(sink->max_items, 1), &dact))) return rc;
+    if (n_off > ctx->shadow_off_cap) {
+        if (ctx->d_shadow_off) cudaFree(ctx->d_shadow_off);
+        ctx->d_shadow_off = nullptr; ctx->shadow_off_cap = 0;
+        CU(dalloc(&ctx->d_shadow_off, n_off));
+        ctx->shadow_off_cap = n_off;
+    }
+    if ((rc = make_keys_resident(ctx))) return rc;
+    ShadowSink &s = ctx->shsink;
+    s.entities = reinterpret_cast<uint64_t *>(de); s.capacity = sink->capacity; s.offsets = doff;
+    s.active = reinterpret_cast<uint8_t *>(dact); s.dev_offsets = ctx->d_shadow_off;
+    ctx->shsink_max_items = sink->max_items;
     return B200VIS_OK;
 }
 
@@ -3150,6 +3199,7 @@ static int32_t register_columns(b200vis_ctx *ctx, ColumnRanges &cr, const char *
             cudaGetLastError();
             ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->h_tab_in.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
             ctx->h_tab_cull.clear(); ctx->cull_attached = false;
+            ctx->h_tab_caster.clear(); ctx->caster_attached = false;
             std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
             ctx->n_tab_chunks = 0;
             return fail(ctx, B200VIS_ERR_CUDA, "%s: cudaHostRegister of %zu bytes at %p failed: %s", who, (size_t)(r.second - r.first),
@@ -3300,6 +3350,7 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
     ctx->n_tab_chunks = (uint32_t)chunks;
     ctx->tables_set = true;
     ctx->cull_attached = false;              // the cull inputs are attached again by b200vis_set_table_cull_inputs
+    ctx->caster_attached = false; ctx->h_tab_caster.clear();   // ... and the table casters by b200vis_set_table_shadow_casters
     queue_table_updates(ctx, {}, reset);
     return B200VIS_OK;
 }
@@ -3486,6 +3537,39 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
     return B200VIS_OK;
 }
 
+extern "C" int32_t b200vis_set_table_shadow_casters(b200vis_ctx *ctx, uint32_t n_tables, const uint8_t *is_caster) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_table_shadow_casters: world_size > 1");
+    if (!n_tables && !is_caster) { ctx->caster_attached = false; ctx->h_tab_caster.clear(); return B200VIS_OK; }
+    if (!ctx->tables_set || ctx->h_tabs.empty()) return fail(ctx, B200VIS_ERR_NOT_READY, "set_table_shadow_casters: no tables are registered");
+    if (n_tables != ctx->h_tabs.size())
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_shadow_casters: %u entries for %zu registered tables", n_tables, ctx->h_tabs.size());
+    if (!is_caster) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_shadow_casters: null is_caster");
+    std::vector<uint8_t> bytes(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t) bytes[t] = is_caster[t] ? 1u : 0u;
+    if (!ctx->d_caster) CU(dalloc(&ctx->d_caster, ctx->cfg.max_entities));
+    // the shadow stage reads each view's VisibleEntities as the visible-diff sets (as for b200vis_upload_shadow_casters)
+    if (!ctx->diff_on) { const int32_t rc = b200vis_enable_visible_diff(ctx, 1); if (rc) return rc; }
+    if (!ctx->d_tab_caster) CU(dalloc(&ctx->d_tab_caster, B200VIS_MAX_TABLES));
+    cudaStream_t st = ctx->stream;
+    CU(cudaStreamSynchronize(st));              // no read in flight reads the old bytes
+    // a table whose byte changed (every table, on an attach after none) is read in full: the same mark as a changed cull
+    // input, cleared by the read
+    bool pending = false;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const bool same = ctx->caster_attached && t < ctx->h_tab_caster.size() && ctx->h_tab_caster[t] == bytes[t];
+        if (same || !ctx->h_tabs[t].capacity) continue;
+        CU(cudaMemsetAsync(ctx->d_tab_fresh + ctx->tab_off[t], 1, ctx->h_tabs[t].capacity, st));
+        pending = true;
+    }
+    CU(cudaMemcpyAsync(ctx->d_tab_caster, bytes.data(), n_tables, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    ctx->cull_fresh_pending |= pending;
+    ctx->h_tab_caster = std::move(bytes);
+    ctx->caster_attached = true;
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick) {
     CHECK_CTX();
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "writeback_tables: world_size > 1");
@@ -3512,7 +3596,8 @@ extern "C" int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_
     launch_read_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_RD_TRANSFORM | B200VIS_RD_GLOBAL_TRANSFORM), last_run, this_run);
     CU(cudaGetLastError());
     if ((which & B200VIS_RD_CULL_INPUTS) && ctx->cull_attached) {
-        launch_read_table_cull(ctx->stream, ctx->rows, tb, ctx->d_tab_cull, ctx->d_tab_fresh, last_run, this_run);
+        launch_read_table_cull(ctx->stream, ctx->rows, tb, ctx->d_tab_cull, ctx->d_tab_fresh, last_run, this_run,
+                               ctx->caster_attached ? ctx->d_tab_caster : nullptr, ctx->d_caster);
         CU(cudaGetLastError());
         ctx->bounds_set = true;
         // F_SPHERE_FROM_GT and HAS_AABB change on full reads only, and the host queued every one of them: the light rows

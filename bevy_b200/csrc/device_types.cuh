@@ -241,6 +241,15 @@ struct ShadowBufs {
     uint32_t list_cap;
     uint32_t *active;        // [n_lights]: the light is in some view's VisibleEntities (written by k_shadow_select)
 };
+// b200vis_set_shadow_entities_sink as the shadow stage sees it (entities == nullptr: no sink)
+struct ShadowSink {
+    uint64_t *entities;      // device alias of the host region [capacity]
+    uint32_t capacity;
+    uint32_t *offsets;       // device alias of the host offsets [n_lights * 6 + 1]
+    uint8_t *active;         // device alias of the host active flags [n_lights]
+    uint32_t *dev_offsets;   // the device copy of offsets the expansion reads
+    const uint64_t *keys;    // the entity keys in rank order
+};
 
 // SURVEY 8(f) N2: the ViewClusterBindings wire format (bevy_pbr/src/cluster/mod.rs:584-800) packed on the device
 struct BindingBufs {

@@ -3216,9 +3216,11 @@ k_read_tables(Rows R, TableBufs tb, uint32_t which, uint32_t last_run, uint32_t 
 // Aabb / Sphere ticks and the InheritedVisibility ticks.  fresh[entry] marks a slot (re)mapped or a table (re)attached
 // since the last such read: that slot is read in full (flags rebuilt from the table's) and its mark cleared.  Otherwise
 // only newer columns are read, so only newer or fresh slots touch their map entry and their 4 to 32 bytes of payload.
+// tab_caster (b200vis_set_table_shadow_casters, nullptr = not attached): a full read also sets the row's shadow-caster byte
+// to its table's.
 __global__ void __launch_bounds__(256)
 k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, uint8_t *__restrict__ fresh, uint32_t last_run,
-                  uint32_t this_run) {
+                  uint32_t this_run, const uint8_t *__restrict__ tab_caster, uint8_t *__restrict__ caster) {
     __shared__ uint4 s_tk[8][2][33];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
@@ -3248,6 +3250,7 @@ k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, u
                 R.bndA[row] = make_float4(c[0], c[1], c[2], x[0]);
                 R.bndB[row] = C.is_aabb ? make_float2(x[1], x[2]) : make_float2(0.0f, 0.0f);
             }
+            if (full && tab_caster != nullptr) caster[row] = tab_caster[t];
             if (full || ni) {
                 const uint32_t iv = C.iv && C.iv[slot] ? (uint32_t)F_INHERITED : 0u;
                 const uint32_t f = R.flags[row];
@@ -3618,9 +3621,14 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
     }
 }
 // the sorted CubemapVisibleEntities lists from the bit sets (same chunked scan as k_expand_visible)
+// kSink: b200vis_set_shadow_entities_sink's instantiation, which also stores each entry's Entity key at off[list] + pos of
+// the host region (rank-ordered keys, so keys[rank] is the entry's key), each store checked against its own capacity and
+// the stores of a warp laid out consecutively
+template <bool kSink>
 __global__ void __launch_bounds__(kChunkWords)
 k_expand_shadow(ShadowBufs sb, uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride,
-                const uint32_t *__restrict__ row_of_rank) {
+                const uint32_t *__restrict__ row_of_rank, const uint64_t *__restrict__ keys, const uint32_t *__restrict__ off,
+                uint64_t *__restrict__ host_entities, uint32_t capacity) {
     __shared__ uint32_t s_warp[32];
     __shared__ uint32_t s_base, s_total;
     const uint32_t item = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
@@ -3658,6 +3666,22 @@ k_expand_shadow(ShadowBufs sb, uint32_t n_words, uint32_t n_chunks, uint32_t wor
         __syncthreads();
         uint32_t pos = s_base + (incl - c) + ((t >> 5) ? s_warp[(t >> 5) - 1] : 0u);
         uint32_t *out = sb.lists + (size_t)list * sb.list_cap;
+        if constexpr (kSink) {
+            // the warp's entries in order, 32 at a time: lane j stores entry k + j, so a warp's stores into the mapped sink are
+            // consecutive 8-byte words.  The entry's owner is the last lane whose exclusive count is <= it (counts ascend
+            // over the lanes), its bit the (e - ex + 1)-th set bit of the owner's word.
+            const uint32_t lane = t & 31u, ex = incl - c, wtot = __shfl_sync(0xFFFFFFFFu, incl, 31);
+            const uint32_t first = off[list] + s_base + ((t >> 5) ? s_warp[(t >> 5) - 1] : 0u);
+            for (uint32_t k = 0; k < wtot; k += 32u) {
+                const uint32_t e = k + lane;
+                uint32_t o = 0;
+#pragma unroll
+                for (uint32_t step = 16; step > 0; step >>= 1) if (__shfl_sync(0xFFFFFFFFu, ex, o + step) <= e) o += step;
+                const uint32_t wo = __shfl_sync(0xFFFFFFFFu, w, o), exo = __shfl_sync(0xFFFFFFFFu, ex, o);
+                if (e < wtot && first + e < capacity)
+                    host_entities[first + e] = keys[(word - lane + o) * 32u + __fns(wo, 0, (int)(e - exo + 1u))];
+            }
+        }
         while (w) {
             const uint32_t b = __ffs(w) - 1; w &= w - 1;
             const uint32_t rk = word * 32u + b;
@@ -3666,6 +3690,46 @@ k_expand_shadow(ShadowBufs sb, uint32_t n_words, uint32_t n_chunks, uint32_t wor
         }
         if (chunk == 0 && t == 0) sb.count[list] = s_total;
     }
+}
+
+// b200vis_set_shadow_entities_sink: every list's length (its chunk counts summed), scanned over the lists in item order
+// into offsets (the device copy the sink expansion reads and the host's), plus the items' active flags.  One CTA: a frame
+// has a few hundred lists of a few dozen chunks each.
+__global__ void __launch_bounds__(1024)
+k_shadow_offsets(ShadowBufs sb, uint32_t n_chunks, uint32_t chunks_stride, uint32_t *__restrict__ dev_off,
+                 uint32_t *__restrict__ host_off, uint8_t *__restrict__ host_active) {
+    __shared__ uint32_t s_warp[32];
+    __shared__ uint32_t s_carry;
+    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5, n_lists = sb.n_lights * 6u;
+    for (uint32_t i = t; i < sb.n_lights; i += 1024u) host_active[i] = sb.active[i] ? 1u : 0u;
+    if (t == 0) s_carry = 0;
+    for (uint32_t l0 = 0; l0 < n_lists; l0 += 1024u) {
+        const uint32_t l = l0 + t;
+        uint32_t c = 0;                                       // faces past an item's own are never counted: zero
+        if (l < n_lists) {
+            const uint32_t *cc = sb.chunk_count + (size_t)l * chunks_stride;
+            for (uint32_t k = 0; k < n_chunks; ++k) c += cc[k];
+        }
+        uint32_t incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += y; }
+        __syncthreads();                                      // the previous round's readers of s_warp / s_carry are done
+        if (lane == 31u) s_warp[warp] = incl;
+        __syncthreads();
+        if (warp == 0) {
+            uint32_t x = s_warp[lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (lane >= (uint32_t)o) x += y; }
+            s_warp[lane] = x;
+        }
+        __syncthreads();
+        const uint32_t excl = s_carry + (warp ? s_warp[warp - 1] : 0u) + (incl - c);
+        if (l < n_lists) { dev_off[l] = excl; host_off[l] = excl; }
+        __syncthreads();
+        if (t == 1023u) s_carry = excl + c;
+    }
+    __syncthreads();
+    if (t == 0) { dev_off[n_lists] = s_carry; host_off[n_lists] = s_carry; }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -4233,11 +4297,24 @@ void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const Clust
                                                                                 host_cap, stats, host_stats, changed_slot, frame, host_view_stats);
 }
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
-                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot) {
-    if (!sb.n_lights || !R.n) return;
+                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
+                        const ShadowSink &sink) {
+    if (!sb.n_lights || (!R.n && sink.entities == nullptr)) return;
     ++g_launches; k_shadow_select<<<cdiv(sb.n_lights, 128), 128, 0, st>>>(sb, R.rank, view_sets, words_stride, n_views);
+    if (!R.n) {                                       // no rows: every list is empty, the sink still gets offsets and flags
+        ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, 0u, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
+        return;
+    }
     ++g_launches; k_shadow_cull<<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
-    ++g_launches; k_expand_shadow<<<dim3(n_chunks, sb.n_lights), kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank);
+    const dim3 grid(n_chunks, sb.n_lights);
+    if (sink.entities == nullptr) {
+        ++g_launches; k_expand_shadow<false><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                           nullptr, nullptr, nullptr, 0u);
+        return;
+    }
+    ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
+    ++g_launches; k_expand_shadow<true><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                      sink.keys, sink.dev_offsets, sink.entities, sink.capacity);
 }
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views) {
     if (bb.mode) { ++g_launches; k_pack_cluster_bindings<<<dim3(16, max_views), 256, 0, st>>>(fc, cb, bb); }
@@ -4266,10 +4343,10 @@ void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uin
     ++g_launches; k_read_tables<<<grid, 256, 0, st>>>(R, tb, which, last_run, this_run);
 }
 void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
-                            uint32_t last_run, uint32_t this_run) {
+                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster) {
     if (!tb.n_chunks) return;
     const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
-    ++g_launches; k_read_table_cull<<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run);
+    ++g_launches; k_read_table_cull<<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run, tab_caster, caster);
 }
 void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick) {
     if (!tb.n_chunks) return;

@@ -28,8 +28,10 @@ void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, con
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R);
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views);
+// sink.entities != nullptr: also the Entity lists, offsets and active flags of b200vis_set_shadow_entities_sink
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
-                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot);
+                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
+                        const ShadowSink &sink);
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views);
 void launch_publish_visible_diff(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, uint32_t *host_rows, uint32_t host_stride,
                                  uint32_t *host_counts, uint32_t n_views, uint32_t max_views);
@@ -50,9 +52,10 @@ void launch_writeback_columns(cudaStream_t st, const Rows &R, float *host_gt, ui
 void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t gt_tick, uint32_t vv_tick);
 // b200vis_read_tables: which = B200VIS_RD_* bits, slots newer by Tick::is_newer_than(last_run, this_run)
 void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t last_run, uint32_t this_run);
-// b200vis_read_tables with RD_CULL_INPUTS: cull[t] = table t's cull inputs, fresh[entry] = read the slot in full (cleared)
+// b200vis_read_tables with RD_CULL_INPUTS: cull[t] = table t's cull inputs, fresh[entry] = read the slot in full (cleared);
+// tab_caster[t] (nullptr = no table casters attached) = the caster byte a full read gives the slot's row
 void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
-                            uint32_t last_run, uint32_t this_run);
+                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster);
 // b200vis_writeback_tables with WB_SET_VISIBLE: set_visible() over the bytes the table slots hold, vv_shadow marked unknown
 void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick);
 // b200vis_set_visible_entities_sink: counts = [max_views][chunks_stride][8] scratch, chunks_stride >= visible_entity_chunks(n_rows)

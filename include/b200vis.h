@@ -540,6 +540,10 @@ B200VIS_API int32_t b200vis_set_table_rows(b200vis_ctx *ctx, uint32_t table, uin
  *                           ViewVisibility write-back knows a slot holds: every mapped slot it covers is marked unknown, so
  *                           a later B200VIS_WB_VIEW_VISIBILITY sends every byte again.  Tables without view_visibility are
  *                           skipped.
+ *                           The light pass: b200vis_run_shadow_culling folds its set_visible() into the device bit 0, so
+ *                           a second call behind it, with the light system's tick, applies set_visible() to the rows
+ *                           only lights see; rows the cameras made visible already hold bit 0 and are left alone.  (The
+ *                           forked build's B200VIS_WB_VIEW_VISIBILITY after the shadow stage does the same job.)
  * Errors: NOT_READY (no b200vis_set_tables yet), UNSUPPORTED (world_size > 1), INVALID_ARG (B200VIS_WB_SET_VISIBLE with
  * B200VIS_WB_VIEW_VISIBILITY; nothing is enqueued then). */
 #define B200VIS_WB_SET_VISIBLE 0x4u
@@ -701,6 +705,47 @@ B200VIS_API int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items,
 B200VIS_API int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx);
 B200VIS_API int32_t b200vis_download_shadow_visible(b200vis_ctx *ctx, uint32_t shadow_light, uint32_t face, uint32_t *rows,
                                                     uint32_t capacity, uint32_t *count);
+/* The shadow lists as Entity values (CubemapVisibleEntities faces, the spot light's VisibleMeshEntities, a cascade's
+ * VisibleMeshEntities), every list of the run back to back in one region; list l = item * 6 + face.  Each entry is
+ * Entity::to_bits() as given to b200vis_set_topology / b200vis_edit_topology, so the shim fills each list with one
+ * extend_from_slice, as for b200vis_set_visible_entities_sink.  While the sink is registered, every
+ * b200vis_run_shadow_culling writes, on the context's stream (readable after the next b200vis_synchronize):
+ *   offsets[0 .. n_items*6]  exclusive prefix sums over the lists in item order: list l is entities[offsets[l] ..
+ *                            offsets[l+1]); faces 1-5 of spot and cascade items are empty.  offsets[n_items*6] is the
+ *                            true total, even when it exceeds capacity.
+ *   active[0 .. n_items)     1 when item i was culled this run: a point / spot item whose light is in some view's
+ *                            VisibleEntities (lib.rs:561-563), and every cascade item; 0 otherwise.  The lists of an
+ *                            inactive item are empty ranges, and its CubemapVisibleEntities / VisibleMeshEntities keep
+ *                            what they held (the reference `continue`s past such a light, lib.rs:568-586).
+ *   entities                 each list ascending by to_bits() (sort_unstable, lib.rs:493, 666, 745); no entry at or past
+ *                            capacity is written.
+ * Nothing past item n_items is written.  The lists come from the bit sets, not from the row lists, so the row lists can be
+ * kept at list_capacity = 1 (b200vis_download_shadow_visible then truncates, as it does today).  Pinned or registered
+ * like the result sink.  While the sink is set the entity keys stay resident on the device (8 bytes per max_entities
+ * row).  NULL removes the sink.
+ * Errors: INVALID_ARG (capacity 0, a NULL pointer, entities not 8-byte aligned), CAPACITY (max_items below the installed
+ * item count; b200vis_set_shadow_items / b200vis_set_shadow_lights with more items than a registered sink's max_items
+ * give CAPACITY too, and change nothing), UNSUPPORTED (world_size > 1). */
+typedef struct b200vis_shadow_entities_sink {
+    uint64_t *entities;   /* [capacity] every list of the run back to back; list l = item * 6 + face */
+    uint32_t  capacity;   /* entries in all lists together */
+    uint32_t  max_items;  /* offsets has max_items * 6 + 1 entries, active has max_items */
+    uint32_t *offsets;    /* [max_items * 6 + 1] */
+    uint8_t  *active;     /* [max_items] */
+} b200vis_shadow_entities_sink;
+B200VIS_API int32_t b200vis_set_shadow_entities_sink(b200vis_ctx *ctx, const b200vis_shadow_entities_sink *sink);
+/* The shadow-caster byte from the archetype tables: is_caster[t] = 1 when table t's archetype is in the light systems'
+ * visible_entity_query (With<Mesh3d>, Without<NotShadowCaster>, Without<DirectionalLight>; NoCpuCulling is a flag of
+ * the cull inputs, lib.rs:526-537, 690-701).  n_tables must equal the registry's size.  Like
+ * b200vis_upload_shadow_casters, the first attach allocates the caster column and switches on the visible-set
+ * bookkeeping.  While attached, b200vis_read_tables(B200VIS_RD_CULL_INPUTS, ..) writes the caster byte of every slot it
+ * reads in full (b200vis_set_table_cull_inputs says which), and a table whose is_caster differs from the previous attach
+ * (every table, on an attach after none) is read in full at the next such read.  Rows of tables that are not read keep
+ * the byte b200vis_upload_shadow_casters gave them.  b200vis_set_tables / _ex drop the attachment as they drop the cull
+ * inputs; NULL, 0 detaches.
+ * Errors: INVALID_ARG (n_tables differs from the registry's size, is_caster NULL with n_tables > 0), NOT_READY (no tables
+ * registered), UNSUPPORTED (world_size > 1); nothing changes then. */
+B200VIS_API int32_t b200vis_set_table_shadow_casters(b200vis_ctx *ctx, uint32_t n_tables, const uint8_t *is_caster);
 /* update_point_light_frusta for one light (no GPU needed): light_gt12 as in upload_global_transforms */
 B200VIS_API void b200vis_host_point_light_frusta(const float *light_gt12, float range, float shadow_map_near_z, float frusta[6][6][4]);
 
