@@ -278,6 +278,66 @@ def host_table_cull_inputs(capacities, layout=BEVY_BOUNDS_LAYOUT, tick_fill=0, b
     return out, buf
 
 
+class VisibilityRangeLayout(C.Structure):
+    """b200vis_visibility_range_layout: bytes per VisibilityRange and the byte offsets of start_margin.start,
+    end_margin.end (f32) and use_aabb (bool)."""
+    _fields_ = [("stride", C.c_uint32), ("start", C.c_uint32), ("end", C.c_uint32), ("use_aabb", C.c_uint32)]
+
+
+# A guess of rustc's layout of VisibilityRange { start_margin: Range<f32>, end_margin: Range<f32>, use_aabb: bool }: the
+# fields in order, 20 bytes.  repr(Rust) promises nothing: the plugin passes size_of / offset_of!, and tests never rely
+# on this guess.
+BEVY_VISIBILITY_RANGE_LAYOUT = (20, 0, 12, 16)
+
+
+class TableVisibilityRanges(C.Structure):
+    """b200vis_table_visibility_ranges: a table's VisibilityRange column and its ticks."""
+    _fields_ = [("ranges", C.c_void_p), ("changed_ticks", C.c_void_p)]
+
+
+class HostRanges:
+    """A table's VisibilityRange column as raw bytes [capacity, stride] in `layout`, with ticks [capacity] uint32."""
+
+    def __init__(self, ranges, ticks, layout):
+        self.ranges, self.ticks, self.layout = ranges, ticks, tuple(layout)
+
+    def put(self, slots, start_end, use_aabb):
+        """Write (start_margin.start, end_margin.end) [k, 2] and the use_aabb bytes [k] into the slots."""
+        slots = np.asarray(slots, np.int64)
+        se = np.ascontiguousarray(start_end, np.float32).reshape(len(slots), 2)
+        _, so, eo, uo = self.layout
+        self.ranges[slots, so:so + 4] = se[:, 0:1].copy().view(np.uint8)
+        self.ranges[slots, eo:eo + 4] = se[:, 1:2].copy().view(np.uint8)
+        self.ranges[slots, uo] = np.asarray(use_aabb, np.uint8)
+
+    def get(self, slots):
+        """([k, 2] float32 (start, end), [k] uint8 use_aabb bytes)."""
+        b = self.ranges[np.asarray(slots, np.int64)]
+        _, so, eo, uo = self.layout
+        se = np.concatenate([np.ascontiguousarray(b[:, o:o + 4]).view(np.float32) for o in (so, eo)], axis=1)
+        return se, b[:, uo].copy()
+
+    def desc(self):
+        return TableVisibilityRanges(self.ranges.ctypes.data, self.ticks.ctypes.data)
+
+
+def host_table_ranges(capacities, layout=BEVY_VISIBILITY_RANGE_LAYOUT, tick_fill=0, byte_fill=0xFF, pad=64):
+    """VisibilityRange columns with ticks over ONE plain numpy buffer, beside host_tables' (same page rules).  Returns
+    (ranges, buffer)."""
+    st = int(layout[0])
+    al = lambda b: (b + pad - 1) // pad * pad
+    page = 4096
+    total = sum(al(c * st) + al(c * 4) for c in capacities)
+    buf = np.zeros((total + 2 * page - 1) // page * page + page, np.uint8)
+    o, out = (-buf.ctypes.data) % page, []
+    for c in capacities:
+        r = buf[o:o + c * st].reshape(c, st); o += al(c * st)
+        t = buf[o:o + c * 4].view(np.uint32); o += al(c * 4)
+        r[:] = byte_fill; t[:] = tick_fill
+        out.append(HostRanges(r, t, layout))
+    return out, buf
+
+
 class ShadowItem(C.Structure):
     _fields_ = [("kind", C.c_uint32), ("light_row", C.c_uint32), ("range", C.c_float), ("range_view_index", C.c_int32),
                 ("layer_mask", C.c_uint64), ("frusta", C.c_float * 144)]
@@ -334,6 +394,7 @@ _SIGNATURES = {
     "b200vis_read_tables": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, C.c_uint32]),
     "b200vis_set_table_cull_inputs": (C.c_int32, [_vp, C.c_uint32, _vp, _P(BoundsLayout)]),
     "b200vis_set_table_shadow_casters": (C.c_int32, [_vp, C.c_uint32, _vp]),
+    "b200vis_set_table_visibility_ranges": (C.c_int32, [_vp, C.c_uint32, _vp, _P(VisibilityRangeLayout)]),
     "b200vis_host_plan_summary": (C.c_int32, [C.c_uint32, _vp, _P(C.c_uint32)]),
     "b200vis_host_tile_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp]),
     "b200vis_host_warp_plan": (C.c_int32, [C.c_uint32, _vp, C.c_uint32, C.c_uint32, _P(C.c_uint32), _vp, _vp, _vp, _vp]),
@@ -1062,6 +1123,22 @@ class Context:
         if n > len(c):                                       # the library reads is_caster[n_tables]
             raise ValueError(f"set_table_shadow_casters: n_tables {n} > {len(c)} entries")
         self._check(self._lib.b200vis_set_table_shadow_casters(self._h, n, _ptr(c)))
+
+    def set_table_visibility_ranges(self, ranges, layout=BEVY_VISIBILITY_RANGE_LAYOUT, n_tables=None):
+        """b200vis_set_table_visibility_ranges: `ranges` = one HostRanges / TableVisibilityRanges / None (no range
+        column) per registered table, or None to detach; `layout` a VisibilityRangeLayout, a 4-tuple or None (NULL).
+        n_tables overrides the count passed (argument tests)."""
+        lay = None if layout is None else (layout if isinstance(layout, VisibilityRangeLayout) else VisibilityRangeLayout(*layout))
+        if ranges is None:
+            self._check(self._lib.b200vis_set_table_visibility_ranges(self._h, 0 if n_tables is None else n_tables, None,
+                                                                      None if lay is None else C.byref(lay)))
+            return
+        descs = [r.desc() if isinstance(r, HostRanges) else (TableVisibilityRanges() if r is None else r) for r in ranges]
+        arr = (TableVisibilityRanges * max(len(descs), 1))(*descs)
+        n = len(descs) if n_tables is None else n_tables
+        if n > len(descs):                                   # the library reads ranges[n_tables]
+            raise ValueError(f"set_table_visibility_ranges: n_tables {n} > {len(descs)} entries")
+        self._check(self._lib.b200vis_set_table_visibility_ranges(self._h, n, arr, None if lay is None else C.byref(lay)))
 
     def p2p_export(self):
         """CUDA IPC handle (64 bytes) of this rank's gathered buffer."""

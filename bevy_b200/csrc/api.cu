@@ -193,6 +193,11 @@ struct b200vis_ctx {
     DevTableCull *d_tab_cull = nullptr; uint8_t *d_tab_fresh = nullptr;
     // b200vis_set_table_shadow_casters: the attached per-table caster bytes, and their device copy
     std::vector<uint8_t> h_tab_caster; bool caster_attached = false; uint8_t *d_tab_caster = nullptr;
+    // b200vis_set_table_visibility_ranges: the last attached entries (a table that stays keeps its entry across set_tables,
+    // so its columns stay registered and it is not read in full when attached again unchanged; empty = none attached),
+    // whether some table's are read, their layout, and their device form
+    std::vector<b200vis_table_visibility_ranges> h_tab_range; b200vis_visibility_range_layout range_layout{};
+    bool range_attached = false; DevTableRange *d_tab_range = nullptr;
     bool cull_fresh_pending = false;    // slots (re)mapped or tables (re)attached since the last RD_CULL_INPUTS read
     double step_t[6] = {0, 0, 0, 0, 0, 0}; uint64_t step_n = 0;   // B200VIS_STEP_TRACE: host time per phase of b200vis_step
     void *nccl_comm = nullptr;          // b200vis_comm_init
@@ -255,7 +260,8 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_shadow_lights, ctx->d_caster, ctx->shadow.mask, ctx->shadow.chunk_count, ctx->shadow.lists,
                    ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
                    ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
-                   ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster};
+                   ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster,
+                   ctx->d_tab_range};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -3129,15 +3135,21 @@ static void cull_columns(size_t cap, const b200vis_table_cull_inputs &cu, const 
     fn(cu.spheres, cap * bl.sphere_stride); fn(cu.sphere_changed_ticks, cap * 4);
     fn(cu.inherited_visibility, cap); fn(cu.iv_changed_ticks, cap * 4);
 }
-// every column of a table: the outputs, the Transform input and the cull inputs, as (pointer, bytes)
+template <typename Fn>
+static void range_columns(size_t cap, const b200vis_table_visibility_ranges &rg, uint32_t stride, Fn &&fn) {
+    fn(rg.ranges, cap * stride); fn(rg.changed_ticks, cap * 4);
+}
+// every column of a table: the outputs, the Transform input, the cull inputs and the VisibilityRange column, as
+// (pointer, bytes)
 template <typename Fn>
 static void table_columns(const b200vis_table &tb, const b200vis_table_inputs &in, uint32_t trs_stride, const b200vis_table_cull_inputs &cu,
-                          const b200vis_bounds_layout &bl, Fn &&fn) {
+                          const b200vis_bounds_layout &bl, const b200vis_table_visibility_ranges &rg, uint32_t range_stride, Fn &&fn) {
     const size_t cap = tb.capacity;
     fn(tb.global_transforms, cap * 64); fn(tb.gt_changed_ticks, cap * 4);
     fn(tb.view_visibility, cap); fn(tb.vv_changed_ticks, cap * 4);
     fn(in.transforms, cap * trs_stride); fn(in.transform_changed_ticks, cap * 4);
     cull_columns(cap, cu, bl, fn);
+    range_columns(cap, rg, range_stride, fn);
 }
 // a column the registry uses: registered by the library unless its owner pinned it
 static void need_column(b200vis_ctx *ctx, const void *p, size_t bytes, bool changed, ColumnRanges &cr) {
@@ -3200,6 +3212,7 @@ static int32_t register_columns(b200vis_ctx *ctx, ColumnRanges &cr, const char *
             ctx->host_regs.clear(); ctx->h_tabs.clear(); ctx->h_tab_in.clear(); ctx->tab_off.clear(); ctx->h_tab_map.clear();
             ctx->h_tab_cull.clear(); ctx->cull_attached = false;
             ctx->h_tab_caster.clear(); ctx->caster_attached = false;
+            ctx->h_tab_range.clear(); ctx->range_attached = false;
             std::fill(ctx->row_slot.begin(), ctx->row_slot.end(), kUnmapped);
             ctx->n_tab_chunks = 0;
             return fail(ctx, B200VIS_ERR_CUDA, "%s: cudaHostRegister of %zu bytes at %p failed: %s", who, (size_t)(r.second - r.first),
@@ -3285,14 +3298,21 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
     auto kept_cull = [&](uint32_t t) -> const b200vis_table_cull_inputs & {
         return t < n_old && t < ctx->h_tab_cull.size() && !moved(t) ? ctx->h_tab_cull[t] : no_cull;
     };
+    const b200vis_table_visibility_ranges no_range{};
+    auto held_range = [&](uint32_t t) -> const b200vis_table_visibility_ranges & {
+        return t < ctx->h_tab_range.size() ? ctx->h_tab_range[t] : no_range;
+    };
+    std::vector<b200vis_table_visibility_ranges> kept_range(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t) if (t < n_old && !moved(t)) kept_range[t] = held_range(t);
     ColumnRanges cr;
     for (uint32_t t = 0; t < n_tables; ++t)
-        table_columns(tables[t], input(t), lay.stride, kept_cull(t), ctx->cull_layout,
+        table_columns(tables[t], input(t), lay.stride, kept_cull(t), ctx->cull_layout, kept_range[t], ctx->range_layout.stride,
                       [&](const void *p, size_t bytes) { need_column(ctx, p, bytes, moved(t), cr); });
     for (uint32_t t = 0; t < n_old; ++t)
         if (moved(t))
             table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, t < ctx->h_tab_cull.size() ? ctx->h_tab_cull[t] : no_cull,
-                          ctx->cull_layout, [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); });
+                          ctx->cull_layout, held_range(t), ctx->range_layout.stride,
+                          [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); });
     { const int32_t rrc = register_columns(ctx, cr, "set_tables"); if (rrc) return rrc; }
     // ---- the device registry: table descriptors, chunk -> table, and the maps when their layout changed ----
     std::vector<DevTable> dt(n_tables);
@@ -3351,6 +3371,7 @@ extern "C" int32_t b200vis_set_tables_ex(b200vis_ctx *ctx, uint32_t n_tables, co
     ctx->tables_set = true;
     ctx->cull_attached = false;              // the cull inputs are attached again by b200vis_set_table_cull_inputs
     ctx->caster_attached = false; ctx->h_tab_caster.clear();   // ... and the table casters by b200vis_set_table_shadow_casters
+    ctx->range_attached = false; ctx->h_tab_range = std::move(kept_range);   // ... and the ranges (kept: registrations held)
     queue_table_updates(ctx, {}, reset);
     return B200VIS_OK;
 }
@@ -3402,6 +3423,51 @@ static bool cull_same(const b200vis_table_cull_inputs &a, const b200vis_bounds_l
            (!a.spheres || a.aabbs || (la.sphere_stride == lb.sphere_stride && la.sphere_center == lb.sphere_center && la.sphere_radius == lb.sphere_radius));
 }
 
+// table t's cull inputs as k_read_table_cull sees them (the aliases derived from the current registrations)
+static cudaError_t dev_cull(const b200vis_ctx *ctx, uint32_t t, const b200vis_table_cull_inputs &c, const b200vis_bounds_layout &lay,
+                            DevTableCull &d) {
+    const uint32_t cap = ctx->h_tabs[t].capacity;
+    cudaError_t lost = cudaSuccess;
+    auto alias = [&](const void *p) -> const void * {
+        void *dp = nullptr;
+        if (!p || !cap) return nullptr;
+        const cudaError_t e = cudaHostGetDevicePointer(&dp, const_cast<void *>(p), 0);
+        if (e != cudaSuccess) lost = e;
+        return dp;
+    };
+    const bool aabb = c.aabbs != nullptr;
+    d = DevTableCull{};
+    d.bnd = static_cast<const uint8_t *>(alias(aabb ? c.aabbs : c.spheres));
+    d.bnd_ticks = static_cast<const uint32_t *>(alias(aabb ? c.aabb_changed_ticks : c.sphere_changed_ticks));
+    d.iv = static_cast<const uint8_t *>(alias(c.inherited_visibility));
+    d.iv_ticks = static_cast<const uint32_t *>(alias(c.iv_changed_ticks));
+    d.flags = c.flags | (aabb ? B200VIS_F_HAS_AABB : c.spheres ? B200VIS_F_HAS_SPHERE : 0u);
+    d.read = cull_reads(c) && cap ? 1u : 0u;
+    d.stride = aabb ? lay.aabb_stride : lay.sphere_stride;
+    d.c_off = aabb ? lay.aabb_center : lay.sphere_center;
+    d.e_off = aabb ? lay.aabb_half_extents : lay.sphere_radius;
+    d.is_aabb = aabb;
+    return lost;
+}
+static const b200vis_table_visibility_ranges &held_range(const b200vis_ctx *ctx, uint32_t t) {
+    static const b200vis_table_visibility_ranges none{};
+    return t < ctx->h_tab_range.size() ? ctx->h_tab_range[t] : none;
+}
+// the device form of per-table range entries: the aliases of the registered columns, derived again whenever
+// registrations may have moved
+static cudaError_t dev_ranges(const b200vis_ctx *ctx, const std::vector<b200vis_table_visibility_ranges> &rg, std::vector<DevTableRange> &out) {
+    out.assign(rg.size(), DevTableRange{nullptr, nullptr});
+    for (size_t t = 0; t < rg.size(); ++t) {
+        if (!rg[t].ranges || !ctx->h_tabs[t].capacity) continue;
+        void *d = nullptr, *dt = nullptr;
+        cudaError_t e = cudaHostGetDevicePointer(&d, const_cast<void *>(rg[t].ranges), 0);
+        if (e == cudaSuccess) e = cudaHostGetDevicePointer(&dt, const_cast<uint32_t *>(rg[t].changed_ticks), 0);
+        if (e != cudaSuccess) return e;
+        out[t] = DevTableRange{static_cast<const uint8_t *>(d), static_cast<const uint32_t *>(dt)};
+    }
+    return cudaSuccess;
+}
+
 extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_cull_inputs *inputs,
                                                  const b200vis_bounds_layout *layout) {
     CHECK_CTX_JOIN();
@@ -3424,6 +3490,11 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
         if (c.flags & ~kArchetypeBits)
             return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: table %u: flags 0x%x has bits other than the per-archetype ones", t, c.flags);
         any_aabb |= c.aabbs != nullptr; any_sphere |= c.spheres != nullptr;
+        // while ranges are attached, HAS_VIS_RANGE and a range column go together (b200vis_set_table_visibility_ranges)
+        if (ctx->range_attached && ((c.flags & B200VIS_F_HAS_VIS_RANGE) != 0) != (ctx->h_tab_range[t].ranges != nullptr))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: table %u: HAS_VIS_RANGE %s while its VisibilityRange "
+                        "column is %s; detach the ranges first", t, (c.flags & B200VIS_F_HAS_VIS_RANGE) ? "set" : "clear",
+                        ctx->h_tab_range[t].ranges ? "attached" : "absent");
     }
     if ((any_aabb || any_sphere) && !layout)
         return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_cull_inputs: a table has aabbs or spheres but no layout was given");
@@ -3459,7 +3530,7 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
     ColumnRanges cr;
     for (uint32_t t = 0; t < n_tables; ++t) {
         const bool moved = !cull_same(inputs[t], lay, prev(t), ctx->cull_layout);
-        table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, inputs[t], lay,
+        table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, inputs[t], lay, held_range(ctx, t), ctx->range_layout.stride,
                       [&](const void *p, size_t bytes) { need_column(ctx, p, bytes, false, cr); });
         if (moved) {
             auto changed = [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); };
@@ -3474,6 +3545,7 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
     auto detach = [&](cudaError_t e, const char *what, uint32_t t) {
         ctx->cull_attached = false;
         ctx->h_tab_cull.clear();
+        ctx->range_attached = false; ctx->h_tab_range.clear();   // the ranges' aliases may have moved as well
         return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA,
                     "set_table_cull_inputs: table %u: %s: %s", t, what, cudaGetErrorString(e));
     };
@@ -3489,30 +3561,9 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
     std::vector<DevTableCull> dc(n_tables);
     bool any = false;
     for (uint32_t t = 0; t < n_tables; ++t) {
-        const b200vis_table_cull_inputs &c = inputs[t];
-        const uint32_t cap = ctx->h_tabs[t].capacity;
-        cudaError_t lost = cudaSuccess;
-        auto alias = [&](const void *p) -> const void * {
-            void *d = nullptr;
-            if (!p || !cap) return nullptr;
-            const cudaError_t e = cudaHostGetDevicePointer(&d, const_cast<void *>(p), 0);
-            if (e != cudaSuccess) lost = e;
-            return d;
-        };
-        const bool aabb = c.aabbs != nullptr;
-        DevTableCull &d = dc[t];
-        d.bnd = static_cast<const uint8_t *>(alias(aabb ? c.aabbs : c.spheres));
-        d.bnd_ticks = static_cast<const uint32_t *>(alias(aabb ? c.aabb_changed_ticks : c.sphere_changed_ticks));
-        d.iv = static_cast<const uint8_t *>(alias(c.inherited_visibility));
-        d.iv_ticks = static_cast<const uint32_t *>(alias(c.iv_changed_ticks));
+        const cudaError_t lost = dev_cull(ctx, t, inputs[t], lay, dc[t]);
         if (lost != cudaSuccess) return detach(lost, "no device alias for a registered column", t);
-        d.flags = c.flags | (aabb ? B200VIS_F_HAS_AABB : c.spheres ? B200VIS_F_HAS_SPHERE : 0u);
-        d.read = cull_reads(c) && cap ? 1u : 0u;
-        d.stride = aabb ? lay.aabb_stride : lay.sphere_stride;
-        d.c_off = aabb ? lay.aabb_center : lay.sphere_center;
-        d.e_off = aabb ? lay.aabb_half_extents : lay.sphere_radius;
-        d.is_aabb = aabb;
-        any |= d.read != 0;
+        any |= dc[t].read != 0;
     }
     cudaStream_t st = ctx->stream;
     cudaError_t e = cudaSuccess;
@@ -3521,6 +3572,12 @@ extern "C" int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_ta
         return detach(e, "table descriptors", 0);
     if ((e = cudaMemcpyAsync(ctx->d_tab_cull, dc.data(), dc.size() * sizeof(DevTableCull), cudaMemcpyHostToDevice, st)) != cudaSuccess)
         return detach(e, "cull descriptors", 0);
+    if (ctx->range_attached) {                  // a range column sharing a page with a cull column may have been registered anew
+        std::vector<DevTableRange> dr;
+        if ((e = dev_ranges(ctx, ctx->h_tab_range, dr)) != cudaSuccess) return detach(e, "no device alias for a range column", 0);
+        if ((e = cudaMemcpyAsync(ctx->d_tab_range, dr.data(), dr.size() * sizeof(DevTableRange), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+            return detach(e, "range descriptors", 0);
+    }
     bool pending = false;
     for (uint32_t t = 0; t < n_tables; ++t)
         if (full[t] && ctx->h_tabs[t].capacity) {
@@ -3570,6 +3627,129 @@ extern "C" int32_t b200vis_set_table_shadow_casters(b200vis_ctx *ctx, uint32_t n
     return B200VIS_OK;
 }
 
+static bool range_same(const b200vis_table_visibility_ranges &a, const b200vis_visibility_range_layout &la,
+                       const b200vis_table_visibility_ranges &b, const b200vis_visibility_range_layout &lb) {
+    return a.ranges == b.ranges && a.changed_ticks == b.changed_ticks &&
+           (!a.ranges || (la.stride == lb.stride && la.start == lb.start && la.end == lb.end && la.use_aabb == lb.use_aabb));
+}
+
+extern "C" int32_t b200vis_set_table_visibility_ranges(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_visibility_ranges *ranges,
+                                                       const b200vis_visibility_range_layout *layout) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_table_visibility_ranges: world_size > 1");
+    if (!n_tables && !ranges) { ctx->range_attached = false; ctx->h_tab_range.clear(); return B200VIS_OK; }
+    if (!ctx->tables_set || ctx->h_tabs.empty()) return fail(ctx, B200VIS_ERR_NOT_READY, "set_table_visibility_ranges: no tables are registered");
+    if (n_tables != ctx->h_tabs.size())
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: %u entries for %zu registered tables", n_tables, ctx->h_tabs.size());
+    if (!ranges) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: null ranges");
+    bool any = false;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const b200vis_table_visibility_ranges &r = ranges[t];
+        if ((r.ranges == nullptr) != (r.changed_ticks == nullptr))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: table %u: ranges and changed_ticks must both be NULL or both be set", t);
+        if ((uintptr_t)r.ranges % 4u || (uintptr_t)r.changed_ticks % 4u)   // the kernel reads f32 fields and u32 ticks
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: table %u: columns need 4-byte alignment", t);
+        // no row is range-tested with parameters nobody supplied: HAS_VIS_RANGE in the attached cull inputs exactly when
+        // the table has a range column
+        const bool ranged = ctx->cull_attached && t < ctx->h_tab_cull.size() && (ctx->h_tab_cull[t].flags & B200VIS_F_HAS_VIS_RANGE);
+        if (ranged != (r.ranges != nullptr))
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: table %u: %s, but its attached cull inputs %s HAS_VIS_RANGE", t,
+                        r.ranges ? "a VisibilityRange column" : "no VisibilityRange column", ranged ? "carry" : "lack");
+        any |= r.ranges != nullptr;
+    }
+    if (any && !layout) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: a table has ranges but no layout was given");
+    b200vis_visibility_range_layout lay{};
+    if (any) {
+        lay = *layout;
+        const uint64_t lo[3] = {lay.start, lay.end, lay.use_aabb}, sz[3] = {4, 4, 1};
+        if (lay.stride % 4u || lay.start % 4u || lay.end % 4u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: the float fields and the stride need 4-byte alignment");
+        for (int i = 0; i < 3; ++i) {
+            if (lo[i] + sz[i] > lay.stride)
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: field at %llu runs past stride %u", (unsigned long long)lo[i], lay.stride);
+            for (int j = 0; j < i; ++j)
+                if (lo[i] < lo[j] + sz[j] && lo[j] < lo[i] + sz[i])
+                    return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_table_visibility_ranges: fields at %llu and %llu overlap",
+                                (unsigned long long)lo[j], (unsigned long long)lo[i]);
+        }
+    }
+    // the resident range columns, as b200vis_upload_visibility_ranges allocates them
+    if (!ctx->d_range_se) {
+        CU(dalloc(&ctx->d_range_se, ctx->cfg.max_entities));
+        CU(dalloc(&ctx->d_range_ua, ctx->cfg.max_entities));
+        CU(dalloc(&ctx->d_range_views, 32));
+    }
+    if (!ctx->d_tab_range) CU(dalloc(&ctx->d_tab_range, B200VIS_MAX_TABLES));
+    CU(cudaStreamSynchronize(ctx->stream));   // no read in flight reads the old range columns or registrations
+    // a table whose entry changed is read in full: every table with ranges on an attach after none (h_tab_range is
+    // empty then); b200vis_set_tables keeps the entries of the tables that stay, as for the cull inputs
+    std::vector<bool> full(n_tables);
+    for (uint32_t t = 0; t < n_tables; ++t)
+        full[t] = ranges[t].ranges && (ctx->h_tab_range.empty() || !range_same(ranges[t], lay, held_range(ctx, t), ctx->range_layout));
+    // ---- registrations: every table's columns with the new ranges; range columns that changed may be reallocated ----
+    const b200vis_table_cull_inputs no_cull{};
+    const uint32_t chunks = ctx->n_tab_chunks;
+    ColumnRanges cr;
+    for (uint32_t t = 0; t < n_tables; ++t) {
+        const b200vis_table_cull_inputs &cu = t < ctx->h_tab_cull.size() ? ctx->h_tab_cull[t] : no_cull;
+        table_columns(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout.stride, cu, ctx->cull_layout, ranges[t], lay.stride,
+                      [&](const void *p, size_t bytes) { need_column(ctx, p, bytes, false, cr); });
+        if (!range_same(ranges[t], lay, held_range(ctx, t), ctx->range_layout)) {
+            auto changed = [&](const void *p, size_t bytes) { if (p && bytes) cr.changed.push_back(page_range(p, bytes)); };
+            range_columns(ctx->h_tabs[t].capacity, ranges[t], lay.stride, changed);
+            range_columns(ctx->h_tabs[t].capacity, held_range(ctx, t), ctx->range_layout.stride, changed);
+        }
+    }
+    { const int32_t rrc = register_columns(ctx, cr, "set_table_visibility_ranges"); if (rrc) return rrc; }
+    ctx->n_tab_chunks = chunks;
+    // From here on registrations may have moved: a failure detaches the cull inputs and the ranges (the next calls read
+    // every table they attach in full) instead of leaving the device pointed at released ranges.
+    auto detach = [&](cudaError_t e, const char *what) {
+        ctx->cull_attached = false; ctx->h_tab_cull.clear();
+        ctx->range_attached = false; ctx->h_tab_range.clear();
+        return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA,
+                    "set_table_visibility_ranges: %s: %s", what, cudaGetErrorString(e));
+    };
+    // ---- the descriptors again: the table's, its cull inputs' and the ranges' aliases ----
+    cudaStream_t st = ctx->stream;
+    cudaError_t e = cudaSuccess;
+    std::vector<DevTable> dt(n_tables);
+    for (uint32_t t = 0, c = 0; t < n_tables; ++t) {
+        if ((e = dev_table(ctx->h_tabs[t], ctx->h_tab_in[t], ctx->tab_layout, ctx->tab_off[t], c, dt[t])) != cudaSuccess)
+            return detach(e, "no device alias for a registered column");
+        c += (ctx->h_tabs[t].len + 127u) / 128u;
+    }
+    if ((e = cudaMemcpyAsync(ctx->d_tabs, dt.data(), dt.size() * sizeof(DevTable), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+        return detach(e, "table descriptors");
+    if (ctx->cull_attached) {
+        std::vector<DevTableCull> dc(n_tables);
+        for (uint32_t t = 0; t < n_tables; ++t) if ((e = dev_cull(ctx, t, ctx->h_tab_cull[t], ctx->cull_layout, dc[t])) != cudaSuccess)
+            return detach(e, "no device alias for a cull column");
+        if ((e = cudaMemcpyAsync(ctx->d_tab_cull, dc.data(), dc.size() * sizeof(DevTableCull), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+            return detach(e, "cull descriptors");
+    }
+    std::vector<b200vis_table_visibility_ranges> rg(ranges, ranges + n_tables);
+    std::vector<DevTableRange> dr;
+    if ((e = dev_ranges(ctx, rg, dr)) != cudaSuccess) return detach(e, "no device alias for a range column");
+    if ((e = cudaMemcpyAsync(ctx->d_tab_range, dr.data(), dr.size() * sizeof(DevTableRange), cudaMemcpyHostToDevice, st)) != cudaSuccess)
+        return detach(e, "range descriptors");
+    bool pending = false;
+    for (uint32_t t = 0; t < n_tables; ++t)
+        if (full[t] && ctx->h_tabs[t].capacity) {
+            if ((e = cudaMemsetAsync(ctx->d_tab_fresh + ctx->tab_off[t], 1, ctx->h_tabs[t].capacity, st)) != cudaSuccess)
+                return detach(e, "full-read marks");
+            pending = true;
+        }
+    if ((e = cudaStreamSynchronize(st)) != cudaSuccess) return detach(e, "cudaStreamSynchronize");
+    // ---- commit ----
+    ctx->cull_fresh_pending |= pending;
+    ctx->h_tab_range = std::move(rg);
+    ctx->range_layout = lay;
+    ctx->range_attached = any;
+    ctx->have_range = true;   // as after b200vis_upload_visibility_ranges: the cull kernels take the non-SIMPLE path
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_writeback_tables(b200vis_ctx *ctx, uint32_t which, uint32_t gt_tick, uint32_t vv_tick) {
     CHECK_CTX();
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "writeback_tables: world_size > 1");
@@ -3596,8 +3776,14 @@ extern "C" int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32_
     launch_read_tables(ctx->stream, ctx->rows, tb, which & (B200VIS_RD_TRANSFORM | B200VIS_RD_GLOBAL_TRANSFORM), last_run, this_run);
     CU(cudaGetLastError());
     if ((which & B200VIS_RD_CULL_INPUTS) && ctx->cull_attached) {
+        // a read while range entries are held but not attached consumes fresh marks without writing range parameters:
+        // the next attach must then read every ranged table in full, as after a detach
+        if (!ctx->range_attached) ctx->h_tab_range.clear();
+        const b200vis_visibility_range_layout &rl = ctx->range_layout;
+        const RangeRead rr{ctx->range_attached ? ctx->d_tab_range : nullptr, rl.stride, rl.start, rl.end, rl.use_aabb,
+                           ctx->d_range_se, ctx->d_range_ua};
         launch_read_table_cull(ctx->stream, ctx->rows, tb, ctx->d_tab_cull, ctx->d_tab_fresh, last_run, this_run,
-                               ctx->caster_attached ? ctx->d_tab_caster : nullptr, ctx->d_caster);
+                               ctx->caster_attached ? ctx->d_tab_caster : nullptr, ctx->d_caster, rr);
         CU(cudaGetLastError());
         ctx->bounds_set = true;
         // F_SPHERE_FROM_GT and HAS_AABB change on full reads only, and the host queued every one of them: the light rows

@@ -302,6 +302,16 @@ struct DevTableCull {
     uint32_t stride, c_off, e_off;   // bytes per slot, center, half_extents (Aabb) or radius (Sphere)
     uint32_t is_aabb;
 };
+// b200vis_set_table_visibility_ranges: one table's VisibilityRange column and ticks (device aliases, nullptr = none)
+struct DevTableRange {
+    const uint8_t *ranges; const uint32_t *ticks;
+};
+// ... all tables', their layout in bytes, and the resident range columns k_unpack_range_params fills
+struct RangeRead {
+    const DevTableRange *tables;
+    uint32_t stride, start, end, use_aabb;
+    float2 *se; uint8_t *ua;
+};
 
 // b200vis_compact_topology: row-valued lists (list l = rows[l * stride .. + count[l * count_step]))
 struct RowLists {

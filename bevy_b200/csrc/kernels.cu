@@ -3218,10 +3218,14 @@ k_read_tables(Rows R, TableBufs tb, uint32_t which, uint32_t last_run, uint32_t 
 // only newer columns are read, so only newer or fresh slots touch their map entry and their 4 to 32 bytes of payload.
 // tab_caster (b200vis_set_table_shadow_casters, nullptr = not attached): a full read also sets the row's shadow-caster byte
 // to its table's.
+// RANGES (b200vis_set_table_visibility_ranges attached): the VisibilityRange tick column is staged beside the others, and a
+// full read or a newer range tick stores the slot's (start_margin.start, end_margin.end) and use_aabb where
+// k_unpack_range_params stores them.  Without it the kernel is what it was.
+template <bool RANGES>
 __global__ void __launch_bounds__(256)
 k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, uint8_t *__restrict__ fresh, uint32_t last_run,
-                  uint32_t this_run, const uint8_t *__restrict__ tab_caster, uint8_t *__restrict__ caster) {
-    __shared__ uint4 s_tk[8][2][33];
+                  uint32_t this_run, const uint8_t *__restrict__ tab_caster, uint8_t *__restrict__ caster, RangeRead rr) {
+    __shared__ uint4 s_tk[8][RANGES ? 3 : 2][33];
     const uint32_t lane = threadIdx.x & 31u, warp = threadIdx.x >> 5;
     for (uint32_t ch = blockIdx.x * 8u + warp; ch < tb.n_chunks; ch += gridDim.x * 8u) {
         const uint32_t t = tb.chunk_table[ch];
@@ -3232,15 +3236,23 @@ k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, u
         const uint32_t base = (ch - T.chunk_begin) * 128u, n = min(len - base, 128u);
         const uint32_t hb = C.bnd ? stage_ticks(C.bnd_ticks, base, base + n, lane, s_tk[warp][0]) : 0u;
         const uint32_t hi = C.iv ? stage_ticks(C.iv_ticks, base, base + n, lane, s_tk[warp][1]) : 0u;
+        DevTableRange G{nullptr, nullptr};
+        uint32_t hr = 0u;
+        if constexpr (RANGES) {
+            G = rr.tables[t];
+            if (G.ranges) hr = stage_ticks(G.ticks, base, base + n, lane, s_tk[warp][RANGES ? 2 : 0]);
+        }
         __syncwarp();
         const uint32_t *tbnd = reinterpret_cast<const uint32_t *>(s_tk[warp][0]) + hb;
         const uint32_t *tiv = reinterpret_cast<const uint32_t *>(s_tk[warp][1]) + hi;
+        const uint32_t *trg = reinterpret_cast<const uint32_t *>(s_tk[warp][RANGES ? 2 : 0]) + hr;
         for (uint32_t i = lane; i < n; i += 32u) {
             const uint32_t slot = base + i, e = map_off + slot;
             const bool full = fresh[e] != 0;
             const bool nb = C.bnd && tick_is_newer(tbnd[i], last_run, this_run);
             const bool ni = C.iv && tick_is_newer(tiv[i], last_run, this_run);
-            if (!full && !nb && !ni) continue;
+            const bool nr = RANGES && G.ranges && tick_is_newer(trg[i], last_run, this_run);
+            if (!full && !nb && !ni && !nr) continue;
             if (full) fresh[e] = 0;
             const uint32_t row = tb.map[e];
             if (row == kNoParent) continue;
@@ -3255,6 +3267,11 @@ k_read_table_cull(Rows R, TableBufs tb, const DevTableCull *__restrict__ cull, u
                 const uint32_t iv = C.iv && C.iv[slot] ? (uint32_t)F_INHERITED : 0u;
                 const uint32_t f = R.flags[row];
                 R.flags[row] = (uint8_t)(full ? (C.flags | iv | (f & F_TCHANGED)) : ((f & ~(uint32_t)F_INHERITED) | iv));
+            }
+            if (RANGES && G.ranges && (full || nr)) {         // what k_unpack_range_params stores
+                const uint8_t *p = G.ranges + (size_t)slot * rr.stride;
+                rr.se[row] = make_float2(*reinterpret_cast<const float *>(p + rr.start), *reinterpret_cast<const float *>(p + rr.end));
+                rr.ua[row] = p[rr.use_aabb] != 0 ? 1u : 0u;
             }
         }
         __syncwarp();                                         // the slab is the warp's next chunk's
@@ -4343,10 +4360,12 @@ void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uin
     ++g_launches; k_read_tables<<<grid, 256, 0, st>>>(R, tb, which, last_run, this_run);
 }
 void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
-                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster) {
+                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster, const RangeRead &rr) {
     if (!tb.n_chunks) return;
     const unsigned grid = tb.n_chunks < 8u * 1184u ? cdiv(tb.n_chunks, 8) : 1184u;
-    ++g_launches; k_read_table_cull<<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run, tab_caster, caster);
+    ++g_launches;
+    if (rr.tables) k_read_table_cull<true><<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run, tab_caster, caster, rr);
+    else k_read_table_cull<false><<<grid, 256, 0, st>>>(R, tb, cull, fresh, last_run, this_run, tab_caster, caster, rr);
 }
 void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick) {
     if (!tb.n_chunks) return;

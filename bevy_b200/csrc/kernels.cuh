@@ -53,9 +53,10 @@ void launch_writeback_tables(cudaStream_t st, const Rows &R, const TableBufs &tb
 // b200vis_read_tables: which = B200VIS_RD_* bits, slots newer by Tick::is_newer_than(last_run, this_run)
 void launch_read_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t which, uint32_t last_run, uint32_t this_run);
 // b200vis_read_tables with RD_CULL_INPUTS: cull[t] = table t's cull inputs, fresh[entry] = read the slot in full (cleared);
-// tab_caster[t] (nullptr = no table casters attached) = the caster byte a full read gives the slot's row
+// tab_caster[t] (nullptr = no table casters attached) = the caster byte a full read gives the slot's row;
+// rr.tables (nullptr = no VisibilityRange columns attached) = the range columns a full read or a newer tick reads
 void launch_read_table_cull(cudaStream_t st, const Rows &R, const TableBufs &tb, const DevTableCull *cull, uint8_t *fresh,
-                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster);
+                            uint32_t last_run, uint32_t this_run, const uint8_t *tab_caster, uint8_t *caster, const RangeRead &rr);
 // b200vis_writeback_tables with WB_SET_VISIBLE: set_visible() over the bytes the table slots hold, vv_shadow marked unknown
 void launch_set_visible_tables(cudaStream_t st, const Rows &R, const TableBufs &tb, uint32_t vv_tick);
 // b200vis_set_visible_entities_sink: counts = [max_views][chunks_stride][8] scratch, chunks_stride >= visible_entity_chunks(n_rows)

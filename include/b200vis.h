@@ -593,7 +593,9 @@ B200VIS_API int32_t b200vis_read_tables(b200vis_ctx *ctx, uint32_t which, uint32
  * of their fields).  Every field is f32: center and half_extents are lanes 0-2 of a Vec3A, radius one float.
  * The other inputs of check_visibility_cpu_culling (Has<NoFrustumCulling>, Has<VisibilityRange>, Without<NoCpuCulling>, a
  * point light's Sphere rebuilt from its GlobalTransform) are fixed for an archetype, so they are given once per table in
- * `flags`.  VisibilityClass, RenderLayers and the VisibleEntityRanges mask are not read: b200vis_upload_bounds carries them. */
+ * `flags`.  VisibilityClass and RenderLayers are not read: b200vis_upload_bounds carries them.  The VisibilityRange
+ * parameters come from the tables through b200vis_set_table_visibility_ranges, or as rows through
+ * b200vis_upload_visibility_ranges; without either, b200vis_upload_bounds carries the VisibleEntityRanges mask. */
 typedef struct b200vis_bounds_layout {
     uint32_t aabb_stride, aabb_center, aabb_half_extents;   /* bytes; each field is 3 floats */
     uint32_t sphere_stride, sphere_center, sphere_radius;   /* center 3 floats, radius 1 float */
@@ -633,9 +635,11 @@ typedef struct b200vis_table_cull_inputs {
  * b200vis_compact_topology; b200vis_set_topology unmaps every slot, so the rows mapped again are read in full.
  * Errors: INVALID_ARG (n_tables differs from the registry's size, only one pointer of a column pair NULL, a pointer not
  * 4-byte aligned, a layout field not 4-byte aligned, overlapping or past its stride, no layout while some table has aabbs
- * or spheres, flags other than the four per-archetype bits), NOT_READY (no tables registered), UNSUPPORTED
+ * or spheres, flags other than the four per-archetype bits, a table whose B200VIS_F_HAS_VIS_RANGE differs from whether
+ * it has an attached VisibilityRange column, see b200vis_set_table_visibility_ranges), NOT_READY (no tables registered), UNSUPPORTED
  * (world_size > 1); nothing changes then.  On B200VIS_ERR_CUDA the registry is left empty when cudaHostRegister refused
- * the memory, and otherwise every cull input is detached (the next call reads every table it attaches in full). */
+ * the memory, and otherwise every cull input and the VisibilityRange attachment are detached (the next calls read every
+ * table they attach in full). */
 B200VIS_API int32_t b200vis_set_table_cull_inputs(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_cull_inputs *inputs,
                                                   const b200vis_bounds_layout *layout);
 
@@ -760,6 +764,46 @@ B200VIS_API int32_t b200vis_upload_visibility_ranges(b200vis_ctx *ctx, uint32_t 
                                                      const uint8_t *use_aabb);
 B200VIS_API int32_t b200vis_set_visibility_range_views(b200vis_ctx *ctx, uint32_t n_views, const float *positions /* [n][3] */);
 B200VIS_API int32_t b200vis_download_visibility_ranges(b200vis_ctx *ctx, uint32_t first_row, uint32_t count, uint32_t *mask);
+/*     The same VisibilityRange columns straight from the archetype tables.  VisibilityRange (range.rs:80-112) is
+ *     repr(Rust): its layout is passed in (size_of, and offset_of! of start_margin.start, end_margin.end and use_aabb).
+ *     ranges[t] belongs to table t of the current registry: n_tables must equal its size.  Like
+ *     b200vis_upload_visibility_ranges, the first attach allocates the resident range columns, after which
+ *     b200vis_set_visibility_range_views works and the cull phase evaluates the masks itself.  The columns are
+ *     registered, kept and released by the code of b200vis_set_tables_ex, and the page rules above apply to them.
+ *     b200vis_set_tables / _ex drop the attachment; NULL, 0 detaches.
+ *     While attached, b200vis_read_tables(B200VIS_RD_CULL_INPUTS, ..) also writes a row's range parameters:
+ *       (start_margin.start, end_margin.end) and use_aabb != 0, on every full read of its slot
+ *       (b200vis_set_table_cull_inputs says which), and where the slot's range tick is newer by the Tick::is_newer_than
+ *       rule of b200vis_read_tables.  A table whose entry (its pointers, or the layout) differs from the previous attach
+ *       is read in full at the next such read: a reallocated table, a table newly given ranges, and every table on an
+ *       attach after a detach or before any attach.  b200vis_set_tables / _ex drop the attachment but, as for the
+ *       cull inputs, a table whose registry entry did not change keeps its entry for that comparison (and its columns
+ *       stay registered), so attaching it again unchanged reads nothing in full -- unless an RD_CULL_INPUTS read ran
+ *       in between: that read may have read slots in full without their range parameters, so the kept entries are
+ *       dropped and the next attach reads every ranged table in full.
+ *     Rule: no row is range-tested with parameters nobody supplied.  B200VIS_F_HAS_VIS_RANGE stays a per-archetype bit of
+ *     the cull inputs' flags, so while ranges are attached a table has a range column exactly when its attached cull
+ *     inputs carry B200VIS_F_HAS_VIS_RANGE (a table without cull inputs has none).  An attach that breaks this, and a
+ *     b200vis_set_table_cull_inputs that would break it while ranges are attached, fail with INVALID_ARG; to change which
+ *     tables are ranged, detach the ranges first.  Rows in no table keep what b200vis_upload_visibility_ranges gave them.
+ *     Errors: INVALID_ARG (n_tables differs from the registry's size, the rule above, only one pointer of a pair NULL, a
+ *     pointer not 4-byte aligned, a float field or the stride not 4-byte aligned, a field past the stride, fields
+ *     overlapping each other or the use_aabb byte, no layout while some table has ranges), NOT_READY (no tables
+ *     registered), UNSUPPORTED (world_size > 1); nothing changes then.  On B200VIS_ERR_CUDA the registry is left empty
+ *     when cudaHostRegister refused the memory, and otherwise both the ranges and the cull inputs are detached (the
+ *     registrations may have moved under either; the next calls read every table they attach in full). */
+typedef struct b200vis_visibility_range_layout {
+    uint32_t stride;    /* size_of::<VisibilityRange>() */
+    uint32_t start;     /* offset_of!(VisibilityRange, start_margin.start), f32 */
+    uint32_t end;       /* offset_of!(VisibilityRange, end_margin.end), f32 */
+    uint32_t use_aabb;  /* offset_of!(VisibilityRange, use_aabb), bool (1 byte, nonzero = true) */
+} b200vis_visibility_range_layout;
+typedef struct b200vis_table_visibility_ranges {
+    const void     *ranges;         /* [capacity] VisibilityRange; NULL = the archetype has none */
+    const uint32_t *changed_ticks;  /* [capacity]; NULL exactly when ranges is */
+} b200vis_table_visibility_ranges;
+B200VIS_API int32_t b200vis_set_table_visibility_ranges(b200vis_ctx *ctx, uint32_t n_tables, const b200vis_table_visibility_ranges *ranges,
+                                                        const b200vis_visibility_range_layout *layout);
 /* (b) visibility_propagate_system (crates/bevy_camera/src/visibility/mod.rs:638-729).  visibility[count]: 0 Inherited,
  *     1 Hidden, 2 Visible (the enum's order, :83-96), | 4 when the entity lacks Visibility / InheritedVisibility.
  *     b200vis_propagate_visibility walks the same level-ordered tiles as the transform propagation and leaves every

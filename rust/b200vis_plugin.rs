@@ -16,16 +16,18 @@
 //! With a three-line patch that makes those two systems removable, the device's ViewVisibility bytes + change ticks are
 //! written into the tables instead (`forked-bevy` feature below).
 //!
-//! Data flow (INTEGRATION.md section 2): Transform, other systems' GlobalTransforms, and the cull inputs Aabb, Sphere and
-//! InheritedVisibility read by the device straight from the archetype tables by their change ticks
-//! (`b200vis_set_tables_ex`, `b200vis_set_table_cull_inputs`, `b200vis_read_tables`); VisibilityClass, RenderLayers and
-//! the VisibleEntityRanges masks -> `upload_bounds` on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
+//! Data flow (INTEGRATION.md section 2): Transform, other systems' GlobalTransforms, and the cull inputs Aabb, Sphere,
+//! InheritedVisibility and VisibilityRange read by the device straight from the archetype tables by their change ticks
+//! (`b200vis_set_tables_ex`, `b200vis_set_table_cull_inputs`, `b200vis_set_table_visibility_ranges`,
+//! `b200vis_read_tables`), the range masks evaluated on the device; VisibilityClass and RenderLayers -> `upload_bounds`
+//! on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
 //! and VisibleEntities as per-class Entity lists through `b200vis_set_visible_entities_sink`), read after one
 //! `b200vis_synchronize` per system; GlobalTransform and ViewVisibility with their change ticks straight into the archetype
 //! tables (`b200vis_writeback_tables`).
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
 use bevy::camera::primitives::{Aabb, Frustum, Sphere};
 use bevy::camera::visibility::*;
+use bevy::camera::ShadowLodOrigin;
 use bevy::ecs::component::Tick;
 use bevy::ecs::entity::EntityHashMap;
 use bevy::ecs::schedule::ScheduleCleanupPolicy::RemoveSystemsOnly;
@@ -68,6 +70,9 @@ pub struct b200vis_table_inputs { transforms: *const Transform, transform_change
 #[repr(C)] #[derive(Clone, Copy, PartialEq)]
 pub struct b200vis_table_cull_inputs { aabbs: *const Aabb, aabb_changed_ticks: *const Tick, spheres: *const Sphere,
     sphere_changed_ticks: *const Tick, inherited_visibility: *const InheritedVisibility, iv_changed_ticks: *const Tick, flags: u32 }
+#[repr(C)] pub struct b200vis_visibility_range_layout { stride: u32, start: u32, end: u32, use_aabb: u32 }
+#[repr(C)] #[derive(Clone, Copy, PartialEq)]
+pub struct b200vis_table_visibility_ranges { ranges: *const VisibilityRange, changed_ticks: *const Tick }
 
 #[link(name = "b200vis")]
 extern "C" {
@@ -100,6 +105,9 @@ extern "C" {
     fn b200vis_read_tables(ctx: *mut b200vis_ctx, which: u32, last_run: u32, this_run: u32) -> i32;
     fn b200vis_set_table_cull_inputs(ctx: *mut b200vis_ctx, n: u32, inputs: *const b200vis_table_cull_inputs,
                                      layout: *const b200vis_bounds_layout) -> i32;
+    fn b200vis_set_table_visibility_ranges(ctx: *mut b200vis_ctx, n: u32, ranges: *const b200vis_table_visibility_ranges,
+                                           layout: *const b200vis_visibility_range_layout) -> i32;
+    fn b200vis_set_visibility_range_views(ctx: *mut b200vis_ctx, n: u32, positions: *const f32) -> i32;
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
@@ -139,6 +147,8 @@ pub struct B200Vis {
     // was built from, and the rows epoch of the maps
     tables: Vec<b200vis_table>, table_inputs: Vec<b200vis_table_inputs>, table_cull: Vec<b200vis_table_cull_inputs>,
     table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
+    // the tables' VisibilityRange columns, attached while the VisibleEntityRanges resource exists (None = detached)
+    table_ranges: Option<Vec<b200vis_table_visibility_ranges>>,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -184,7 +194,7 @@ impl Plugin for B200VisibilityPlugin {
             entity_offsets: vec![[0; 9]; max_views],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
             planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_cull: Vec::new(), table_entities: Vec::new(),
-            maps_epoch: u64::MAX,
+            maps_epoch: u64::MAX, table_ranges: None,
         };
         // the sorted row lists stay on the device: VisibleEntities arrives as Entity values through the entities sink, and
         // GlobalTransform and ViewVisibility go straight into the archetype tables (b200vis_set_tables)
@@ -210,6 +220,9 @@ impl Plugin for B200VisibilityPlugin {
             app.add_systems(schedule, (b200_sync_tables, b200_propagate).chain().in_set(TransformSystems::Propagate));
         }
         app.remove_systems_in_set(PostUpdate, check_visibility_cpu_culling, RemoveSystemsOnly);
+        // check_visibility_ranges stays: the device evaluates the ranges the cull uses from the tables' VisibilityRange
+        // columns, but the CPU light-visibility systems, which this plugin does not replace yet, read VisibleEntityRanges
+        // (DESIGN.md section 9 item 0).
         app.remove_systems_in_set(PostUpdate, SimulationLightSystems::AssignLightsToClusters, RemoveSystemsOnly);
         app.add_systems(PostUpdate, (
             (b200_sync_tables, b200_check_visibility).chain().in_set(VisibilitySystems::CheckVisibility),
@@ -316,9 +329,17 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     let markers = [(world.component_id::<NoFrustumCulling>(), F_NO_FRUSTUM), (world.component_id::<VisibilityRange>(), F_RANGE),
                    (world.component_id::<NoCpuCulling>(), F_NO_CPU_CULLING)];
     let light_id = world.component_id::<PointLight>();
+    // VisibilityRange is repr(Rust) too.  Without the VisibleEntityRanges resource the reference does not range-cull at
+    // all (visibility/mod.rs:813-819), so nothing is attached then.
+    let range_layout = b200vis_visibility_range_layout { stride: size_of::<VisibilityRange>() as u32,
+        start: (offset_of!(VisibilityRange, start_margin) + offset_of!(core::ops::Range<f32>, start)) as u32,
+        end: (offset_of!(VisibilityRange, end_margin) + offset_of!(core::ops::Range<f32>, end)) as u32,
+        use_aabb: offset_of!(VisibilityRange, use_aabb) as u32 };
+    let range_id = world.component_id::<VisibilityRange>();
+    let use_ranges = world.contains_resource::<VisibleEntityRanges>();
     world.resource_scope(|world, mut vis: Mut<B200Vis>| {
         let vis = &mut *vis;
-        let (mut descs, mut inputs, mut culls, mut entities) = (Vec::new(), Vec::new(), Vec::new(), Vec::new());
+        let (mut descs, mut inputs, mut culls, mut entities, mut ranges) = (Vec::new(), Vec::new(), Vec::new(), Vec::new(), Vec::new());
         for table in world.storages().tables.iter() {
             if !table.has_column(gt_id) { continue; }
             // SAFETY: the columns hold GlobalTransform / ViewVisibility.  Only raw pointers are kept; the GPU writes through
@@ -354,6 +375,9 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             if has(light_id) && aabb.is_null() && !sphere.is_null() { flags |= F_SPHERE_FROM_GT; }
             culls.push(b200vis_table_cull_inputs { aabbs: aabb, aabb_changed_ticks: aabb_t, spheres: sphere, sphere_changed_ticks: sphere_t,
                                                    inherited_visibility: iv, iv_changed_ticks: iv_t, flags: flags as u32 });
+            // the VisibilityRange column goes with the table's F_RANGE bit, as the library requires
+            let (range, range_t) = column::<VisibilityRange>(table, range_id);
+            ranges.push(b200vis_table_visibility_ranges { ranges: range, changed_ticks: range_t });
             entities.push(table.entities());
         }
         let registry_changed = descs != vis.tables || inputs != vis.table_inputs;
@@ -361,11 +385,26 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             vis.check(unsafe { b200vis_set_tables_ex(vis.ctx, descs.len() as u32, descs.as_ptr(), inputs.as_ptr(), &layout) })?;
             vis.tables = descs;
             vis.table_inputs = inputs;
+            vis.table_ranges = None;                // ... and drops the cull inputs and the ranges
         }
         // b200vis_set_tables_ex drops the cull inputs: attach them again (a table whose entry is unchanged is not read in full)
         if registry_changed || culls != vis.table_cull {
+            // the ranges leave first: the cull inputs may change which tables carry F_RANGE
+            if vis.table_ranges.take().is_some() {
+                vis.check(unsafe { b200vis_set_table_visibility_ranges(vis.ctx, 0, core::ptr::null(), core::ptr::null()) })?;
+            }
             vis.check(unsafe { b200vis_set_table_cull_inputs(vis.ctx, culls.len() as u32, culls.as_ptr(), &bounds_layout) })?;
             vis.table_cull = culls;
+        }
+        // the VisibilityRange columns the cull read takes the range parameters from (an attach after none reads every
+        // ranged table in full)
+        let want = if use_ranges && !vis.tables.is_empty() { Some(ranges) } else { None };
+        if want != vis.table_ranges {
+            match &want {
+                Some(r) => vis.check(unsafe { b200vis_set_table_visibility_ranges(vis.ctx, r.len() as u32, r.as_ptr(), &range_layout) })?,
+                None => vis.check(unsafe { b200vis_set_table_visibility_ranges(vis.ctx, 0, core::ptr::null(), core::ptr::null()) })?,
+            }
+            vis.table_ranges = want;
         }
         let renumbered = vis.maps_epoch != vis.columns_epoch;
         let stale: Vec<bool> = entities.iter().enumerate()
@@ -408,11 +447,23 @@ fn b200_check_visibility(
     visible_aabb_query: Query<(Entity, Ref<InheritedVisibility>, &mut ViewVisibility, Option<Ref<VisibilityClass>>, Option<Ref<RenderLayers>>,
                                    Option<Ref<Aabb>>, Option<Ref<Sphere>>, &GlobalTransform, Has<NoFrustumCulling>, Has<VisibilityRange>,
                                    Has<PointLight>), Without<NoCpuCulling>>,
-    visible_entity_ranges: Option<Res<VisibleEntityRanges>>,
-    dirty_query: Query<Entity, (Without<NoCpuCulling>, Or<(Changed<VisibilityClass>, Changed<RenderLayers>, With<VisibilityRange>)>)>,
+    // check_visibility_ranges' view query and its cap of 32 (visibility/range.rs:236, 247)
+    range_views: Query<(Entity, &GlobalTransform), Or<(With<Camera>, With<ShadowLodOrigin>)>>,
+    dirty_query: Query<Entity, (Without<NoCpuCulling>, Or<(Changed<VisibilityClass>, Changed<RenderLayers>)>)>,
     mut removed_layers: RemovedComponents<RenderLayers>,
 ) -> Result<(), BevyError> {
     let vis = &mut *vis;
+    // ---- the VisibilityRange views: the device evaluates check_visibility_ranges itself, from the tables' range columns
+    // b200_sync_tables attached (only while the VisibleEntityRanges resource exists) and this frame's GlobalTransforms ----
+    let ranged = vis.table_ranges.is_some();
+    let (mut range_entities, mut range_pos) = (Vec::new(), Vec::new());
+    if ranged {
+        for (e, g) in range_views.iter().take(32) {
+            let t = g.translation();
+            range_entities.push(e); range_pos.extend_from_slice(&[t.x, t.y, t.z]);
+        }
+        vis.check(unsafe { b200vis_set_visibility_range_views(vis.ctx, range_entities.len() as u32, range_pos.as_ptr()) })?;
+    }
     // ---- views: half spaces copied verbatim from `Frustum` (bit-identical by construction) ----
     let mut views = Vec::new();
     vis.view_entities.clear();
@@ -421,15 +472,15 @@ fn b200_check_visibility(
                                    flags: (camera.is_active as u8 * VIEW_ACTIVE) | (no_cpu_culling as u8 * VIEW_NO_CPU_CULLING),
                                    range_view_index: -1, pad: [0; 6] };
         for (k, hs) in frustum.half_spaces.iter().enumerate() { v.half_spaces[k] = hs.normal_d().to_array(); }
-        // VisibleEntityRanges keeps its view -> bit table private; the shim builds its own masks below with bit v = device view v
-        if visible_entity_ranges.is_some() { v.range_view_index = views.len() as i8; }
+        // the view's bit in the device's range masks; -1 = not among the range views: entity_is_in_range_of_view is
+        // then false for every entity with a VisibilityRange (range.rs:218-220), so the view culls them all
+        if ranged { v.range_view_index = range_entities.iter().position(|r| *r == entity).map_or(-1, |i| i as i8); }
         views.push(v); vis.view_entities.push(entity);
         if views.len() == vis.max_views { break; }
     }
     vis.check(unsafe { b200vis_set_views(vis.ctx, views.len() as u32, views.as_ptr()) })?;
-    // ---- VisibilityClass, RenderLayers and the VisibleEntityRanges masks (which the device cannot read from the tables):
-    // every row after a renumbering, otherwise only the rows whose class or layers changed and the rows with a
-    // VisibilityRange (VisibleEntityRanges is rebuilt by check_visibility_ranges every frame), as contiguous ranges.
+    // ---- VisibilityClass and RenderLayers (which the device cannot read from the tables): every row after a renumbering,
+    // otherwise only the rows whose class or layers changed, as contiguous ranges.
     // upload_bounds also takes the rows' current bounds and flags; the table read below, enqueued after it, then brings
     // every row's Aabb / Sphere / InheritedVisibility up to date by their change ticks.  No loop over every entity. ----
     let all = vis.bounds_epoch != vis.columns_epoch;
@@ -440,7 +491,7 @@ fn b200_check_visibility(
     dirty.sort_unstable();
     dirty.dedup();
     let k = dirty.len();
-    let (mut bounds, mut flags, mut class, mut layer, mut range) = (vec![0f32; k * 6], vec![F_NO_CPU_CULLING; k], vec![0u8; k], vec![1u64; k], vec![0u32; k]);
+    let (mut bounds, mut flags, mut class, mut layer) = (vec![0f32; k * 6], vec![F_NO_CPU_CULLING; k], vec![0u8; k], vec![1u64; k]);
     for (i, &r) in dirty.iter().enumerate() {
         let e = vis.entity_of[r as usize];
         // a row outside visible_aabb_query stays NO_CPU_CULLING, as its table's cull inputs say
@@ -454,21 +505,18 @@ fn b200_check_visibility(
         flags[i] = f;
         class[i] = vclass.as_ref().map_or(0, |c| c.iter().fold(0u8, |m, id| m | vis.class_bit(*id)));
         layer[i] = layers.as_ref().map_or(1, |l| l.bits()[0]);
-        range[i] = match (&visible_entity_ranges, has_range) {       // entity_is_in_range_of_view (visibility/range.rs:214-222)
-            (Some(vr), true) => vis.view_entities.iter().enumerate().fold(0u32, |m, (v, view)| m | ((vr.entity_is_in_range_of_view(e, *view) as u32) << v)),
-            _ => 0,
-        };
     }
     let mut i = 0;
     while i < k {                                               // coalesce into [first, first + count) ranges
         let mut j = i + 1;
         while j < k && dirty[j] == dirty[j - 1] + 1 { j += 1; }
         vis.check(unsafe { b200vis_upload_bounds(vis.ctx, dirty[i], (j - i) as u32, bounds[i * 6..].as_ptr(), flags[i..].as_ptr(),
-            class[i..].as_ptr(), layer[i..].as_ptr(), if visible_entity_ranges.is_some() { range[i..].as_ptr() } else { core::ptr::null() }) })?;
+            class[i..].as_ptr(), layer[i..].as_ptr(), core::ptr::null()) })?;
         i = j;
     }
-    // Aabb, Sphere and InheritedVisibility straight from the tables, by this system's own change ticks; rows (re)mapped
-    // since the last read (archetype moves, a renumbering) are read in full, their per-archetype flags with them
+    // Aabb, Sphere, InheritedVisibility and VisibilityRange straight from the tables, by this system's own change ticks;
+    // rows (re)mapped since the last read (archetype moves, a renumbering) are read in full, their per-archetype flags
+    // with them
     if !vis.tables.is_empty() {
         vis.check(unsafe { b200vis_read_tables(vis.ctx, RD_CULL_INPUTS, this_run.last_run().get(), this_run.this_run().get()) })?;
     }
