@@ -352,6 +352,14 @@ class ShadowEntitiesSink(C.Structure):
                 ("active", C.c_void_p)]
 
 
+class ShadowDiffSink(C.Structure):
+    _fields_ = [("added", C.c_void_p), ("added_capacity", C.c_uint32), ("removed", C.c_void_p), ("removed_capacity", C.c_uint32),
+                ("added_offsets", C.c_void_p), ("removed_offsets", C.c_void_p), ("max_items", C.c_uint32), ("max_slots", C.c_uint32)]
+
+
+SHADOW_NO_SLOT = 0xFFFFFFFF
+
+
 class ResultSink(C.Structure):
     _fields_ = [("stats", C.POINTER(FrameStats)), ("visible_rows", C.c_void_p), ("visible_capacity", C.c_uint32),
                 ("visible_classes", C.c_void_p), ("cluster_offsets", C.c_void_p), ("cluster_indices", C.c_void_p), ("cluster_capacity", C.c_uint32)]
@@ -433,6 +441,8 @@ _SIGNATURES = {
     "b200vis_run_shadow_culling": (C.c_int32, [_vp]),
     "b200vis_download_shadow_visible": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
     "b200vis_set_shadow_entities_sink": (C.c_int32, [_vp, _P(ShadowEntitiesSink)]),
+    "b200vis_set_shadow_diff_sink": (C.c_int32, [_vp, _P(ShadowDiffSink)]),
+    "b200vis_set_shadow_items_ex": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _vp]),
     "b200vis_host_point_light_frusta": (None, [_vp, C.c_float, C.c_float, _vp]),
     "b200vis_upload_visibility_ranges": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "b200vis_set_visibility_range_views": (C.c_int32, [_vp, C.c_uint32, _vp]),
@@ -899,8 +909,10 @@ class Context:
         self._check(self._lib.b200vis_set_shadow_lights(self._h, len(o), _ptr(o), _ptr(fr), None if lm is None else _ptr(lm),
                                                         int(lod_origin_range_index), int(list_capacity)))
 
-    def set_shadow_items(self, items, list_capacity=0):
-        """items: list of dicts(kind, light_row, range, range_view_index, layer_mask, frusta [6,6,4] or [6,4])."""
+    def set_shadow_items(self, items, list_capacity=0, diff_slots=None):
+        """items: list of dicts(kind, light_row, range, range_view_index, layer_mask, frusta [6,6,4] or [6,4]).
+        diff_slots: one diff slot per item (SHADOW_NO_SLOT = none) for the shadow diff sink (b200vis_set_shadow_items_ex);
+        None is b200vis_set_shadow_items."""
         arr = (ShadowItem * max(len(items), 1))()
         for i, it in enumerate(items):
             arr[i].kind = it["kind"]; arr[i].light_row = it.get("light_row", 0); arr[i].range = it.get("range", 0.0)
@@ -912,7 +924,13 @@ class Context:
             else:
                 fr[:] = f
             arr[i].frusta[:] = fr.reshape(-1).tolist()
-        self._check(self._lib.b200vis_set_shadow_items(self._h, len(items), arr, list_capacity))
+        if diff_slots is None:
+            self._check(self._lib.b200vis_set_shadow_items(self._h, len(items), arr, list_capacity))
+            return
+        sl = np.ascontiguousarray(diff_slots, np.uint32)
+        if len(sl) < len(items):                             # the library reads diff_slots[n_items]
+            raise ValueError(f"set_shadow_items: {len(sl)} diff slots for {len(items)} items")
+        self._check(self._lib.b200vis_set_shadow_items_ex(self._h, len(items), arr, list_capacity, _ptr(sl)))
 
     def run_shadow_culling(self):
         self._check(self._lib.b200vis_run_shadow_culling(self._h))
@@ -942,6 +960,30 @@ class Context:
         s = ShadowEntitiesSink(ptr(entities), cap, mi, ptr(offsets), ptr(active))
         self._check(self._lib.b200vis_set_shadow_entities_sink(self._h, C.byref(s)))
         self._shadow_sink = (entities, offsets, active)
+
+    def set_shadow_diff_sink(self, added, removed, added_offsets, removed_offsets, max_slots=0, added_capacity=None,
+                             removed_capacity=None, max_items=None):
+        """b200vis_set_shadow_diff_sink: pinned (or registrable) host numpy arrays added / removed [capacity] uint64
+        (Entity::to_bits() of every list's added / removed entries, back to back) and added_offsets / removed_offsets
+        [max_items * 6 + 1] uint32 (list item * 6 + face is added[added_offsets[l]:added_offsets[l + 1]]); max_slots diff
+        slots.  The capacities and max_items default to the arrays' sizes and override the counts passed (argument tests).
+        All None removes the sink."""
+        if added is None and removed is None and added_offsets is None and removed_offsets is None:
+            self._check(self._lib.b200vis_set_shadow_diff_sink(self._h, None))
+            self._shadow_diff_sink = None
+            return
+        ptr = lambda a: None if a is None else a.ctypes.data
+        size = lambda a: 0 if a is None else a.size
+        ac = size(added) if added_capacity is None else added_capacity
+        rc = size(removed) if removed_capacity is None else removed_capacity
+        mi = (max(size(added_offsets) - 1, 0) // 6) if max_items is None else max_items
+        if added is not None and ac > added.size or removed is not None and rc > removed.size or \
+                added_offsets is not None and mi * 6 + 1 > added_offsets.size or \
+                removed_offsets is not None and mi * 6 + 1 > removed_offsets.size:
+            raise ValueError("set_shadow_diff_sink: the arrays are smaller than the capacities / max_items say")
+        s = ShadowDiffSink(ptr(added), ac, ptr(removed), rc, ptr(added_offsets), ptr(removed_offsets), mi, max_slots)
+        self._check(self._lib.b200vis_set_shadow_diff_sink(self._h, C.byref(s)))
+        self._shadow_diff_sink = (added, removed, added_offsets, removed_offsets)
 
     # ---- SURVEY 8(f) N4 ----
     def upload_visibility_ranges(self, first, start_end, use_aabb):

@@ -166,6 +166,10 @@ struct b200vis_ctx {
     uint32_t *d_ent_counts = nullptr; uint32_t ent_chunks = 0;
     // b200vis_set_shadow_entities_sink: device aliases (entities == nullptr: none), its max_items, and the device offsets
     ShadowSink shsink{}; uint32_t shsink_max_items = 0; uint32_t *d_shadow_off = nullptr; size_t shadow_off_cap = 0;
+    // b200vis_set_shadow_diff_sink: the device state (added == nullptr: none) and the host's side of it: max_items / max_slots,
+    // the installed items' slots, and which slots may hold entries (the ones a run named since they were last emptied)
+    ShadowDiff sdiff{}; uint32_t sdiff_max_items = 0, sdiff_max_slots = 0;
+    std::vector<uint32_t> h_sdiff_slot; std::vector<uint8_t> sdiff_held;
 
     b200vis_column_sinks colsink{}; bool have_colsink = false;          // b200vis_set_column_sinks (device aliases below)
     float *col_gt_d = nullptr; uint32_t *col_gt_bits_d = nullptr, *col_vv_bits_d = nullptr; uint8_t *col_vv_d = nullptr;
@@ -261,7 +265,8 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->shadow.count, ctx->shadow.active, ctx->d_keys, ctx->d_keys2, ctx->d_rank2, ctx->d_row_of_rank2,
                    ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
                    ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster,
-                   ctx->d_tab_range};
+                   ctx->d_tab_range, const_cast<uint32_t *>(ctx->sdiff.slot), ctx->sdiff.prev, ctx->sdiff.prev_count,
+                   ctx->sdiff.words, ctx->sdiff.chunk, ctx->sdiff.dev_offsets};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -1035,6 +1040,11 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
     CU(cudaMemset(ctx->d_stats, 0, sizeof(DevStats)));
     CU(cudaMemset(ctx->d_slab, 0, ctx->slab_bytes));
     if (ctx->diff.prev) CU(cudaMemset(ctx->diff.prev, 0, (size_t)ctx->vis.words_stride * ctx->cfg.max_views * 4));   // ranks changed: old list = empty
+    if (ctx->sdiff.added) {                      // ... and every shadow diff slot: the next run reports every list as added
+        CU(cudaMemset(ctx->sdiff.prev, 0, (size_t)ctx->sdiff_max_slots * 6 * ctx->vis.words_stride * 4));
+        CU(cudaMemset(ctx->sdiff.prev_count, 0, (size_t)ctx->sdiff_max_slots * 6 * ctx->vis.chunks_stride * 4));
+        std::fill(ctx->sdiff_held.begin(), ctx->sdiff_held.end(), 0);
+    }
     ctx->topology_set = true;
     ctx->gt_aos_valid = false;
     {   // what b200vis_edit_topology starts from: the plan, and the keys in rank order (uploaded by the first merge)
@@ -1046,7 +1056,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         ctx->keys_resident = false;
         ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
     }
-    if (ctx->ent_sink_d || ctx->shsink.entities) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sinks read them
+    if (ctx->ent_sink_d || ctx->shsink.entities || ctx->sdiff.added) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sinks read them
     return tables_unmap_all(ctx);
 }
 
@@ -1090,6 +1100,26 @@ static int32_t alloc_rank_spares(b200vis_ctx *ctx, bool keys) {
     if (k) ctx->d_keys2 = k;
     if (r) ctx->d_rank2 = r;
     if (rr) ctx->d_row_of_rank2 = rr;
+    return B200VIS_OK;
+}
+
+// The shadow diff slots' sets (bit = rank) to new ranks: each slot that may hold entries, through the added / removed words
+// (free between runs; they hold at least 12 sets).  compacting: the set is cleared first, so words past the new end are
+// empty.  A remapped slot's per-chunk counts become "unknown" (non-zero), so that the next run reads every chunk of it.
+static int32_t remap_shadow_diff_slots(b200vis_ctx *ctx, bool compacting, uint32_t n_words, uint32_t n_rows, uint32_t n_old_rows,
+                                       const uint32_t *row_of_rank, const uint32_t *old_rank) {
+    if (!ctx->sdiff.added) return B200VIS_OK;
+    cudaStream_t st = ctx->stream;
+    const size_t ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
+    for (uint32_t s = 0; s < ctx->sdiff_max_slots; ++s) {
+        if (!ctx->sdiff_held[s]) continue;
+        uint32_t *set = ctx->sdiff.prev + (size_t)s * 6 * ws;
+        CU(cudaMemcpyAsync(ctx->sdiff.words, set, 6 * ws * 4, cudaMemcpyDeviceToDevice, st));
+        if (compacting) CU(cudaMemsetAsync(set, 0, 6 * ws * 4, st));
+        launch_remap_rank_sets(st, ctx->sdiff.words, set, (uint32_t)ws, 6, n_words, n_rows, n_old_rows, row_of_rank, old_rank);
+        CU(cudaGetLastError());
+        CU(cudaMemsetAsync(ctx->sdiff.prev_count + (size_t)s * 6 * cs, 0xFF, 6 * cs * 4, st));
+    }
     return B200VIS_OK;
 }
 
@@ -1226,6 +1256,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
                                    ctx->d_row_of_rank, old_rank);
             CU(cudaGetLastError());
         }
+        if ((rc = remap_shadow_diff_slots(ctx, false, (n2 + 31) / 32, n2, n, ctx->d_row_of_rank, old_rank))) return rc;
         ctx->rank_identity = false;
     } else if (n_spawn) {
         if (ctx->keys_resident) { if ((rc = put(ctx->d_keys + n, spawn_entity_bits, (size_t)n_spawn * 8))) return rc; CU(cudaEventRecord(ctx->ev_edit, st)); }
@@ -1278,6 +1309,11 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
         for (uint32_t i = 0; i < n_lists; ++i) launch_mark_listed_rows(st, lists[i], n, ctx->d_dirty, n);
         if (diff)   // last frame's visible sets: a row in them is reported removed by the next diff
             launch_mark_set_rows(st, ctx->diff.prev, ctx->vis.words_stride, V, (n + 31) / 32, ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->d_dirty);
+        if (ctx->sdiff.added)   // ... and the shadow diff slots' sets, likewise
+            for (uint32_t s = 0; s < ctx->sdiff_max_slots; ++s)
+                if (ctx->sdiff_held[s])
+                    launch_mark_set_rows(st, ctx->sdiff.prev + (size_t)s * 6 * ctx->vis.words_stride, ctx->vis.words_stride, 6, (n + 31) / 32,
+                                         ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->d_dirty);
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(ctx->h_stage, ctx->d_dirty, n, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
@@ -1399,6 +1435,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
         launch_remap_rank_sets(st, ctx->diff.words, ctx->diff.prev, ctx->vis.words_stride, V, (n2 + 31) / 32, n2, n, d_src, nullptr);
         CU(cudaGetLastError());
     }
+    if ((rc = remap_shadow_diff_slots(ctx, true, (n2 + 31) / 32, n2, n, d_src, nullptr))) return rc;
     // ---- the lists results hold, renumbered in place (survivors keep their rank order, so every list stays sorted) ----
     for (uint32_t i = 0; i < n_lists; ++i) launch_renumber_listed_rows(st, lists[i], n, d_o2n, n);
     if ((rc = flush_table_updates(ctx))) return rc;      // queued map updates carry the old row numbers
@@ -2583,7 +2620,8 @@ extern "C" int32_t b200vis_upload_shadow_casters(b200vis_ctx *ctx, uint32_t firs
     CU(cudaMemcpyAsync(ctx->d_caster + first, caster, count, cudaMemcpyHostToDevice, ctx->stream));
     return B200VIS_OK;
 }
-static int32_t install_shadow_items(b200vis_ctx *ctx, uint32_t n_items, uint32_t list_capacity) {
+// diff_slots: the items' diff slots (validated), nullptr = none
+static int32_t install_shadow_items(b200vis_ctx *ctx, uint32_t n_items, uint32_t list_capacity, const uint32_t *diff_slots) {
     if (!list_capacity) list_capacity = std::max<uint32_t>(ctx->cfg.max_entities, 1);
     if (!ctx->diff_on) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_items: the visible-set bookkeeping was switched off after upload_shadow_casters");
     CU(cudaStreamSynchronize(ctx->stream));
@@ -2603,6 +2641,19 @@ static int32_t install_shadow_items(b200vis_ctx *ctx, uint32_t n_items, uint32_t
     if (n_items) CU(cudaMemcpy(ctx->d_shadow_lights, ctx->h_shadow.data(), n_items * sizeof(ShadowLight), cudaMemcpyHostToDevice));
     ctx->shadow.n_lights = n_items; ctx->shadow.lights = ctx->d_shadow_lights; ctx->shadow.caster = ctx->d_caster;
     ctx->shadow.list_cap = ctx->shadow_cap_list;
+    if (ctx->sdiff.added) {
+        ctx->h_sdiff_slot.assign(n_items, kNoDiffSlot);
+        if (diff_slots) std::copy(diff_slots, diff_slots + n_items, ctx->h_sdiff_slot.begin());
+        if (n_items) CU(cudaMemcpy(const_cast<uint32_t *>(ctx->sdiff.slot), ctx->h_sdiff_slot.data(), (size_t)n_items * 4, cudaMemcpyHostToDevice));
+    }
+    return B200VIS_OK;
+}
+// the item counts a registered sink bounds (nothing is changed when one is exceeded)
+static int32_t check_shadow_sink_items(b200vis_ctx *ctx, uint32_t n_items, const char *who) {
+    if (ctx->shsink.entities && n_items > ctx->shsink_max_items)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "%s: %u items > the shadow entity sink's max_items %u", who, n_items, ctx->shsink_max_items);
+    if (ctx->sdiff.added && n_items > ctx->sdiff_max_items)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "%s: %u items > the shadow diff sink's max_items %u", who, n_items, ctx->sdiff_max_items);
     return B200VIS_OK;
 }
 extern "C" int32_t b200vis_set_shadow_lights(b200vis_ctx *ctx, uint32_t n_lights, const uint32_t *light_ordinals, const float *frusta,
@@ -2610,8 +2661,7 @@ extern "C" int32_t b200vis_set_shadow_lights(b200vis_ctx *ctx, uint32_t n_lights
     CHECK_CTX_JOIN();
     if (n_lights && (!light_ordinals || !frusta)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_lights: null");
     if (!ctx->d_caster) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_lights: upload the shadow-caster column first");
-    if (ctx->shsink.entities && n_lights > ctx->shsink_max_items)
-        return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_lights: %u items > the shadow entity sink's max_items %u", n_lights, ctx->shsink_max_items);
+    { const int32_t rc = check_shadow_sink_items(ctx, n_lights, "set_shadow_lights"); if (rc) return rc; }
     for (uint32_t i = 0; i < n_lights; ++i)
         if (light_ordinals[i] >= ctx->lights.n) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_lights: light ordinal %u >= %u lights", light_ordinals[i], ctx->lights.n);
     ctx->h_shadow.resize(n_lights);
@@ -2623,14 +2673,13 @@ extern "C" int32_t b200vis_set_shadow_lights(b200vis_ctx *ctx, uint32_t n_lights
         s.row = ctx->h_light_row[light_ordinals[i]]; s.range = ctx->h_light_range[light_ordinals[i]]; s.kind = 0;
         s.range_index = (lod_origin_range_index >= 0 && lod_origin_range_index < 32) ? lod_origin_range_index : -1;
     }
-    return install_shadow_items(ctx, n_lights, list_capacity);
+    return install_shadow_items(ctx, n_lights, list_capacity, nullptr);
 }
-extern "C" int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items, uint32_t list_capacity) {
-    CHECK_CTX_JOIN();
+static int32_t set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items, uint32_t list_capacity,
+                                const uint32_t *diff_slots) {
     if (n_items && !items) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items: null");
     if (!ctx->d_caster) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_items: upload the shadow-caster column first");
-    if (ctx->shsink.entities && n_items > ctx->shsink_max_items)
-        return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_items: %u items > the shadow entity sink's max_items %u", n_items, ctx->shsink_max_items);
+    { const int32_t rc = check_shadow_sink_items(ctx, n_items, "set_shadow_items"); if (rc) return rc; }
     ctx->h_shadow.resize(n_items);
     for (uint32_t i = 0; i < n_items; ++i) {
         const b200vis_shadow_item &it = items[i];
@@ -2643,15 +2692,55 @@ extern "C" int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, 
         s.layers = it.layer_mask; s.row = it.kind == B200VIS_SHADOW_DIRECTIONAL_CASCADE ? 0u : it.light_row; s.range = it.range;
         s.kind = it.kind; s.range_index = (it.range_view_index >= 0 && it.range_view_index < 32) ? it.range_view_index : -1;
     }
-    return install_shadow_items(ctx, n_items, list_capacity);
+    return install_shadow_items(ctx, n_items, list_capacity, diff_slots);
+}
+extern "C" int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items, uint32_t list_capacity) {
+    CHECK_CTX_JOIN();
+    return set_shadow_items(ctx, n_items, items, list_capacity, nullptr);
+}
+extern "C" int32_t b200vis_set_shadow_items_ex(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items, uint32_t list_capacity,
+                                               const uint32_t *diff_slots) {
+    CHECK_CTX_JOIN();
+    if (diff_slots) {
+        if (!ctx->sdiff.added) return fail(ctx, B200VIS_ERR_NOT_READY, "set_shadow_items_ex: diff slots without a shadow diff sink");
+        std::vector<uint8_t> seen(ctx->sdiff_max_slots, 0);
+        for (uint32_t i = 0; i < n_items; ++i) {
+            const uint32_t s = diff_slots[i];
+            if (s == B200VIS_SHADOW_NO_SLOT) continue;
+            if (s >= ctx->sdiff_max_slots)
+                return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items_ex: item %u: slot %u >= max_slots %u", i, s, ctx->sdiff_max_slots);
+            if (seen[s]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_items_ex: slot %u named twice", s);
+            seen[s] = 1;
+        }
+    }
+    return set_shadow_items(ctx, n_items, items, list_capacity, diff_slots);
 }
 extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     CHECK_CTX_JOIN();   // reads what the frame's CULL stage (incl. its tail on the side stream) left behind
     if (!ctx->d_caster || !ctx->diff.prev) return fail(ctx, B200VIS_ERR_NOT_READY, "run_shadow_culling: call b200vis_set_shadow_lights first");
     if (ctx->frame == 0) return fail(ctx, B200VIS_ERR_NOT_READY, "run_shadow_culling: run the CULL stage first");
     cudaStream_t st = ctx->stream;
-    if (!ctx->shadow.n_lights) {                // the sink's one offset: a memset, no launch
+    if (ctx->sdiff.added) {
+        // a slot no item of this run names is emptied (the render world drops an unextracted light's lists): only the ones
+        // that may hold entries, so a steady frame clears nothing.  An inactive item's slot is emptied by the expansion.
+        std::vector<uint8_t> named(ctx->sdiff_max_slots, 0);
+        for (uint32_t i = 0; i < ctx->shadow.n_lights; ++i)
+            if (ctx->h_sdiff_slot[i] != kNoDiffSlot) named[ctx->h_sdiff_slot[i]] = 1;
+        const size_t ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
+        for (uint32_t s = 0; s < ctx->sdiff_max_slots; ++s) {
+            if (ctx->sdiff_held[s] && !named[s]) {
+                CU(cudaMemsetAsync(ctx->sdiff.prev + (size_t)s * 6 * ws, 0, 6 * ws * 4, st));
+                CU(cudaMemsetAsync(ctx->sdiff.prev_count + (size_t)s * 6 * cs, 0, 6 * cs * 4, st));
+            }
+            ctx->sdiff_held[s] = named[s];
+        }
+    }
+    if (!ctx->shadow.n_lights) {                // the sinks' one offset: a memset, no launch
         if (ctx->shsink.entities) CU(cudaMemsetAsync(ctx->shsink.offsets, 0, 4, st));
+        if (ctx->sdiff.added) {
+            CU(cudaMemsetAsync(ctx->sdiff.added_offsets, 0, 4, st));
+            CU(cudaMemsetAsync(ctx->sdiff.removed_offsets, 0, 4, st));
+        }
         return B200VIS_OK;
     }
     Rows R = ctx->rows;
@@ -2664,8 +2753,10 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     CU(cudaMemsetAsync(sb.chunk_count, 0, (size_t)sb.n_lights * 6 * ctx->vis.chunks_stride * 4, st));
     ShadowSink sink = ctx->shsink;
     sink.keys = ctx->d_keys;                    // a compaction swaps the key buffers
+    ShadowDiff sd = ctx->sdiff;
+    sd.keys = ctx->d_keys;
     launch_shadow_cull(st, R, sb, ctx->diff.prev, active_consts(ctx).n_views, ctx->vis.n_words, ctx->vis.n_chunks,
-                       ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u, sink);
+                       ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u, sink, sd);
     CU(cudaGetLastError());
     return B200VIS_OK;
 }
@@ -2721,6 +2812,66 @@ extern "C" int32_t b200vis_set_shadow_entities_sink(b200vis_ctx *ctx, const b200
     s.entities = reinterpret_cast<uint64_t *>(de); s.capacity = sink->capacity; s.offsets = doff;
     s.active = reinterpret_cast<uint8_t *>(dact); s.dev_offsets = ctx->d_shadow_off;
     ctx->shsink_max_items = sink->max_items;
+    return B200VIS_OK;
+}
+
+static void free_shadow_diff(b200vis_ctx *ctx) {
+    ShadowDiff &d = ctx->sdiff;
+    for (void *p : {(void *)d.slot, (void *)d.prev, (void *)d.prev_count, (void *)d.words, (void *)d.chunk, (void *)d.dev_offsets})
+        if (p) cudaFree(p);
+    d = ShadowDiff{}; ctx->sdiff_max_items = ctx->sdiff_max_slots = 0;
+    ctx->h_sdiff_slot.clear(); ctx->sdiff_held.clear();
+}
+extern "C" int32_t b200vis_set_shadow_diff_sink(b200vis_ctx *ctx, const b200vis_shadow_diff_sink *sink) {
+    CHECK_CTX_JOIN();
+    if (sink) {
+        if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_shadow_diff_sink: world_size > 1");
+        if (!sink->added || !sink->removed || !sink->added_offsets || !sink->removed_offsets || !sink->added_capacity || !sink->removed_capacity)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_diff_sink: added, removed, both offsets and both capacities go together");
+        if ((reinterpret_cast<uintptr_t>(sink->added) | reinterpret_cast<uintptr_t>(sink->removed)) & 7u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_diff_sink: added / removed is not 8-byte aligned");
+        if (sink->max_items < ctx->shadow.n_lights)
+            return fail(ctx, B200VIS_ERR_CAPACITY, "set_shadow_diff_sink: max_items %u < %u installed shadow items", sink->max_items,
+                        ctx->shadow.n_lights);
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    free_shadow_diff(ctx);
+    if (!sink) return B200VIS_OK;
+    const size_t n_off = (size_t)sink->max_items * 6 + 1, ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
+    const size_t lists = std::max<size_t>(sink->max_items, 1) * 6;
+    int32_t rc;
+    uint32_t *da = nullptr, *dr = nullptr, *dao = nullptr, *dro = nullptr;
+    if ((rc = map_host(ctx, sink->added, (size_t)sink->added_capacity * 8, &da))) return rc;
+    if ((rc = map_host(ctx, sink->removed, (size_t)sink->removed_capacity * 8, &dr))) return rc;
+    if ((rc = map_host(ctx, sink->added_offsets, n_off * 4, &dao))) return rc;
+    if ((rc = map_host(ctx, sink->removed_offsets, n_off * 4, &dro))) return rc;
+    if ((rc = make_keys_resident(ctx))) return rc;
+    ShadowDiff &d = ctx->sdiff;
+    uint32_t *slot = nullptr;
+    const cudaError_t e = [&]() {
+        cudaError_t x;
+        if ((x = dalloc(&slot, sink->max_items)) != cudaSuccess) return x;
+        d.slot = slot;
+        if ((x = dalloc(&d.prev, (size_t)sink->max_slots * 6 * ws)) != cudaSuccess) return x;          // every slot empty
+        if ((x = dalloc(&d.prev_count, (size_t)sink->max_slots * 6 * cs)) != cudaSuccess) return x;
+        if ((x = dalloc(&d.words, 2 * lists * ws)) != cudaSuccess) return x;
+        if ((x = dalloc(&d.chunk, lists * cs)) != cudaSuccess) return x;
+        return dalloc(&d.dev_offsets, 2 * (lists + 1));
+    }();
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        free_shadow_diff(ctx);
+        return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA, "set_shadow_diff_sink: %zu slot sets: %s",
+                    (size_t)sink->max_slots * 6, cudaGetErrorString(e));
+    }
+    d.lists = (uint32_t)lists;
+    d.added = reinterpret_cast<uint64_t *>(da); d.removed = reinterpret_cast<uint64_t *>(dr);
+    d.added_capacity = sink->added_capacity; d.removed_capacity = sink->removed_capacity;
+    d.added_offsets = dao; d.removed_offsets = dro;
+    ctx->sdiff_max_items = sink->max_items; ctx->sdiff_max_slots = sink->max_slots;
+    ctx->sdiff_held.assign(sink->max_slots, 0);
+    ctx->h_sdiff_slot.assign(ctx->shadow.n_lights, kNoDiffSlot);   // the installed items have no slot until they are set again
+    if (ctx->shadow.n_lights) CU(cudaMemset(slot, 0xFF, (size_t)ctx->shadow.n_lights * 4));
     return B200VIS_OK;
 }
 

@@ -250,6 +250,22 @@ struct ShadowSink {
     uint32_t *dev_offsets;   // the device copy of offsets the expansion reads
     const uint64_t *keys;    // the entity keys in rank order
 };
+// b200vis_set_shadow_diff_sink as the shadow stage sees it (added == nullptr: no sink).  A slot is the caller's persistent
+// identity of one light subview (RetainedViewEntity); its six sets hold the lists last reported for it.
+constexpr uint32_t kNoDiffSlot = 0xFFFFFFFFu;
+struct ShadowDiff {
+    const uint32_t *slot;    // [n_lights] the item's slot, kNoDiffSlot = no diff
+    uint32_t *prev;          // [max_slots * 6][words_stride] last lists reported per (slot, face), bit = rank
+    uint32_t *prev_count;    // [max_slots * 6][chunks_stride] their entries per chunk; 0 = the chunk of the set is empty
+    uint32_t *words;         // [2][lists][words_stride] this run's added, removed bits per list (item * 6 + face)
+    uint32_t *chunk;         // [lists][chunks_stride] per chunk: added count | removed count << 16
+    uint32_t lists;          // max_items * 6: the distance of the removed words from the added ones, in sets
+    uint64_t *added, *removed;              // device aliases of the host regions
+    uint32_t added_capacity, removed_capacity;
+    uint32_t *added_offsets, *removed_offsets;   // device aliases of the host offsets [n_lights * 6 + 1]
+    uint32_t *dev_offsets;   // [2][lists + 1] the device copy of both offsets the emit reads
+    const uint64_t *keys;    // the entity keys in rank order
+};
 
 // SURVEY 8(f) N2: the ViewClusterBindings wire format (bevy_pbr/src/cluster/mod.rs:584-800) packed on the device
 struct BindingBufs {

@@ -3637,35 +3637,88 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
         atomicAdd(&stats->changed[changed_slot][1], prev ? 0xFFFFFFFFu : 1u);
     }
 }
+// The set bits of a warp's words w, as entity keys, stored in order from out[first]: 32 entries at a time, lane j storing
+// entry k + j, so a warp's stores into mapped host memory are consecutive 8-byte words.  ex = the entries of the lanes
+// below this one, wtot = the warp's entries, word = this lane's word (bit b of it is rank word * 32 + b).  The entry's
+// owner is the last lane whose exclusive count is <= it (counts ascend over the lanes), its bit the (e - ex + 1)-th set
+// bit of the owner's word.  Each store is checked against the capacity.
+__device__ __forceinline__ void store_warp_keys(uint32_t w, uint32_t ex, uint32_t wtot, uint32_t word, uint32_t lane, uint32_t first,
+                                                const uint64_t *__restrict__ keys, uint64_t *__restrict__ out, uint32_t capacity) {
+    for (uint32_t k = 0; k < wtot; k += 32u) {
+        const uint32_t e = k + lane;
+        uint32_t o = 0;
+#pragma unroll
+        for (uint32_t step = 16; step > 0; step >>= 1) if (__shfl_sync(0xFFFFFFFFu, ex, o + step) <= e) o += step;
+        const uint32_t wo = __shfl_sync(0xFFFFFFFFu, w, o), exo = __shfl_sync(0xFFFFFFFFu, ex, o);
+        if (e < wtot && first + e < capacity)
+            out[first + e] = keys[(word - lane + o) * 32u + __fns(wo, 0, (int)(e - exo + 1u))];
+    }
+}
 // the sorted CubemapVisibleEntities lists from the bit sets (same chunked scan as k_expand_visible)
 // kSink: b200vis_set_shadow_entities_sink's instantiation, which also stores each entry's Entity key at off[list] + pos of
 // the host region (rank-ordered keys, so keys[rank] is the entry's key), each store checked against its own capacity and
 // the stores of a warp laid out consecutively
-template <bool kSink>
+// kDiff: b200vis_set_shadow_diff_sink's instantiation.  For an item with a slot it also does the set algebra of
+// update_cpu_culled_entities (bevy_render/src/view/visibility/mod.rs:194-249) on each mask word it holds: added = new &
+// ~prev, removed = prev & ~new (both empty for an inactive item), prev := new, with the per-chunk (added | removed << 16)
+// counts and the slot's per-chunk counts for the next run.  A chunk is skipped only when it is empty this run and was
+// empty in the slot's set last run.
+template <bool kSink, bool kDiff>
 __global__ void __launch_bounds__(kChunkWords)
 k_expand_shadow(ShadowBufs sb, uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride,
                 const uint32_t *__restrict__ row_of_rank, const uint64_t *__restrict__ keys, const uint32_t *__restrict__ off,
-                uint64_t *__restrict__ host_entities, uint32_t capacity) {
+                uint64_t *__restrict__ host_entities, uint32_t capacity, ShadowDiff sd) {
     __shared__ uint32_t s_warp[32];
     __shared__ uint32_t s_base, s_total;
+    __shared__ uint32_t s_diff[32], s_dsum;   // kDiff: the warps' packed diff counts, the chunk's
     const uint32_t item = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
     const uint32_t n_faces = sb.lights[item].kind == 0u ? 6u : 1u;
+    uint32_t slot = kNoDiffSlot, on = 0;
+    if constexpr (kDiff) { slot = sd.slot[item]; on = sb.active[item]; }
     for (uint32_t face = 0; face < 6u; ++face) {
         const uint32_t list = item * 6u + face;
-        if (face >= n_faces) { if (chunk == 0 && t == 0) sb.count[list] = 0; continue; }
         const uint32_t *cc = sb.chunk_count + (size_t)list * chunks_stride;
+        uint32_t had = 0;                      // kDiff: the slot set's entries in this chunk last run
+        if constexpr (kDiff) {
+            if (slot != kNoDiffSlot) {
+                had = sd.prev_count[((size_t)slot * 6u + face) * chunks_stride + chunk];
+                if (had == 0 && cc[chunk] == 0 && (chunk != 0 || face >= n_faces)) {   // nothing now, nothing then
+                    if (t == 0) sd.chunk[(size_t)list * chunks_stride + chunk] = 0;
+                    if (chunk == 0 && t == 0) sb.count[list] = 0;
+                    continue;
+                }
+            }
+        }
+        if (face >= n_faces && had == 0) { if (chunk == 0 && t == 0) sb.count[list] = 0; continue; }
         // almost every (list, chunk) is empty (a light reaches a few trees): its mask words are all zero, nothing to read or emit
-        if (chunk != 0 && cc[chunk] == 0) continue;
+        if (chunk != 0 && cc[chunk] == 0 && had == 0) continue;
         const uint32_t word = chunk * kChunkWords + t;
         uint32_t *mask = sb.mask + (size_t)list * words_stride;
         uint32_t w = 0;
         if (word < n_words) { w = mask[word]; if (w) mask[word] = 0; }
         const uint32_t c = __popc(w);
+        uint32_t a = 0, r = 0;
+        if constexpr (kDiff) {
+            if (slot != kNoDiffSlot && word < n_words) {
+                uint32_t *pv = sd.prev + ((size_t)slot * 6u + face) * words_stride + word;
+                const uint32_t old = *pv;
+                if (old != w) *pv = w;         // an inactive item's lists are empty: its slot set is emptied
+                if (on) { a = w & ~old; r = old & ~w; }
+            }
+        }
         uint32_t incl = c;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((t & 31u) >= (uint32_t)o) incl += y; }
         __syncthreads();                       // the previous face's readers of s_warp / s_base are done
         if ((t & 31u) == 31u) s_warp[t >> 5] = incl;
+        if constexpr (kDiff) {
+            if (slot != kNoDiffSlot) {
+                uint32_t d = __popc(a) | (__popc(r) << 16);   // a chunk holds 32768 rows: both sums fit 16 bits
+#pragma unroll
+                for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xFFFFFFFFu, d, o);
+                if ((t & 31u) == 0) s_diff[t >> 5] = d;
+            }
+        }
         if (t < 32) {
             uint32_t part = 0, tot = 0;
             for (uint32_t i = t; i < n_chunks; i += 32) { const uint32_t x = cc[i]; tot += x; if (i < chunk) part += x; }
@@ -3680,24 +3733,34 @@ k_expand_shadow(ShadowBufs sb, uint32_t n_words, uint32_t n_chunks, uint32_t wor
             for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (t >= (uint32_t)o) x += y; }
             s_warp[t] = x;
         }
+        if constexpr (kDiff) {
+            if (slot != kNoDiffSlot) {
+                if (t < 32) {
+                    uint32_t d = s_diff[t];
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xFFFFFFFFu, d, o);
+                    if (t == 0) {
+                        s_dsum = d;
+                        sd.chunk[(size_t)list * chunks_stride + chunk] = d;
+                        sd.prev_count[((size_t)slot * 6u + face) * chunks_stride + chunk] = cc[chunk];   // every thread read `had`
+                    }
+                }
+            }
+        }
         __syncthreads();
+        if constexpr (kDiff) {
+            // only the chunks with a change are read by the emit: a steady chunk writes no words
+            if (slot != kNoDiffSlot && s_dsum != 0u && word < n_words) {
+                sd.words[(size_t)list * words_stride + word] = a;
+                sd.words[((size_t)sd.lists + list) * words_stride + word] = r;
+            }
+        }
         uint32_t pos = s_base + (incl - c) + ((t >> 5) ? s_warp[(t >> 5) - 1] : 0u);
         uint32_t *out = sb.lists + (size_t)list * sb.list_cap;
         if constexpr (kSink) {
-            // the warp's entries in order, 32 at a time: lane j stores entry k + j, so a warp's stores into the mapped sink are
-            // consecutive 8-byte words.  The entry's owner is the last lane whose exclusive count is <= it (counts ascend
-            // over the lanes), its bit the (e - ex + 1)-th set bit of the owner's word.
-            const uint32_t lane = t & 31u, ex = incl - c, wtot = __shfl_sync(0xFFFFFFFFu, incl, 31);
+            const uint32_t lane = t & 31u, wtot = __shfl_sync(0xFFFFFFFFu, incl, 31);
             const uint32_t first = off[list] + s_base + ((t >> 5) ? s_warp[(t >> 5) - 1] : 0u);
-            for (uint32_t k = 0; k < wtot; k += 32u) {
-                const uint32_t e = k + lane;
-                uint32_t o = 0;
-#pragma unroll
-                for (uint32_t step = 16; step > 0; step >>= 1) if (__shfl_sync(0xFFFFFFFFu, ex, o + step) <= e) o += step;
-                const uint32_t wo = __shfl_sync(0xFFFFFFFFu, w, o), exo = __shfl_sync(0xFFFFFFFFu, ex, o);
-                if (e < wtot && first + e < capacity)
-                    host_entities[first + e] = keys[(word - lane + o) * 32u + __fns(wo, 0, (int)(e - exo + 1u))];
-            }
+            store_warp_keys(w, incl - c, wtot, word, lane, first, keys, host_entities, capacity);
         }
         while (w) {
             const uint32_t b = __ffs(w) - 1; w &= w - 1;
@@ -3747,6 +3810,99 @@ k_shadow_offsets(ShadowBufs sb, uint32_t n_chunks, uint32_t chunks_stride, uint3
     }
     __syncthreads();
     if (t == 0) { dev_off[n_lists] = s_carry; host_off[n_lists] = s_carry; }
+}
+
+// b200vis_set_shadow_diff_sink: every list's added and removed totals (the per-chunk counts k_expand_shadow<., true> left
+// behind, summed; zero for an item without a slot), scanned over the lists in item order into both offset arrays (the
+// device copy the emit reads and the host's).  One CTA, as k_shadow_offsets.
+__global__ void __launch_bounds__(1024)
+k_shadow_diff_offsets(ShadowBufs sb, ShadowDiff sd, uint32_t n_chunks, uint32_t chunks_stride) {
+    __shared__ uint32_t s_warp[2][32];
+    __shared__ uint32_t s_carry[2];
+    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5, n_lists = sb.n_lights * 6u;
+    uint32_t *dev_rem = sd.dev_offsets + sd.lists + 1u;
+    if (t < 2) s_carry[t] = 0;
+    for (uint32_t l0 = 0; l0 < n_lists; l0 += 1024u) {
+        const uint32_t l = l0 + t;
+        uint32_t ca = 0, cr = 0;                              // an item without a slot: no diff (its counts were never written)
+        if (l < n_lists && sd.slot[l / 6u] != kNoDiffSlot) {
+            const uint32_t *dc = sd.chunk + (size_t)l * chunks_stride;
+            for (uint32_t k = 0; k < n_chunks; ++k) { const uint32_t x = dc[k]; ca += x & 0xFFFFu; cr += x >> 16; }
+        }
+        uint32_t ia = ca, ir = cr;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t ya = __shfl_up_sync(0xFFFFFFFFu, ia, o), yr = __shfl_up_sync(0xFFFFFFFFu, ir, o);
+            if (lane >= (uint32_t)o) { ia += ya; ir += yr; }
+        }
+        __syncthreads();                                      // the previous round's readers of s_warp / s_carry are done
+        if (lane == 31u) { s_warp[0][warp] = ia; s_warp[1][warp] = ir; }
+        __syncthreads();
+        if (warp < 2) {
+            uint32_t x = s_warp[warp][lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (lane >= (uint32_t)o) x += y; }
+            s_warp[warp][lane] = x;
+        }
+        __syncthreads();
+        const uint32_t ea = s_carry[0] + (warp ? s_warp[0][warp - 1] : 0u) + (ia - ca);
+        const uint32_t er = s_carry[1] + (warp ? s_warp[1][warp - 1] : 0u) + (ir - cr);
+        if (l < n_lists) { sd.dev_offsets[l] = ea; sd.added_offsets[l] = ea; dev_rem[l] = er; sd.removed_offsets[l] = er; }
+        __syncthreads();
+        if (t == 1023u) { s_carry[0] = ea + ca; s_carry[1] = er + cr; }
+    }
+    __syncthreads();
+    if (t == 0) {
+        sd.dev_offsets[n_lists] = s_carry[0]; sd.added_offsets[n_lists] = s_carry[0];
+        dev_rem[n_lists] = s_carry[1]; sd.removed_offsets[n_lists] = s_carry[1];
+    }
+}
+// b200vis_set_shadow_diff_sink: the ordered emit of each list's added and removed entries as keys[rank] into the two host
+// regions, from the bits and per-chunk counts k_expand_shadow<., true> left behind (the chunking of k_emit_visible_diff,
+// the stores of the entity sink).  Chunks without a change are skipped.
+__global__ void __launch_bounds__(kChunkWords)
+k_emit_shadow_diff(ShadowDiff sd, uint32_t n_words, uint32_t words_stride, uint32_t chunks_stride) {
+    __shared__ uint32_t s_warp[32];
+    __shared__ uint32_t s_base[2];
+    const uint32_t item = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x, lane = t & 31u;
+    if (sd.slot[item] == kNoDiffSlot) return;
+    for (uint32_t face = 0; face < 6u; ++face) {
+        const uint32_t list = item * 6u + face;
+        const uint32_t *dc = sd.chunk + (size_t)list * chunks_stride;
+        if (dc[chunk] == 0) continue;
+        const uint32_t word = chunk * kChunkWords + t;
+        uint32_t a = 0, r = 0;
+        if (word < n_words) {
+            a = sd.words[(size_t)list * words_stride + word];
+            r = sd.words[((size_t)sd.lists + list) * words_stride + word];
+        }
+        const uint32_t c = __popc(a) | (__popc(r) << 16);    // both sums of a chunk fit 16 bits
+        uint32_t incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += y; }
+        __syncthreads();                                      // the previous face's readers of s_warp / s_base are done
+        if (lane == 31u) s_warp[t >> 5] = incl;
+        if (t < 32) {                                         // bases: the chunks before this one (unpacked: lists exceed 16 bits)
+            uint32_t pa = 0, pr = 0;
+            for (uint32_t i = t; i < chunk; i += 32) { const uint32_t x = dc[i]; pa += x & 0xFFFFu; pr += x >> 16; }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) { pa += __shfl_xor_sync(0xFFFFFFFFu, pa, o); pr += __shfl_xor_sync(0xFFFFFFFFu, pr, o); }
+            if (t == 0) { s_base[0] = pa; s_base[1] = pr; }
+        }
+        __syncthreads();
+        if (t < 32) {
+            uint32_t x = s_warp[t];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (t >= (uint32_t)o) x += y; }
+            s_warp[t] = x;
+        }
+        __syncthreads();
+        const uint32_t wex = (t >> 5) ? s_warp[(t >> 5) - 1] : 0u, ex = incl - c, wtot = __shfl_sync(0xFFFFFFFFu, incl, 31);
+        store_warp_keys(a, ex & 0xFFFFu, wtot & 0xFFFFu, word, lane, sd.dev_offsets[list] + s_base[0] + (wex & 0xFFFFu), sd.keys,
+                        sd.added, sd.added_capacity);
+        store_warp_keys(r, ex >> 16, wtot >> 16, word, lane, sd.dev_offsets[sd.lists + 1u + list] + s_base[1] + (wex >> 16), sd.keys,
+                        sd.removed, sd.removed_capacity);
+    }
 }
 
 // ------------------------------------------------------------------------------------------
@@ -4315,23 +4471,34 @@ void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const Clust
 }
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
                         uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
-                        const ShadowSink &sink) {
-    if (!sb.n_lights || (!R.n && sink.entities == nullptr)) return;
+                        const ShadowSink &sink, const ShadowDiff &sd) {
+    const bool diff = sd.added != nullptr;
+    if (!sb.n_lights || (!R.n && sink.entities == nullptr && !diff)) return;
     ++g_launches; k_shadow_select<<<cdiv(sb.n_lights, 128), 128, 0, st>>>(sb, R.rank, view_sets, words_stride, n_views);
-    if (!R.n) {                                       // no rows: every list is empty, the sink still gets offsets and flags
-        ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, 0u, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
+    if (!R.n) {                                       // no rows: every list is empty, the sinks still get offsets and flags
+        if (sink.entities != nullptr) { ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, 0u, chunks_stride, sink.dev_offsets, sink.offsets, sink.active); }
+        if (diff) { ++g_launches; k_shadow_diff_offsets<<<1, 1024, 0, st>>>(sb, sd, 0u, chunks_stride); }
         return;
     }
     ++g_launches; k_shadow_cull<<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
     const dim3 grid(n_chunks, sb.n_lights);
-    if (sink.entities == nullptr) {
-        ++g_launches; k_expand_shadow<false><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
-                                                                           nullptr, nullptr, nullptr, 0u);
-        return;
-    }
-    ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
-    ++g_launches; k_expand_shadow<true><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
-                                                                      sink.keys, sink.dev_offsets, sink.entities, sink.capacity);
+    if (sink.entities != nullptr) { ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active); }
+    ++g_launches;
+    if (sink.entities == nullptr && !diff)
+        k_expand_shadow<false, false><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                    nullptr, nullptr, nullptr, 0u, sd);
+    else if (!diff)
+        k_expand_shadow<true, false><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                   sink.keys, sink.dev_offsets, sink.entities, sink.capacity, sd);
+    else if (sink.entities == nullptr)
+        k_expand_shadow<false, true><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                   nullptr, nullptr, nullptr, 0u, sd);
+    else
+        k_expand_shadow<true, true><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
+                                                                  sink.keys, sink.dev_offsets, sink.entities, sink.capacity, sd);
+    if (!diff) return;
+    ++g_launches; k_shadow_diff_offsets<<<1, 1024, 0, st>>>(sb, sd, n_chunks, chunks_stride);
+    ++g_launches; k_emit_shadow_diff<<<grid, kChunkWords, 0, st>>>(sd, n_words, words_stride, chunks_stride);
 }
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views) {
     if (bb.mode) { ++g_launches; k_pack_cluster_bindings<<<dim3(16, max_views), 256, 0, st>>>(fc, cb, bb); }

@@ -28,10 +28,11 @@ void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, con
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R);
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views);
-// sink.entities != nullptr: also the Entity lists, offsets and active flags of b200vis_set_shadow_entities_sink
+// sink.entities != nullptr: also the Entity lists, offsets and active flags of b200vis_set_shadow_entities_sink;
+// sd.added != nullptr: also the added / removed Entity lists and offsets of b200vis_set_shadow_diff_sink
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
                         uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
-                        const ShadowSink &sink);
+                        const ShadowSink &sink, const ShadowDiff &sd);
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views);
 void launch_publish_visible_diff(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, uint32_t *host_rows, uint32_t host_stride,
                                  uint32_t *host_counts, uint32_t n_views, uint32_t max_views);

@@ -738,6 +738,56 @@ typedef struct b200vis_shadow_entities_sink {
     uint8_t  *active;     /* [max_items] */
 } b200vis_shadow_entities_sink;
 B200VIS_API int32_t b200vis_set_shadow_entities_sink(b200vis_ctx *ctx, const b200vis_shadow_entities_sink *sink);
+/* The shadow lists' changes: what collect_visible_cpu_culled_entities computes for the light subviews (render
+ * view/visibility/mod.rs:333-381 calling update_cpu_culled_entities, :194-249), as Entity values.  The caller gives each
+ * item a diff slot with b200vis_set_shadow_items_ex: a persistent identity for the item's RetainedViewEntity (one per
+ * (point light, face), (spot light, 0), (directional light, view, cascade); bevy_pbr render/light.rs:511-551), so the
+ * diff does not depend on the items' order, which may change from frame to frame.  A slot holds six sets, one per face,
+ * with the lists last reported for it; faces past an item's own are empty lists.  Every b200vis_run_shadow_culling then,
+ * on the context's stream (readable after the next b200vis_synchronize):
+ *   - an active item with a slot (the entity sink's active byte 1): for each face f, added = list_f \ prev[slot][f] and
+ *     removed = prev[slot][f] \ list_f, both ascending by to_bits(); then prev[slot][f] := list_f.  (The render-world
+ *     Entity of a mesh is Entity::PLACEHOLDER, mod.rs:78-81: the main-world key decides.)
+ *   - an inactive item with a slot: empty lists, and the slot is emptied;
+ *   - a slot no item of the run names: emptied.  Both follow the render world, which drops the
+ *     RenderShadowMapVisibleEntities of a light it did not extract (light.rs:468, 482-487, 940-951): when the light comes
+ *     back, every entity is added.  A slot survives a run only if an active item names it, so no "clear" call is needed.
+ *   - an item without a slot (B200VIS_SHADOW_NO_SLOT) has no diff: its lists are empty ranges.
+ * Written, with list l = item * 6 + face in item order as in the entity sink:
+ *   added_offsets / removed_offsets[0 .. n_items*6]  exclusive prefix sums; list l of added is added[added_offsets[l] ..
+ *                            added_offsets[l+1]), likewise removed.  The last offset is the true total, even past the
+ *                            capacity; no entry at or past the capacity is written.  Nothing past item n_items is written.
+ *   added / removed          Entity::to_bits() of the entries.
+ * The sets are bit sets over the rank order (ascending to_bits()).  b200vis_set_topology empties every slot (the rows'
+ * identities change), as it does the camera diff.  b200vis_edit_topology and b200vis_compact_topology carry the slots
+ * across: a despawned row in a slot's set is reported removed with its own entity bits by the next run (a compaction keeps
+ * it as a tombstone until then), spawned rows are added when they are listed.
+ * The diff works with or without the entity sink and with list_capacity = 1.  Pinned or registered like the result sink.
+ * Registering allocates max_slots x 6 rank-ordered sets and their per-chunk counts (max_slots x 6 x (words + chunks) x 4
+ * bytes, words = max_entities / 32 rounded up: about 0.75 MB per slot at one million rows), plus the run's added / removed
+ * bits (2 x max_items x 6 sets); every slot starts empty, and the installed items have no slot until items are set again.
+ * While the sink is set the entity keys stay resident on the device.  NULL removes the sink and frees the sets.
+ * Errors, with nothing changed: INVALID_ARG (a NULL pointer, a zero capacity, added / removed not 8-byte aligned),
+ * CAPACITY (max_items below the installed item count; b200vis_set_shadow_items / _ex / b200vis_set_shadow_lights with more
+ * items than a registered sink's max_items), UNSUPPORTED (world_size > 1). */
+#define B200VIS_SHADOW_NO_SLOT 0xFFFFFFFFu
+typedef struct b200vis_shadow_diff_sink {
+    uint64_t *added;            /* [added_capacity] every list's added entries, back to back */
+    uint32_t  added_capacity;
+    uint64_t *removed;          /* [removed_capacity] every list's removed entries, back to back */
+    uint32_t  removed_capacity;
+    uint32_t *added_offsets;    /* [max_items * 6 + 1] */
+    uint32_t *removed_offsets;  /* [max_items * 6 + 1] */
+    uint32_t  max_items;
+    uint32_t  max_slots;        /* slots are 0 .. max_slots - 1 */
+} b200vis_shadow_diff_sink;
+B200VIS_API int32_t b200vis_set_shadow_diff_sink(b200vis_ctx *ctx, const b200vis_shadow_diff_sink *sink);
+/* b200vis_set_shadow_items with a diff slot per item (diff_slots[n_items], B200VIS_SHADOW_NO_SLOT = none); diff_slots ==
+ * NULL is exactly b200vis_set_shadow_items.  Errors, with nothing changed: INVALID_ARG (a slot >= max_slots, the same
+ * slot twice), NOT_READY (slots without a registered b200vis_set_shadow_diff_sink), CAPACITY (as above), and those of
+ * b200vis_set_shadow_items. */
+B200VIS_API int32_t b200vis_set_shadow_items_ex(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items,
+                                                uint32_t list_capacity, const uint32_t *diff_slots);
 /* The shadow-caster byte from the archetype tables: is_caster[t] = 1 when table t's archetype is in the light systems'
  * visible_entity_query (With<Mesh3d>, Without<NotShadowCaster>, Without<DirectionalLight>; NoCpuCulling is a flag of
  * the cull inputs, lib.rs:526-537, 690-701).  n_tables must equal the registry's size.  Like
