@@ -360,6 +360,14 @@ class ShadowDiffSink(C.Structure):
 SHADOW_NO_SLOT = 0xFFFFFFFF
 
 
+class ViewDiffSink(C.Structure):
+    _fields_ = [("added", C.c_void_p), ("added_capacity", C.c_uint32), ("removed", C.c_void_p), ("removed_capacity", C.c_uint32),
+                ("added_offsets", C.c_void_p), ("removed_offsets", C.c_void_p), ("max_slots", C.c_uint32)]
+
+
+VIEW_NO_SLOT = 0xFFFFFFFF
+
+
 class ResultSink(C.Structure):
     _fields_ = [("stats", C.POINTER(FrameStats)), ("visible_rows", C.c_void_p), ("visible_capacity", C.c_uint32),
                 ("visible_classes", C.c_void_p), ("cluster_offsets", C.c_void_p), ("cluster_indices", C.c_void_p), ("cluster_capacity", C.c_uint32)]
@@ -443,6 +451,8 @@ _SIGNATURES = {
     "b200vis_set_shadow_entities_sink": (C.c_int32, [_vp, _P(ShadowEntitiesSink)]),
     "b200vis_set_shadow_diff_sink": (C.c_int32, [_vp, _P(ShadowDiffSink)]),
     "b200vis_set_shadow_items_ex": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _vp]),
+    "b200vis_set_view_diff_sink": (C.c_int32, [_vp, _P(ViewDiffSink)]),
+    "b200vis_set_view_diff_slots": (C.c_int32, [_vp, C.c_uint32, _vp]),
     "b200vis_host_point_light_frusta": (None, [_vp, C.c_float, C.c_float, _vp]),
     "b200vis_upload_visibility_ranges": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "b200vis_set_visibility_range_views": (C.c_int32, [_vp, C.c_uint32, _vp]),
@@ -1091,6 +1101,33 @@ class Context:
                                 None if offsets is None else offsets.ctypes.data)
         self._check(self._lib.b200vis_set_visible_entities_sink(self._h, C.byref(s)))
         self._ent_sink = (entities, offsets)
+
+    def set_view_diff_sink(self, added, removed, added_offsets, removed_offsets, max_slots=0, added_capacity=None,
+                           removed_capacity=None):
+        """b200vis_set_view_diff_sink: pinned (or registrable) host numpy arrays added / removed [capacity] uint64
+        (Entity::to_bits() of every (view, class) list's added / removed entries, back to back) and added_offsets /
+        removed_offsets [max_views * 8 + 1] uint32 (list view * 8 + class is added[added_offsets[l]:added_offsets[l + 1]]);
+        max_slots diff slots.  The capacities default to the arrays' sizes.  All None removes the sink."""
+        if added is None and removed is None and added_offsets is None and removed_offsets is None:
+            self._check(self._lib.b200vis_set_view_diff_sink(self._h, None))
+            self._view_diff_sink = None
+            return
+        ptr = lambda a: None if a is None else a.ctypes.data
+        size = lambda a: 0 if a is None else a.size
+        ac = size(added) if added_capacity is None else added_capacity
+        rc = size(removed) if removed_capacity is None else removed_capacity
+        n_off = self.max_views * 8 + 1
+        if added is not None and ac > added.size or removed is not None and rc > removed.size or \
+                added_offsets is not None and added_offsets.size < n_off or removed_offsets is not None and removed_offsets.size < n_off:
+            raise ValueError("set_view_diff_sink: the arrays are smaller than the capacities / max_views * 8 + 1 offsets")
+        s = ViewDiffSink(ptr(added), ac, ptr(removed), rc, ptr(added_offsets), ptr(removed_offsets), max_slots)
+        self._check(self._lib.b200vis_set_view_diff_sink(self._h, C.byref(s)))
+        self._view_diff_sink = (added, removed, added_offsets, removed_offsets)
+
+    def set_view_diff_slots(self, slots):
+        """b200vis_set_view_diff_slots: view i's diff slot is slots[i] (VIEW_NO_SLOT = none); views past len(slots) have none."""
+        sl = np.ascontiguousarray(slots, np.uint32)
+        self._check(self._lib.b200vis_set_view_diff_slots(self._h, len(sl), _ptr(sl) if len(sl) else None))
 
     def set_column_sinks(self, gt=None, gt_changed_bits=None, view_visibility=None, vv_changed_bits=None):
         """b200vis_set_column_sinks: numpy arrays over (ideally pinned) host memory; gt is [n, 12] or [n, 16] float32.

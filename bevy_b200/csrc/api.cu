@@ -170,6 +170,10 @@ struct b200vis_ctx {
     // the installed items' slots, and which slots may hold entries (the ones a run named since they were last emptied)
     ShadowDiff sdiff{}; uint32_t sdiff_max_items = 0, sdiff_max_slots = 0;
     std::vector<uint32_t> h_sdiff_slot; std::vector<uint8_t> sdiff_held;
+    // b200vis_set_view_diff_sink: the device state (added == nullptr: none), max_slots, the view -> slot map of
+    // b200vis_set_view_diff_slots ([max_views], kNoDiffSlot = none), and which slots may hold entries
+    ViewDiff vdiff{}; uint32_t vdiff_max_slots = 0;
+    std::vector<uint32_t> h_vdiff_slot; std::vector<uint8_t> vdiff_held;
 
     b200vis_column_sinks colsink{}; bool have_colsink = false;          // b200vis_set_column_sinks (device aliases below)
     float *col_gt_d = nullptr; uint32_t *col_gt_bits_d = nullptr, *col_vv_bits_d = nullptr; uint8_t *col_vv_d = nullptr;
@@ -266,7 +270,8 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_tabs, ctx->d_tab_chunks, ctx->d_tab_map, ctx->d_tab_total, ctx->d_tvv_shadow, ctx->d_tab_upd,
                    ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster,
                    ctx->d_tab_range, const_cast<uint32_t *>(ctx->sdiff.slot), ctx->sdiff.prev, ctx->sdiff.prev_count,
-                   ctx->sdiff.words, ctx->sdiff.chunk, ctx->sdiff.dev_offsets};
+                   ctx->sdiff.words, ctx->sdiff.chunk, ctx->sdiff.dev_offsets, ctx->vdiff.prev, ctx->vdiff.prev_count,
+                   ctx->vdiff.words, ctx->vdiff.chunk, ctx->vdiff.dev_offsets};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -1045,6 +1050,11 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         CU(cudaMemset(ctx->sdiff.prev_count, 0, (size_t)ctx->sdiff_max_slots * 6 * ctx->vis.chunks_stride * 4));
         std::fill(ctx->sdiff_held.begin(), ctx->sdiff_held.end(), 0);
     }
+    if (ctx->vdiff.added) {                      // ... and every view diff slot
+        CU(cudaMemset(ctx->vdiff.prev, 0, (size_t)ctx->vdiff_max_slots * 8 * ctx->vis.words_stride * 4));
+        CU(cudaMemset(ctx->vdiff.prev_count, 0, (size_t)ctx->vdiff_max_slots * ctx->vis.chunks_stride * 4));
+        std::fill(ctx->vdiff_held.begin(), ctx->vdiff_held.end(), 0);
+    }
     ctx->topology_set = true;
     ctx->gt_aos_valid = false;
     {   // what b200vis_edit_topology starts from: the plan, and the keys in rank order (uploaded by the first merge)
@@ -1056,7 +1066,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
         ctx->keys_resident = false;
         ctx->max_key = n ? ctx->h_keys[n - 1] : 0;
     }
-    if (ctx->ent_sink_d || ctx->shsink.entities || ctx->sdiff.added) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sinks read them
+    if (ctx->ent_sink_d || ctx->shsink.entities || ctx->sdiff.added || ctx->vdiff.added) { const int32_t krc = make_keys_resident(ctx); if (krc) return krc; }   // the Entity sinks read them
     return tables_unmap_all(ctx);
 }
 
@@ -1103,23 +1113,38 @@ static int32_t alloc_rank_spares(b200vis_ctx *ctx, bool keys) {
     return B200VIS_OK;
 }
 
-// The shadow diff slots' sets (bit = rank) to new ranks: each slot that may hold entries, through the added / removed words
-// (free between runs; they hold at least 12 sets).  compacting: the set is cleared first, so words past the new end are
-// empty.  A remapped slot's per-chunk counts become "unknown" (non-zero), so that the next run reads every chunk of it.
-static int32_t remap_shadow_diff_slots(b200vis_ctx *ctx, bool compacting, uint32_t n_words, uint32_t n_rows, uint32_t n_old_rows,
-                                       const uint32_t *row_of_rank, const uint32_t *old_rank) {
-    if (!ctx->sdiff.added) return B200VIS_OK;
+// Diff slots' sets (bit = rank) to new ranks: each slot that may hold entries (held), `sets` sets per slot, through the
+// run's added / removed words (free between runs; they hold at least 2 * sets sets).  compacting: the set is cleared
+// first, so words past the new end are empty.  A remapped slot's per-chunk counts (`count_sets` rows of them per slot)
+// become "unknown" (non-zero), so that the next run reads every chunk of it.
+static int32_t remap_slot_sets(b200vis_ctx *ctx, uint32_t *prev, uint32_t *prev_count, uint32_t *scratch, uint32_t sets, uint32_t count_sets,
+                               const std::vector<uint8_t> &held, bool compacting, uint32_t n_words, uint32_t n_rows, uint32_t n_old_rows,
+                               const uint32_t *row_of_rank, const uint32_t *old_rank) {
     cudaStream_t st = ctx->stream;
     const size_t ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
-    for (uint32_t s = 0; s < ctx->sdiff_max_slots; ++s) {
-        if (!ctx->sdiff_held[s]) continue;
-        uint32_t *set = ctx->sdiff.prev + (size_t)s * 6 * ws;
-        CU(cudaMemcpyAsync(ctx->sdiff.words, set, 6 * ws * 4, cudaMemcpyDeviceToDevice, st));
-        if (compacting) CU(cudaMemsetAsync(set, 0, 6 * ws * 4, st));
-        launch_remap_rank_sets(st, ctx->sdiff.words, set, (uint32_t)ws, 6, n_words, n_rows, n_old_rows, row_of_rank, old_rank);
+    for (uint32_t s = 0; s < held.size(); ++s) {
+        if (!held[s]) continue;
+        uint32_t *set = prev + (size_t)s * sets * ws;
+        CU(cudaMemcpyAsync(scratch, set, sets * ws * 4, cudaMemcpyDeviceToDevice, st));
+        if (compacting) CU(cudaMemsetAsync(set, 0, sets * ws * 4, st));
+        launch_remap_rank_sets(st, scratch, set, (uint32_t)ws, sets, n_words, n_rows, n_old_rows, row_of_rank, old_rank);
         CU(cudaGetLastError());
-        CU(cudaMemsetAsync(ctx->sdiff.prev_count + (size_t)s * 6 * cs, 0xFF, 6 * cs * 4, st));
+        CU(cudaMemsetAsync(prev_count + (size_t)s * count_sets * cs, 0xFF, count_sets * cs * 4, st));
     }
+    return B200VIS_OK;
+}
+// ... for the shadow diff's slots (six sets each) and the view diff's (eight sets each, one count row)
+static int32_t remap_diff_slots(b200vis_ctx *ctx, bool compacting, uint32_t n_words, uint32_t n_rows, uint32_t n_old_rows,
+                                const uint32_t *row_of_rank, const uint32_t *old_rank) {
+    int32_t rc;
+    if (ctx->sdiff.added &&
+        (rc = remap_slot_sets(ctx, ctx->sdiff.prev, ctx->sdiff.prev_count, ctx->sdiff.words, 6, 6, ctx->sdiff_held, compacting, n_words,
+                              n_rows, n_old_rows, row_of_rank, old_rank)))
+        return rc;
+    if (ctx->vdiff.added &&
+        (rc = remap_slot_sets(ctx, ctx->vdiff.prev, ctx->vdiff.prev_count, ctx->vdiff.words, 8, 1, ctx->vdiff_held, compacting, n_words,
+                              n_rows, n_old_rows, row_of_rank, old_rank)))
+        return rc;
     return B200VIS_OK;
 }
 
@@ -1256,7 +1281,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
                                    ctx->d_row_of_rank, old_rank);
             CU(cudaGetLastError());
         }
-        if ((rc = remap_shadow_diff_slots(ctx, false, (n2 + 31) / 32, n2, n, ctx->d_row_of_rank, old_rank))) return rc;
+        if ((rc = remap_diff_slots(ctx, false, (n2 + 31) / 32, n2, n, ctx->d_row_of_rank, old_rank))) return rc;
         ctx->rank_identity = false;
     } else if (n_spawn) {
         if (ctx->keys_resident) { if ((rc = put(ctx->d_keys + n, spawn_entity_bits, (size_t)n_spawn * 8))) return rc; CU(cudaEventRecord(ctx->ev_edit, st)); }
@@ -1313,6 +1338,11 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
             for (uint32_t s = 0; s < ctx->sdiff_max_slots; ++s)
                 if (ctx->sdiff_held[s])
                     launch_mark_set_rows(st, ctx->sdiff.prev + (size_t)s * 6 * ctx->vis.words_stride, ctx->vis.words_stride, 6, (n + 31) / 32,
+                                         ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->d_dirty);
+        if (ctx->vdiff.added)   // ... and the view diff slots' sets
+            for (uint32_t s = 0; s < ctx->vdiff_max_slots; ++s)
+                if (ctx->vdiff_held[s])
+                    launch_mark_set_rows(st, ctx->vdiff.prev + (size_t)s * 8 * ctx->vis.words_stride, ctx->vis.words_stride, 8, (n + 31) / 32,
                                          ctx->rank_identity ? nullptr : ctx->d_row_of_rank, ctx->d_dirty);
         CU(cudaGetLastError());
         CU(cudaMemcpyAsync(ctx->h_stage, ctx->d_dirty, n, cudaMemcpyDeviceToHost, st));
@@ -1435,7 +1465,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
         launch_remap_rank_sets(st, ctx->diff.words, ctx->diff.prev, ctx->vis.words_stride, V, (n2 + 31) / 32, n2, n, d_src, nullptr);
         CU(cudaGetLastError());
     }
-    if ((rc = remap_shadow_diff_slots(ctx, true, (n2 + 31) / 32, n2, n, d_src, nullptr))) return rc;
+    if ((rc = remap_diff_slots(ctx, true, (n2 + 31) / 32, n2, n, d_src, nullptr))) return rc;
     // ---- the lists results hold, renumbered in place (survivors keep their rank order, so every list stays sorted) ----
     for (uint32_t i = 0; i < n_lists; ++i) launch_renumber_listed_rows(st, lists[i], n, d_o2n, n);
     if ((rc = flush_table_updates(ctx))) return rc;      // queued map updates carry the old row numbers
@@ -2218,6 +2248,30 @@ extern "C" int32_t b200vis_join(b200vis_ctx *ctx) {
     return join_all(ctx);
 }
 
+// b200vis_set_view_diff_sink, once per run that culls: the run's view -> slot map (views at or past the frame's view count
+// have no slot; slotted = one past the last view with a slot), and the slots no view of the run names emptied on the tail
+// stream ahead of the diff.  Only the slots that may hold entries are cleared, so a steady frame clears nothing; an
+// inactive view's slot is emptied by k_view_diff.
+static int32_t view_diff_slots_of_run(b200vis_ctx *ctx, cudaStream_t tail, uint32_t n_views, ViewSlots &vs, uint32_t &slotted) {
+    std::fill(std::begin(vs.slot), std::end(vs.slot), kNoDiffSlot);
+    slotted = 0;
+    std::vector<uint8_t> named(ctx->vdiff_max_slots, 0);
+    for (uint32_t v = 0; v < n_views && v < ctx->h_vdiff_slot.size(); ++v) {
+        const uint32_t s = ctx->h_vdiff_slot[v];
+        if (s == kNoDiffSlot) continue;
+        vs.slot[v] = s; named[s] = 1; slotted = v + 1;
+    }
+    const size_t ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
+    for (uint32_t s = 0; s < ctx->vdiff_max_slots; ++s) {
+        if (ctx->vdiff_held[s] && !named[s]) {
+            CU(cudaMemsetAsync(ctx->vdiff.prev + (size_t)s * 8 * ws, 0, 8 * ws * 4, tail));
+            CU(cudaMemsetAsync(ctx->vdiff.prev_count + (size_t)s * cs, 0, cs * 4, tail));
+        }
+        ctx->vdiff_held[s] = named[s];
+    }
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     CHECK_CTX();
     if (!ctx->topology_set) return fail(ctx, B200VIS_ERR_NOT_READY, "run: b200vis_set_topology has not been called");
@@ -2435,6 +2489,14 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     if (exchange_first) { const int32_t rc = issue_assign_and_exchange(); if (rc) return rc; }
     if (pe) CU(cudaEventRecord(pe[5], tail));
     if (do_cull && ctx->pub_pending) { CU(cudaStreamWaitEvent(tail, ctx->ev_pub, 0)); ctx->pub_pending = false; }   // lists are rewritten
+    ViewDiff vd = ctx->vdiff;
+    ViewSlots vs;
+    uint32_t slotted = 0;
+    if (do_cull && vd.added) {                   // ahead of the expansion, which consumes the masks
+        const int32_t rc = view_diff_slots_of_run(ctx, tail, afc.n_views, vs, slotted); if (rc) return rc;
+        vd.keys = ctx->d_keys;                   // a compaction swaps the key buffers
+        launch_view_diff(tail, vb, vd, vs, R.row_of_rank, fc, cslot, slotted);
+    }
     if (do_cull) {
         launch_expand_visible(tail, vb, ctx->diff_on ? ctx->diff : DiffBufs{}, R.row_of_rank, fc, ctx->d_stats, cslot, ctx->n, ctx->cfg.max_views);
         if (pipelined) CU(cudaEventRecord(ctx->ev_expand[mslot], tail));   // this frame's masks / counters are free again
@@ -2444,6 +2506,7 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
         if (ctx->ent_sink_d)
             launch_emit_visible_entities(tail, vb, R.rank, ctx->d_keys, fc, ctx->d_stats, ctx->n, ctx->cfg.max_views, ctx->d_ent_counts,
                                          ctx->ent_chunks, ctx->ent_sink_d, ctx->ent_cap, ctx->ent_off_d);
+        if (vd.added) launch_emit_view_diff(tail, vb, vd, vs, afc.n_views, slotted);
     }
     if (do_cull && ctx->have_sink && ctx->sink_rows_d) {
         // posting ~1 MB of visible rows over PCIe takes tens of microseconds: in the serial (non-pipelined) case do it on the
@@ -2872,6 +2935,79 @@ extern "C" int32_t b200vis_set_shadow_diff_sink(b200vis_ctx *ctx, const b200vis_
     ctx->sdiff_held.assign(sink->max_slots, 0);
     ctx->h_sdiff_slot.assign(ctx->shadow.n_lights, kNoDiffSlot);   // the installed items have no slot until they are set again
     if (ctx->shadow.n_lights) CU(cudaMemset(slot, 0xFF, (size_t)ctx->shadow.n_lights * 4));
+    return B200VIS_OK;
+}
+
+static void free_view_diff(ViewDiff &d) {
+    for (void *p : {(void *)d.prev, (void *)d.prev_count, (void *)d.words, (void *)d.chunk, (void *)d.dev_offsets})
+        if (p) cudaFree(p);
+    d = ViewDiff{};
+}
+extern "C" int32_t b200vis_set_view_diff_sink(b200vis_ctx *ctx, const b200vis_view_diff_sink *sink) {
+    CHECK_CTX_JOIN();
+    if (sink) {
+        if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_view_diff_sink: world_size > 1");
+        if (!sink->added || !sink->removed || !sink->added_offsets || !sink->removed_offsets || !sink->added_capacity || !sink->removed_capacity)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_sink: added, removed, both offsets and both capacities go together");
+        if ((reinterpret_cast<uintptr_t>(sink->added) | reinterpret_cast<uintptr_t>(sink->removed)) & 7u)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_sink: added / removed is not 8-byte aligned");
+    }
+    CU(cudaStreamSynchronize(ctx->stream));
+    if (!sink) {
+        free_view_diff(ctx->vdiff); ctx->vdiff_max_slots = 0;
+        ctx->h_vdiff_slot.clear(); ctx->vdiff_held.clear();
+        return B200VIS_OK;
+    }
+    const size_t lists = (size_t)ctx->cfg.max_views * 8, ws = ctx->vis.words_stride, cs = ctx->vis.chunks_stride;
+    const size_t sets = (size_t)std::max<uint32_t>(sink->max_slots, 1) * 8;
+    int32_t rc;
+    uint32_t *da = nullptr, *dr = nullptr, *dao = nullptr, *dro = nullptr;
+    if ((rc = map_host(ctx, sink->added, (size_t)sink->added_capacity * 8, &da))) return rc;
+    if ((rc = map_host(ctx, sink->removed, (size_t)sink->removed_capacity * 8, &dr))) return rc;
+    if ((rc = map_host(ctx, sink->added_offsets, (lists + 1) * 4, &dao))) return rc;
+    if ((rc = map_host(ctx, sink->removed_offsets, (lists + 1) * 4, &dro))) return rc;
+    ViewDiff d{};
+    const cudaError_t e = [&]() {
+        cudaError_t x;
+        if ((x = dalloc(&d.prev, sets * ws)) != cudaSuccess) return x;              // every slot empty
+        if ((x = dalloc(&d.prev_count, sets / 8 * cs)) != cudaSuccess) return x;
+        if ((x = dalloc(&d.words, 2 * sets * ws)) != cudaSuccess) return x;
+        if ((x = dalloc(&d.chunk, sets * cs)) != cudaSuccess) return x;
+        return dalloc(&d.dev_offsets, 2 * (lists + 1));
+    }();
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        free_view_diff(d);
+        return fail(ctx, e == cudaErrorMemoryAllocation ? B200VIS_ERR_OUT_OF_MEMORY : B200VIS_ERR_CUDA, "set_view_diff_sink: %zu slot sets: %s",
+                    sets, cudaGetErrorString(e));
+    }
+    if ((rc = make_keys_resident(ctx))) { free_view_diff(d); return rc; }
+    d.sets = (uint32_t)sets; d.lists = (uint32_t)lists;
+    d.added = reinterpret_cast<uint64_t *>(da); d.removed = reinterpret_cast<uint64_t *>(dr);
+    d.added_capacity = sink->added_capacity; d.removed_capacity = sink->removed_capacity;
+    d.added_offsets = dao; d.removed_offsets = dro;
+    free_view_diff(ctx->vdiff);
+    ctx->vdiff = d; ctx->vdiff_max_slots = sink->max_slots;
+    ctx->vdiff_held.assign(sink->max_slots, 0);
+    ctx->h_vdiff_slot.assign(ctx->cfg.max_views, kNoDiffSlot);   // no view has a slot until the slots are set
+    return B200VIS_OK;
+}
+extern "C" int32_t b200vis_set_view_diff_slots(b200vis_ctx *ctx, uint32_t n_views, const uint32_t *slots) {
+    CHECK_CTX();
+    if (n_views > ctx->cfg.max_views) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_slots: %u views > max_views %u", n_views, ctx->cfg.max_views);
+    if (n_views && !slots) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_slots: null");
+    if (!ctx->vdiff.added) return fail(ctx, B200VIS_ERR_NOT_READY, "set_view_diff_slots: no view diff sink is registered");
+    std::vector<uint8_t> seen(ctx->vdiff_max_slots, 0);
+    for (uint32_t v = 0; v < n_views; ++v) {
+        const uint32_t s = slots[v];
+        if (s == B200VIS_VIEW_NO_SLOT) continue;
+        if (s >= ctx->vdiff_max_slots)
+            return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_slots: view %u: slot %u >= max_slots %u", v, s, ctx->vdiff_max_slots);
+        if (seen[s]) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_view_diff_slots: slot %u named twice", s);
+        seen[s] = 1;
+    }
+    std::fill(ctx->h_vdiff_slot.begin(), ctx->h_vdiff_slot.end(), kNoDiffSlot);
+    std::copy(slots, slots + n_views, ctx->h_vdiff_slot.begin());
     return B200VIS_OK;
 }
 

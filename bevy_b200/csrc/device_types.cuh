@@ -266,6 +266,25 @@ struct ShadowDiff {
     uint32_t *dev_offsets;   // [2][lists + 1] the device copy of both offsets the emit reads
     const uint64_t *keys;    // the entity keys in rank order
 };
+// b200vis_set_view_diff_sink as the frame's tail sees it (added == nullptr: no sink).  A slot is the caller's persistent
+// identity of one camera's RenderVisibleEntities; its eight sets, one per VisibilityClass, hold the lists last reported
+// for it.  Everything per slot is indexed by the slot, so the scratch grows with max_slots, not with max_views.
+struct ViewDiff {
+    uint32_t *prev;          // [max_slots * 8][words_stride] last lists reported per (slot, class), bit = rank
+    uint32_t *prev_count;    // [max_slots][chunks_stride] the slot's listed rows per chunk last run (any class); 0 = empty
+    uint32_t *words;         // [2][sets][words_stride] this run's added, removed bits per (slot, class)
+    uint32_t *chunk;         // [sets][chunks_stride] per chunk: added count | removed count << 16
+    uint32_t sets;           // max_slots * 8: the distance of the removed words from the added ones, in sets
+    uint32_t lists;          // max_views * 8: the distance of the removed offsets from the added ones, less one
+    uint64_t *added, *removed;              // device aliases of the host regions
+    uint32_t added_capacity, removed_capacity;
+    uint32_t *added_offsets, *removed_offsets;   // device aliases of the host offsets [max_views * 8 + 1]
+    uint32_t *dev_offsets;   // [2][lists + 1] the device copy of both offsets the emit reads
+    const uint64_t *keys;    // the entity keys in rank order
+};
+// One run's view -> slot map (kNoDiffSlot = none), passed by value: it travels with the launches of its frame, so a
+// pipelined tail of frame f uses frame f's map while the caller installs the one for frame f + 1.
+struct ViewSlots { uint32_t slot[kMaxCameras]; };
 
 // SURVEY 8(f) N2: the ViewClusterBindings wire format (bevy_pbr/src/cluster/mod.rs:584-800) packed on the device
 struct BindingBufs {

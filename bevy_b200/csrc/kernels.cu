@@ -3906,6 +3906,168 @@ k_emit_shadow_diff(ShadowDiff sd, uint32_t n_words, uint32_t words_stride, uint3
 }
 
 // ------------------------------------------------------------------------------------------
+// Kernel 2c (SURVEY 8(f) N1, b200vis_set_view_diff_sink): update_cpu_culled_entities per (camera, VisibilityClass)
+// (bevy_render/src/view/visibility/mod.rs:389-431).  One CTA per (1024-word chunk, view), launched before
+// k_expand_visible, which still consumes and zeroes the mask.  The mask holds exactly the listed rows (visible, with a
+// class): each thread splits its word into eight per-class words by gathering the rows' class masks, then does the set
+// algebra against the slot's eight sets: added = new & ~prev, removed = prev & ~new (both empty for an inactive view,
+// whose slot is emptied), prev := new.  It leaves the per-(slot, class, chunk) counts and, for the chunks with a change
+// only, the added / removed words.  A chunk is skipped only when it is empty this run and was empty in the slot last run.
+// ------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kChunkWords)
+k_view_diff(VisibleBufs vb, ViewDiff vd, ViewSlots vs, const uint32_t *__restrict__ row_of_rank, const FrameConsts *__restrict__ fc,
+            uint32_t parity) {
+    __shared__ uint32_t s_cnt[8];
+    const uint32_t v = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
+    const uint32_t slot = vs.slot[v];
+    if (slot == kNoDiffSlot) return;
+    const bool on = (fc->views[v].flags & 1u) != 0u;
+    const size_t cs = vb.chunks_stride, ws = vb.words_stride;
+    const uint32_t now = on ? vb.chunk_count[chunk_counter_index(parity, v) * cs + chunk] : 0u;
+    uint32_t *had_p = vd.prev_count + (size_t)slot * cs + chunk;
+    const uint32_t had = *had_p;                                  // 0xFFFFFFFF after a remap: unknown
+    uint32_t *dc = vd.chunk + (size_t)slot * 8u * cs + chunk;
+    if (now == 0u && had == 0u) {                                 // nothing now, nothing then
+        if (t < 8u) dc[t * cs] = 0u;
+        return;
+    }
+    if (t < 8u) s_cnt[t] = 0u;
+    const uint32_t word = chunk * kChunkWords + t;
+    uint32_t nw[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) nw[k] = 0u;
+    if (now != 0u && word < vb.n_words) {
+        uint32_t w = vb.mask[(size_t)v * ws + word];
+        while (w) {
+            const uint32_t b = __ffs(w) - 1; w &= w - 1;
+            const uint32_t rk = word * 32u + b;
+            const uint32_t c = vb.cls[row_of_rank ? row_of_rank[rk] : rk];
+#pragma unroll
+            for (int k = 0; k < 8; ++k) nw[k] |= ((c >> k) & 1u) << b;
+        }
+    }
+    __syncthreads();                                              // s_cnt is zeroed
+    uint32_t a[8], r[8];
+#pragma unroll
+    for (int k = 0; k < 8; ++k) {
+        a[k] = r[k] = 0u;
+        if (word < vb.n_words) {
+            uint32_t *pv = vd.prev + ((size_t)slot * 8u + k) * ws + word;
+            const uint32_t old = had ? *pv : 0u;
+            if (old != nw[k]) *pv = nw[k];
+            if (on) { a[k] = nw[k] & ~old; r[k] = old & ~nw[k]; }
+        }
+        const uint32_t d = __reduce_add_sync(0xFFFFFFFFu, __popc(a[k]) | (__popc(r[k]) << 16));   // a chunk: both fit 16 bits
+        if ((t & 31u) == 0u && d) atomicAdd(&s_cnt[k], d);
+    }
+    __syncthreads();                                              // every thread has read `had` and added its counts
+    if (t < 8u) dc[t * cs] = s_cnt[t];
+    if (t == 0u) *had_p = now;
+    if (word < vb.n_words) {
+#pragma unroll
+        for (int k = 0; k < 8; ++k) {
+            if (!s_cnt[k]) continue;                              // only the chunks with a change are read by the emit
+            vd.words[((size_t)slot * 8u + k) * ws + word] = a[k];
+            vd.words[((size_t)vd.sets + slot * 8u + k) * ws + word] = r[k];
+        }
+    }
+}
+// b200vis_set_view_diff_sink: every list's added and removed totals (list l = view * 8 + class; zero for a view without a
+// slot), scanned in list order into both offset arrays (the device copy the emit reads and the host's).  One CTA, as
+// k_shadow_diff_offsets, whose lists are indexed by list rather than by slot.
+__global__ void __launch_bounds__(1024)
+k_view_diff_offsets(ViewDiff vd, ViewSlots vs, uint32_t n_lists, uint32_t n_chunks, uint32_t chunks_stride) {
+    __shared__ uint32_t s_warp[2][32];
+    __shared__ uint32_t s_carry[2];
+    const uint32_t t = threadIdx.x, lane = t & 31u, warp = t >> 5;
+    uint32_t *dev_rem = vd.dev_offsets + vd.lists + 1u;
+    if (t < 2) s_carry[t] = 0;
+    for (uint32_t l0 = 0; l0 < n_lists; l0 += 1024u) {
+        const uint32_t l = l0 + t;
+        uint32_t ca = 0, cr = 0;
+        const uint32_t slot = l < n_lists ? vs.slot[l >> 3] : kNoDiffSlot;
+        if (slot != kNoDiffSlot) {
+            const uint32_t *dc = vd.chunk + ((size_t)slot * 8u + (l & 7u)) * chunks_stride;
+            for (uint32_t k = 0; k < n_chunks; ++k) { const uint32_t x = dc[k]; ca += x & 0xFFFFu; cr += x >> 16; }
+        }
+        uint32_t ia = ca, ir = cr;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+            const uint32_t ya = __shfl_up_sync(0xFFFFFFFFu, ia, o), yr = __shfl_up_sync(0xFFFFFFFFu, ir, o);
+            if (lane >= (uint32_t)o) { ia += ya; ir += yr; }
+        }
+        __syncthreads();                                      // the previous round's readers of s_warp / s_carry are done
+        if (lane == 31u) { s_warp[0][warp] = ia; s_warp[1][warp] = ir; }
+        __syncthreads();
+        if (warp < 2) {
+            uint32_t x = s_warp[warp][lane];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (lane >= (uint32_t)o) x += y; }
+            s_warp[warp][lane] = x;
+        }
+        __syncthreads();
+        const uint32_t ea = s_carry[0] + (warp ? s_warp[0][warp - 1] : 0u) + (ia - ca);
+        const uint32_t er = s_carry[1] + (warp ? s_warp[1][warp - 1] : 0u) + (ir - cr);
+        if (l < n_lists) { vd.dev_offsets[l] = ea; vd.added_offsets[l] = ea; dev_rem[l] = er; vd.removed_offsets[l] = er; }
+        __syncthreads();
+        if (t == 1023u) { s_carry[0] = ea + ca; s_carry[1] = er + cr; }
+    }
+    __syncthreads();
+    if (t == 0) {
+        vd.dev_offsets[n_lists] = s_carry[0]; vd.added_offsets[n_lists] = s_carry[0];
+        dev_rem[n_lists] = s_carry[1]; vd.removed_offsets[n_lists] = s_carry[1];
+    }
+}
+// b200vis_set_view_diff_sink: the ordered emit of each (view, class) list's added and removed entries as keys[rank] into
+// the two host regions, from the words and per-chunk counts k_view_diff left behind (k_emit_shadow_diff's chunking and
+// stores, with the counts indexed by slot).  Chunks without a change are skipped.
+__global__ void __launch_bounds__(kChunkWords)
+k_emit_view_diff(ViewDiff vd, ViewSlots vs, uint32_t n_words, uint32_t words_stride, uint32_t chunks_stride) {
+    __shared__ uint32_t s_warp[32];
+    __shared__ uint32_t s_base[2];
+    const uint32_t v = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x, lane = t & 31u;
+    const uint32_t slot = vs.slot[v];
+    if (slot == kNoDiffSlot) return;
+    for (uint32_t k = 0; k < 8u; ++k) {
+        const uint32_t list = v * 8u + k, set = slot * 8u + k;
+        const uint32_t *dc = vd.chunk + (size_t)set * chunks_stride;
+        if (dc[chunk] == 0) continue;
+        const uint32_t word = chunk * kChunkWords + t;
+        uint32_t a = 0, r = 0;
+        if (word < n_words) {
+            a = vd.words[(size_t)set * words_stride + word];
+            r = vd.words[((size_t)vd.sets + set) * words_stride + word];
+        }
+        const uint32_t c = __popc(a) | (__popc(r) << 16);    // both sums of a chunk fit 16 bits
+        uint32_t incl = c;
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += y; }
+        __syncthreads();                                      // the previous class's readers of s_warp / s_base are done
+        if (lane == 31u) s_warp[t >> 5] = incl;
+        if (t < 32) {                                         // bases: the chunks before this one (unpacked: lists exceed 16 bits)
+            uint32_t pa = 0, pr = 0;
+            for (uint32_t i = t; i < chunk; i += 32) { const uint32_t x = dc[i]; pa += x & 0xFFFFu; pr += x >> 16; }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) { pa += __shfl_xor_sync(0xFFFFFFFFu, pa, o); pr += __shfl_xor_sync(0xFFFFFFFFu, pr, o); }
+            if (t == 0) { s_base[0] = pa; s_base[1] = pr; }
+        }
+        __syncthreads();
+        if (t < 32) {
+            uint32_t x = s_warp[t];
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (t >= (uint32_t)o) x += y; }
+            s_warp[t] = x;
+        }
+        __syncthreads();
+        const uint32_t wex = (t >> 5) ? s_warp[(t >> 5) - 1] : 0u, ex = incl - c, wtot = __shfl_sync(0xFFFFFFFFu, incl, 31);
+        store_warp_keys(a, ex & 0xFFFFu, wtot & 0xFFFFu, word, lane, vd.dev_offsets[list] + s_base[0] + (wex & 0xFFFFu), vd.keys,
+                        vd.added, vd.added_capacity);
+        store_warp_keys(r, ex >> 16, wtot >> 16, word, lane, vd.dev_offsets[vd.lists + 1u + list] + s_base[1] + (wex >> 16), vd.keys,
+                        vd.removed, vd.removed_capacity);
+    }
+}
+
+// ------------------------------------------------------------------------------------------
 // Kernel 4b (SURVEY 8(f) N2): Clusters -> ViewClusterBindings.  The reference walks a record stream
 // (ClusterHeader, Light, Light, ..., bevy_pbr/src/cluster/mod.rs:419-470) and pushes offsets-and-counts / indices
 // one by one (:494-520, :609-697); with the CSR already on the device every output word is independent.
@@ -4391,6 +4553,18 @@ void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBuf
     if (vb.n_chunks == 0) return;
     ++g_launches; k_expand_visible<<<dim3(vb.n_chunks, max_views), kChunkWords, 0, st>>>(vb, db, row_of_rank, fc, stats, parity, n_rows);
     if (db.prev != nullptr) { ++g_launches; k_emit_visible_diff<<<dim3(vb.n_chunks, max_views), kChunkWords, 0, st>>>(vb, db, row_of_rank, fc); }
+}
+void launch_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, const uint32_t *row_of_rank,
+                      const FrameConsts *fc, uint32_t parity, uint32_t slotted_views) {
+    if (vb.n_chunks == 0 || slotted_views == 0) return;
+    ++g_launches; k_view_diff<<<dim3(vb.n_chunks, slotted_views), kChunkWords, 0, st>>>(vb, vd, vs, row_of_rank, fc, parity);
+}
+void launch_emit_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, uint32_t n_views,
+                           uint32_t slotted_views) {
+    const uint32_t n_chunks = slotted_views ? vb.n_chunks : 0u;   // no slot: every list is empty
+    ++g_launches; k_view_diff_offsets<<<1, 1024, 0, st>>>(vd, vs, n_views * 8u, n_chunks, vb.chunks_stride);
+    if (n_chunks == 0) return;
+    ++g_launches; k_emit_view_diff<<<dim3(n_chunks, slotted_views), kChunkWords, 0, st>>>(vd, vs, vb.n_words, vb.words_stride, vb.chunks_stride);
 }
 void launch_publish_visible_diff(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, uint32_t *host_rows, uint32_t host_stride,
                                  uint32_t *host_counts, uint32_t n_views, uint32_t max_views) {

@@ -28,6 +28,13 @@ void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, con
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R);
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views);
+// b200vis_set_view_diff_sink: the per-class set algebra of views 0 .. slotted_views - 1 against their slots (vs), which must
+// run before launch_expand_visible consumes the masks; then, anywhere behind it, the offsets of lists 0 .. n_views * 8
+// and the ordered emit of the added / removed Entity lists
+void launch_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, const uint32_t *row_of_rank,
+                      const FrameConsts *fc, uint32_t parity, uint32_t slotted_views);
+void launch_emit_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, uint32_t n_views,
+                           uint32_t slotted_views);
 // sink.entities != nullptr: also the Entity lists, offsets and active flags of b200vis_set_shadow_entities_sink;
 // sd.added != nullptr: also the added / removed Entity lists and offsets of b200vis_set_shadow_diff_sink
 void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,

@@ -660,6 +660,55 @@ B200VIS_API int32_t b200vis_download_visible_diff(b200vis_ctx *ctx, uint32_t vie
  * truncated (the count still says how long it was).  A result sink whose visible_rows is NULL then keeps the full
  * lists on the device.  NULL, 0, NULL removes the sink. */
 B200VIS_API int32_t b200vis_set_visible_diff_sink(b200vis_ctx *ctx, uint32_t *rows, uint32_t capacity, uint32_t *counts);
+/* The camera half of collect_visible_cpu_culled_entities (render view/visibility/mod.rs:389-431) as Entity values: one
+ * diff per (camera, VisibilityClass), against the lists last reported for that camera.  The caller gives each view a diff
+ * slot with b200vis_set_view_diff_slots: a persistent identity for one camera's RenderVisibleEntities, so the diff does
+ * not depend on the order of the view query, which may change from frame to frame.  A slot holds eight sets, one per
+ * class (bit k of b200vis_upload_bounds' class mask), with the lists last reported for it.  Every run that culls then,
+ * on the frame's tail behind the visible-list expansion (pipelined STAGE_ALL, B200VIS_PIPELINE=0, b200vis_step, CULL-only
+ * runs, more than eight views, recorded frame constants, after edits and compactions; readable after the next
+ * b200vis_synchronize):
+ *   - an active view with a slot: for each class k, added_k = list_k \ prev[slot][k] and removed_k = prev[slot][k] \
+ *     list_k, both ascending by to_bits() (MainEntity order: the march compares main entities only, mod.rs:213-231, so
+ *     pairing each entry with a render entity is the shim's job, Entity::PLACEHOLDER for meshes); then prev[slot][k] :=
+ *     list_k.  list_k is the view's VisibleEntities list of class k, as b200vis_set_visible_entities_sink writes it.
+ *   - an inactive view (B200VIS_VIEW_ACTIVE clear) with a slot: empty lists, and the slot is emptied.  The render world
+ *     removes RenderVisibleEntities from an inactive camera (render camera.rs:515-525, 549-575): when it is active again,
+ *     everything is added.
+ *   - a slot no view of the run names: emptied.
+ *   - a view without a slot: empty lists.
+ * Written, with list l = view * 8 + k for the views 0 .. n_views-1 of the frame:
+ *   added_offsets / removed_offsets[0 .. n_views*8]  exclusive prefix sums; list l of added is added[added_offsets[l] ..
+ *                            added_offsets[l+1]), likewise removed.  The last offset is the true total, even past the
+ *                            capacity; no entry at or past the capacity is written, nothing past list n_views*8.
+ *   added / removed          Entity::to_bits() of the entries.
+ * b200vis_set_topology empties every slot (the rows' identities change).  b200vis_edit_topology and
+ * b200vis_compact_topology carry the slots across: a despawned entity in a slot's set is reported removed with its own
+ * entity bits by the next run (a compaction keeps it as a tombstone until then), spawned entities are added when they
+ * are listed.  The camera diff of b200vis_enable_visible_diff is independent of this one and unchanged by it.
+ * Pinned or registered like the result sink.  Registering allocates, for max_slots slots, the eight sets per slot and
+ * their per-chunk counts, plus the run's added / removed bits and per-chunk counts: max_slots x (24 x words + 9 x
+ * chunks) x 4 bytes, words = max_entities / 32 and chunks = words / 1024 rounded up (about 3 MB per slot at one million
+ * rows), and 2 x (max_views x 8 + 1) offsets.  Every slot starts empty and no view has a slot until the slots are set.
+ * While the sink is set the entity keys stay resident on the device.  NULL removes the sink and frees the sets.
+ * Errors, with nothing changed: INVALID_ARG (a NULL pointer, a zero capacity, added / removed not 8-byte aligned),
+ * UNSUPPORTED (world_size > 1). */
+#define B200VIS_VIEW_NO_SLOT 0xFFFFFFFFu
+typedef struct b200vis_view_diff_sink {
+    uint64_t *added;            /* [added_capacity] every list's added Entity::to_bits(), back to back */
+    uint32_t  added_capacity;
+    uint64_t *removed;          /* [removed_capacity] every list's removed entries, back to back */
+    uint32_t  removed_capacity;
+    uint32_t *added_offsets;    /* [max_views * 8 + 1] */
+    uint32_t *removed_offsets;  /* [max_views * 8 + 1] */
+    uint32_t  max_slots;        /* slots are 0 .. max_slots - 1 */
+} b200vis_view_diff_sink;
+B200VIS_API int32_t b200vis_set_view_diff_sink(b200vis_ctx *ctx, const b200vis_view_diff_sink *sink);
+/* View i gets slot slots[i] (B200VIS_VIEW_NO_SLOT = none); views at or past n_views have no slot.  The map holds from the
+ * next run that culls until it is set again; a pipelined frame's tail uses the map of its own run.  Errors, with nothing
+ * changed: INVALID_ARG (n_views > max_views, slots NULL with n_views > 0, a slot >= max_slots, the same slot twice),
+ * NOT_READY (no b200vis_set_view_diff_sink registered). */
+B200VIS_API int32_t b200vis_set_view_diff_slots(b200vis_ctx *ctx, uint32_t n_views, const uint32_t *slots);
 
 /* ---- SURVEY.md 8(f) N3: shadow-view culling of point lights -------------------------------------------------------
  * check_point_light_mesh_visibility (crates/bevy_light/src/lib.rs:517-668): for every point light that is in some
