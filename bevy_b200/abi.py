@@ -397,6 +397,8 @@ _SIGNATURES = {
     "b200vis_p2p_link": (C.c_int32, [_vp, C.c_uint32]),
     "b200vis_upload_render_layers_ext": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp]),
     "b200vis_set_view_render_layers_ext": (C.c_int32, [_vp, C.c_uint32, _vp]),
+    "b200vis_set_light_render_layers_ext": (C.c_int32, [_vp, C.c_uint32, _vp]),
+    "b200vis_set_shadow_item_render_layers_ext": (C.c_int32, [_vp, C.c_uint32, _vp]),
     "b200vis_set_shadow_items": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32]),
     "b200vis_download_visible_classes": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
     "b200vis_cluster_view_dims": (C.c_int32, [_vp, C.c_uint32, _P(C.c_uint32)]),
@@ -829,6 +831,14 @@ class Context:
     def set_lights(self, light_row, light_range, layer_mask=None):
         r = _arr(light_row, np.uint32); g = _arr(light_range, np.float32); l = _arr(layer_mask, np.uint64)
         self._check(self._lib.b200vis_set_lights(self._h, len(r), _ptr(r), _ptr(g), _ptr(l)))
+        self.n_lights = len(r)
+
+    def set_light_render_layers_ext(self, blocks, n_lights=None):
+        """RenderLayers blocks 1..3 of the lights, [n_lights, 3] uint64 in set_lights order; None empties them.
+        n_lights defaults to the rows of `blocks` (to the current light count for None)."""
+        b = None if blocks is None else _arr(blocks, np.uint64).reshape(-1, 3)
+        n = (getattr(self, "n_lights", 0) if b is None else len(b)) if n_lights is None else n_lights
+        self._check(self._lib.b200vis_set_light_render_layers_ext(self._h, n, _ptr(b)))
 
     def cluster_dims(self, view):
         """Number of clusters of the view's current grid (0 = clustering off)."""
@@ -918,6 +928,7 @@ class Context:
         lm = None if layer_mask is None else np.ascontiguousarray(layer_mask, np.uint64)
         self._check(self._lib.b200vis_set_shadow_lights(self._h, len(o), _ptr(o), _ptr(fr), None if lm is None else _ptr(lm),
                                                         int(lod_origin_range_index), int(list_capacity)))
+        self.n_shadow_items = len(o)
 
     def set_shadow_items(self, items, list_capacity=0, diff_slots=None):
         """items: list of dicts(kind, light_row, range, range_view_index, layer_mask, frusta [6,6,4] or [6,4]).
@@ -936,11 +947,20 @@ class Context:
             arr[i].frusta[:] = fr.reshape(-1).tolist()
         if diff_slots is None:
             self._check(self._lib.b200vis_set_shadow_items(self._h, len(items), arr, list_capacity))
+            self.n_shadow_items = len(items)
             return
         sl = np.ascontiguousarray(diff_slots, np.uint32)
         if len(sl) < len(items):                             # the library reads diff_slots[n_items]
             raise ValueError(f"set_shadow_items: {len(sl)} diff slots for {len(items)} items")
         self._check(self._lib.b200vis_set_shadow_items_ex(self._h, len(items), arr, list_capacity, _ptr(sl)))
+        self.n_shadow_items = len(items)
+
+    def set_shadow_item_render_layers_ext(self, blocks, n_items=None):
+        """RenderLayers blocks 1..3 of the installed shadow items, [n_items, 3] uint64 in item order; None empties them.
+        n_items defaults to the rows of `blocks` (to the installed item count for None)."""
+        b = None if blocks is None else _arr(blocks, np.uint64).reshape(-1, 3)
+        n = (getattr(self, "n_shadow_items", 0) if b is None else len(b)) if n_items is None else n_items
+        self._check(self._lib.b200vis_set_shadow_item_render_layers_ext(self._h, n, _ptr(b)))
 
     def run_shadow_culling(self):
         self._check(self._lib.b200vis_run_shadow_culling(self._h))

@@ -153,6 +153,10 @@ struct b200vis_ctx {
     // lights + clusters
     std::vector<uint32_t> h_light_row; std::vector<float> h_light_range;   // host copies (b200vis_set_shadow_lights resolves ordinals)
     Lights lights{}; uint32_t *d_light_row = nullptr; float *d_light_range = nullptr; uint64_t *d_light_layers = nullptr;
+    // RenderLayers blocks 1..3 of the lights (by ordinal) and of the shadow items (by item), allocated on first use; *_ext_on:
+    // some entry is nonzero (b200vis_set_light_render_layers_ext / b200vis_set_shadow_item_render_layers_ext)
+    uint64_t *d_light_layers_ext = nullptr; bool light_ext_on = false;
+    uint64_t *d_shadow_layers_ext = nullptr; uint32_t shadow_ext_cap = 0; bool shadow_ext_on = false;
     ClusterBufs cl{}; uint32_t *d_slab = nullptr; void *ext_send = nullptr, *ext_recv = nullptr;
     size_t slab_bytes = 0;
 
@@ -271,7 +275,7 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster,
                    ctx->d_tab_range, const_cast<uint32_t *>(ctx->sdiff.slot), ctx->sdiff.prev, ctx->sdiff.prev_count,
                    ctx->sdiff.words, ctx->sdiff.chunk, ctx->sdiff.dev_offsets, ctx->vdiff.prev, ctx->vdiff.prev_count,
-                   ctx->vdiff.words, ctx->vdiff.chunk, ctx->vdiff.dev_offsets};
+                   ctx->vdiff.words, ctx->vdiff.chunk, ctx->vdiff.dev_offsets, ctx->d_light_layers_ext, ctx->d_shadow_layers_ext};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -354,8 +358,10 @@ extern "C" int32_t b200vis_create(const b200vis_config *cfg, b200vis_ctx **out) 
         CU(dalloc(&ctx->d_tile_counter, 1));
         CU(dalloc(&ctx->d_tile_ticket, 1)); CU(cudaMemset(ctx->d_tile_ticket, 0, 4));
         r.wtopo = ctx->d_wtopo;
-        // worst case tables: every view with three (kMaxClusters+1)-entry plane tables + kMaxClusters thresholds
-        ctx->blob_cap = sizeof(FrameConsts) + V * (3 * (size_t)(kMaxClusters + 1) * 16 + (size_t)kMaxClusters * 4);
+        // worst case tables: every view with three (kMaxClusters+1)-entry plane tables + kMaxClusters thresholds, and the views'
+        // RenderLayers blocks 1..3 (FrameConsts::view_ext_off)
+        ctx->blob_cap = sizeof(FrameConsts) + V * (3 * (size_t)(kMaxClusters + 1) * 16 + (size_t)kMaxClusters * 4) +
+                        sizeof(uint64_t) * 3 * kMaxCameras;
         CU(dalloc(&ctx->d_blob2[0], ctx->blob_cap)); CU(dalloc(&ctx->d_blob2[1], ctx->blob_cap)); CU(dalloc(&ctx->d_blob2[2], ctx->blob_cap));
         ctx->d_blob = ctx->d_blob2[0];
         ctx->d_consts = reinterpret_cast<FrameConsts *>(ctx->d_blob);
@@ -1876,6 +1882,7 @@ extern "C" int32_t b200vis_upload_render_layers_ext(b200vis_ctx *ctx, uint32_t f
 extern "C" int32_t b200vis_set_view_render_layers_ext(b200vis_ctx *ctx, uint32_t view, const uint64_t blocks[3]) {
     if (!ctx || view >= std::max<uint32_t>(ctx->cfg.max_views, kMaxViews)) return B200VIS_ERR_INVALID_ARG;   // views 0..7 always
     for (int k = 0; k < 3; ++k) ctx->view_layers_ext[view][k] = blocks ? blocks[k] : 0ull;
+    if (ctx->light_ext_on) ctx->consts_dirty = true;   // the cluster kernels read the views' blocks from the frame blob
     return B200VIS_OK;
 }
 extern "C" int32_t b200vis_upload_view_visibility(b200vis_ctx *ctx, uint32_t first, uint32_t count, const uint8_t *vv) {
@@ -1957,6 +1964,7 @@ extern "C" int32_t b200vis_set_lights(b200vis_ctx *ctx, uint32_t n_lights, const
     ctx->lights.n = n_lights; ctx->lights.row = ctx->d_light_row; ctx->lights.range = ctx->d_light_range;
     ctx->lights.layers = layer_mask ? ctx->d_light_layers : nullptr;
     ctx->lights_tag_dirty = true;
+    if (ctx->light_ext_on) { ctx->light_ext_on = false; ctx->consts_dirty = true; }   // every light's blocks 1..3 are empty again
     {   // the light blocks: stale snapshots out, ranges and layer masks in (rare: the tail of the frame in flight is joined first)
         const int32_t jrc = join_all(ctx); if (jrc) return jrc;
         const uint32_t cap = ctx->cl.max_lights;
@@ -1967,6 +1975,44 @@ extern "C" int32_t b200vis_set_lights(b200vis_ctx *ctx, uint32_t n_lights, const
         CU(cudaStreamSynchronize(ctx->stream));
         for (int k = 0; k < 3; ++k) CU(cudaMemcpy(ctx->d_lrec + k * ctx->lrec_bytes, blk.data(), ctx->lrec_bytes, cudaMemcpyHostToDevice));
     }
+    return B200VIS_OK;
+}
+
+// blocks[n][3] -> dev (allocated with `cap` entries on first use); returns whether any block is nonzero
+static int32_t upload_layer_blocks(b200vis_ctx *ctx, uint64_t **dev, uint32_t cap, uint32_t n, const uint64_t *blocks, bool *any) {
+    *any = false;
+    for (size_t i = 0; blocks && i < (size_t)n * 3; ++i) *any = *any || blocks[i] != 0ull;
+    if (!*any) return B200VIS_OK;
+    CU(cudaStreamSynchronize(ctx->stream));     // no kernel of the context still reads the old blocks
+    if (!*dev) CU(dalloc(dev, (size_t)std::max<uint32_t>(cap, 1) * 3));
+    CU(cudaMemcpy(*dev, blocks, (size_t)n * 24, cudaMemcpyHostToDevice));
+    return B200VIS_OK;
+}
+extern "C" int32_t b200vis_set_light_render_layers_ext(b200vis_ctx *ctx, uint32_t n_lights, const uint64_t *blocks) {
+    CHECK_CTX_JOIN();   // the frame in flight may still be reading the lights' blocks
+    if (ctx->cfg.world_size > 1)
+        return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_light_render_layers_ext: world_size > 1 (the light records carry block 0 only)");
+    if (n_lights != ctx->lights.n)
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_light_render_layers_ext: %u lights, b200vis_set_lights gave %u", n_lights, ctx->lights.n);
+    bool any = false;
+    const int32_t rc = upload_layer_blocks(ctx, &ctx->d_light_layers_ext, ctx->cfg.max_lights, n_lights, blocks, &any); if (rc) return rc;
+    if (any != ctx->light_ext_on) ctx->consts_dirty = true;   // the frame blob gains / drops the views' blocks
+    ctx->light_ext_on = any;
+    return B200VIS_OK;
+}
+extern "C" int32_t b200vis_set_shadow_item_render_layers_ext(b200vis_ctx *ctx, uint32_t n_items, const uint64_t *blocks) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "set_shadow_item_render_layers_ext: world_size > 1");
+    if (n_items != ctx->shadow.n_lights)
+        return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_shadow_item_render_layers_ext: %u items, %u installed", n_items, ctx->shadow.n_lights);
+    if (ctx->d_shadow_layers_ext && ctx->shadow_ext_cap < n_items) {   // the item capacity grew since the array was made
+        CU(cudaStreamSynchronize(ctx->stream));
+        CU(cudaFree(ctx->d_shadow_layers_ext)); ctx->d_shadow_layers_ext = nullptr;
+    }
+    if (!ctx->d_shadow_layers_ext) ctx->shadow_ext_cap = ctx->shadow_cap_lights;
+    bool any = false;
+    const int32_t rc = upload_layer_blocks(ctx, &ctx->d_shadow_layers_ext, ctx->shadow_ext_cap, n_items, blocks, &any); if (rc) return rc;
+    ctx->shadow_ext_on = any;
     return B200VIS_OK;
 }
 
@@ -2021,6 +2067,12 @@ static int32_t flush_consts(b200vis_ctx *ctx) {
             memcpy(h + off, tabs[k]->data(), tabs[k]->size() * 4);
             off += (tabs[k]->size() * 4 + 15) & ~(size_t)15;
         }
+    }
+    ctx->consts.view_ext_off = 0;
+    if (ctx->light_ext_on) {   // the views' RenderLayers blocks 1..3, for the lights that have some (k_cluster_assign<true>)
+        ctx->consts.view_ext_off = (uint32_t)(off / 4);
+        memcpy(h + off, ctx->view_layers_ext, sizeof ctx->view_layers_ext);
+        off += (sizeof ctx->view_layers_ext + 15) & ~(size_t)15;
     }
     memcpy(h, &ctx->consts, sizeof(FrameConsts));
     CU(cudaMemcpyAsync(ctx->d_blob, h, off, cudaMemcpyHostToDevice, ctx->stream));
@@ -2413,6 +2465,9 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     }
     Lights lights = ctx->lights;
     lights.snap = nullptr;
+    // lights with RenderLayers blocks 1..3: only with the views' blocks in this frame's constants (a frame recorded before the
+    // light blocks were set has none, and its views then see block 0 alone)
+    lights.layers_ext = ctx->light_ext_on && afc.view_ext_off ? ctx->d_light_layers_ext : nullptr;
     cudaStream_t tail = st;
     if (pipelined) {
         lights.snap = ctx->light_snap_slot(cslot);
@@ -2702,6 +2757,7 @@ static int32_t install_shadow_items(b200vis_ctx *ctx, uint32_t n_items, uint32_t
         ctx->shadow_cap_lights = (uint32_t)nl; ctx->shadow_cap_list = (uint32_t)lc;
     }
     if (n_items) CU(cudaMemcpy(ctx->d_shadow_lights, ctx->h_shadow.data(), n_items * sizeof(ShadowLight), cudaMemcpyHostToDevice));
+    ctx->shadow_ext_on = false;                 // every item's RenderLayers blocks 1..3 are empty again
     ctx->shadow.n_lights = n_items; ctx->shadow.lights = ctx->d_shadow_lights; ctx->shadow.caster = ctx->d_caster;
     ctx->shadow.list_cap = ctx->shadow_cap_list;
     if (ctx->sdiff.added) {
@@ -2813,6 +2869,10 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     R.row_of_rank = ctx->rank_identity ? nullptr : ctx->d_row_of_rank;
     ShadowBufs sb = ctx->shadow;
     sb.has_ranges = ctx->have_range ? 1u : 0u;
+    if (ctx->shadow_ext_on && ctx->have_layers_ext) {   // blocks 1..3 on both sides: k_shadow_cull<true>
+        sb.layers_ext = ctx->d_shadow_layers_ext;
+        R.layers_ext = ctx->d_layers_ext;
+    }
     CU(cudaMemsetAsync(sb.chunk_count, 0, (size_t)sb.n_lights * 6 * ctx->vis.chunks_stride * 4, st));
     ShadowSink sink = ctx->shsink;
     sink.keys = ctx->d_keys;                    // a compaction swaps the key buffers

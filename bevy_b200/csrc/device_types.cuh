@@ -121,7 +121,10 @@ struct DevClusterView {
 };
 
 struct FrameConsts {
-    uint32_t n_views, pad[3];
+    uint32_t n_views;
+    uint32_t view_ext_off;   // offset (in floats) of the views' RenderLayers blocks 1..3 [kMaxCameras][3] in the frame blob;
+                             //   0 = not packed (no light has blocks 1..3, b200vis_set_light_render_layers_ext)
+    uint32_t pad[2];
     DevView views[kMaxCameras];
     DevClusterView cviews[kMaxCameras];
 };
@@ -178,6 +181,7 @@ struct Lights {
     // (28 bytes per light: what assign_objects_to_clusters needs of a light).  per_rank == 0: the flat arrays above.
     uint32_t per_rank, block_bytes;
     const uint8_t *blocks;
+    const uint64_t *layers_ext;  // [n][3] RenderLayers blocks 1..3 by ordinal (flat arrays only), or nullptr: block 0 alone decides
 };
 #ifdef __CUDACC__
 __device__ __forceinline__ float4 light_snap_of(const Lights &L, uint32_t li) {
@@ -240,6 +244,8 @@ struct ShadowBufs {
     uint32_t *count;         // [n_lights * 6]
     uint32_t list_cap;
     uint32_t *active;        // [n_lights]: the light is in some view's VisibleEntities (written by k_shadow_select)
+    const uint64_t *layers_ext;  // [n_lights][3] the items' RenderLayers blocks 1..3, or nullptr when no item has one (or no row
+                                 //   has blocks uploaded): kept out of ShadowLight, which is staged in shared memory
 };
 // b200vis_set_shadow_entities_sink as the shadow stage sees it (entities == nullptr: no sink)
 struct ShadowSink {

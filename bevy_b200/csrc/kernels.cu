@@ -2613,6 +2613,16 @@ __device__ __forceinline__ bool assign_one_light(const DevClusterView &cv, const
     return true;
 }
 
+// RenderLayers::intersects (render_layers.rs:121-135) past block 0, for a light of the flat arrays: blocks 1..3 of light li
+// (Lights::layers_ext) against those of view v, packed into the frame blob at FrameConsts::view_ext_off
+__device__ __forceinline__ bool light_layers_ext_intersect(const Lights &L, const FrameConsts *fc, uint32_t v, uint32_t li) {
+    const uint64_t *e = L.layers_ext + (size_t)li * 3;
+    const uint64_t *w = reinterpret_cast<const uint64_t *>(reinterpret_cast<const float *>(fc) + fc->view_ext_off) + (size_t)v * 3;
+    return ((e[0] & w[0]) | (e[1] & w[1]) | (e[2] & w[2])) != 0ull;
+}
+
+// EXT: some light has RenderLayers blocks 1..3 (L.layers_ext != nullptr).  The <false> instantiation is the block-0 kernel.
+template <bool EXT>
 __global__ void __launch_bounds__(256)
 k_cluster_assign(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBufs cb, DevStats *__restrict__ stats) {
     __shared__ float4 s_planes[kStagedPlanes];
@@ -2647,7 +2657,7 @@ k_cluster_assign(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBu
         px = R.gt0[row].w; py = R.gt1[row].w; pz = R.gt2[row].w;        // GlobalTransform::translation
     }
     const unsigned long long ll = L.layers ? L.layers[li] : 1ull;
-    if (!(cv.layer_mask & ll)) return;                                  // assign.rs:489
+    if (!(cv.layer_mask & ll) && !(EXT && light_layers_ext_intersect(L, fc, v, li))) return;   // assign.rs:489
     const float range = L.range[li];
     ClusterTables tb;
     tb.thr = staged ? s_thr : cb.blob + cv.thr_off;
@@ -2699,6 +2709,7 @@ __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t *p) {
     asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
     return v;
 }
+template <bool EXT>   // as k_cluster_assign; EXT is never set for the gathered light records (per_rank)
 __global__ void __launch_bounds__(kFusedThreads)
 k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBufs cb, DevStats *__restrict__ stats) {
     extern __shared__ __align__(16) uint8_t smem_fused[];
@@ -2761,7 +2772,7 @@ k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBuf
             px = R.gt0[row].w; py = R.gt1[row].w; pz = R.gt2[row].w;
         }
         const unsigned long long ll = light_layers_of(L, li);
-        if (!(cv.layer_mask & ll)) continue;                                // assign.rs:489
+        if (!(cv.layer_mask & ll) && !(EXT && light_layers_ext_intersect(L, fc, v, li))) continue;   // assign.rs:489
         const uint32_t bit = 1u << (li & 31u), wbase = (li >> 5) * per;
         uint32_t count = 0;
         float this_far = 0.0f;
@@ -3459,6 +3470,9 @@ __global__ void k_shadow_select(ShadowBufs sb, const uint32_t *__restrict__ rank
     for (uint32_t v = 0; v < n_views; ++v) on |= (view_sets[(size_t)v * words_stride + (rk >> 5)] >> (rk & 31u)) & 1u;
     sb.active[s] = on;
 }
+// EXT: some item has RenderLayers blocks 1..3 (sb.layers_ext) and the rows have theirs (R.layers_ext): the layer gate is the
+// whole RenderLayers::intersects (render_layers.rs:121-135).  The <false> instantiation is the block-0 kernel.
+template <bool EXT>
 __global__ void __launch_bounds__(256)
 k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stride, DevStats *__restrict__ stats,
               uint32_t changed_slot) {
@@ -3471,7 +3485,7 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
     Aff g; g.r0 = g.r1 = g.r2 = make_float4(0, 0, 0, 0);
     float4 bA = g.r0; float2 bB = make_float2(0, 0);
     bool eligible = false;
-    unsigned long long elayers = 1ull;
+    unsigned long long elayers = 1ull, ex0 = 0ull, ex1 = 0ull, ex2 = 0ull;   // ex*: the row's blocks 1..3 (EXT only)
     uint32_t rnk = row;
     if (active) {
         f = R.flags[row]; st8 = R.state[row];
@@ -3480,6 +3494,7 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
             g.r0 = R.gt0[row]; g.r1 = R.gt1[row]; g.r2 = R.gt2[row];
             bA = R.bndA[row]; bB = R.bndB[row];
             if (R.layers != nullptr) elayers = R.layers[row];
+            if (EXT) { const uint64_t *e = R.layers_ext + (size_t)row * 3; ex0 = e[0]; ex1 = e[1]; ex2 = e[2]; }
             if ((f & F_RANGE) && sb.has_ranges && R.range != nullptr) erange = R.range[row];
         }
         if (R.rank != nullptr) rnk = R.rank[row];
@@ -3578,6 +3593,10 @@ k_shadow_cull(Rows R, ShadowBufs sb, uint32_t words_stride, uint32_t chunks_stri
             const ShadowLight &sl = s_light[i];
             const uint32_t kind = sl.kind, n_faces = kind == 0u ? 6u : 1u;
             bool in = eligible && (sl.layers & elayers) != 0ull;
+            if (EXT && eligible && !in) {                            // lib.rs:437, 611, 703: the blocks past the first
+                const uint64_t *x = sb.layers_ext + (size_t)s0 * 3;
+                in = ((x[0] & ex0) | (x[1] & ex1) | (x[2] & ex2)) != 0ull;
+            }
             if (in && ranged) in = sl.range_index >= 0 && sl.range_index < 32 && ((erange >> sl.range_index) & 1u);
             uint32_t faces = kind == 0u ? 0x3Fu : 1u;                // no Aabb: pushed to every list of the item (lib.rs:639-645)
             if (in && has_aabb && !no_fc) {
@@ -4574,7 +4593,9 @@ void launch_publish_visible_diff(cudaStream_t st, const VisibleBufs &vb, const D
 void launch_cluster_assign(cudaStream_t st, const Rows &R, const Lights &L, const FrameConsts *fc, const ClusterBufs &cb,
                            DevStats *stats, uint32_t max_views) {
     if (L.n == 0) return;
-    ++g_launches; k_cluster_assign<<<dim3(cdiv(L.n, 8), max_views), 256, 0, st>>>(R, L, fc, cb, stats);
+    ++g_launches;
+    if (L.layers_ext != nullptr) k_cluster_assign<true><<<dim3(cdiv(L.n, 8), max_views), 256, 0, st>>>(R, L, fc, cb, stats);
+    else k_cluster_assign<false><<<dim3(cdiv(L.n, 8), max_views), 256, 0, st>>>(R, L, fc, cb, stats);
 }
 // assign + lists of every view in one launch (single GPU): thread-block clusters of 8 (16 beyond ~3200 lights) CTAs per view
 // Can the one-launch cluster stage hold `n_lights` mask bits per cluster in a thread-block cluster's shared memory?
@@ -4595,9 +4616,12 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
         nrank_env = r ? atoi(r) : 0;
     }
     if (first_call_on_device(seen)) {
-        cudaFuncSetAttribute(k_cluster_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
-        cudaFuncSetAttribute(k_cluster_fused, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        for (const void *k : {(const void *)k_cluster_fused<false>, (const void *)k_cluster_fused<true>}) {
+            cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024);
+            cudaFuncSetAttribute(k, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+        }
     }
+    const bool ext = L.layers_ext != nullptr;
     if (!enabled) return false;
     const uint32_t words = (L.n + 31u) / 32u;
     // every CTA popcounts, scans and emits its kMaxClusters / nrank owned clusters with one thread each: nrank >= 4
@@ -4615,18 +4639,22 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
     // Whether the device can co-schedule nrank CTAs of ~200 KB shared memory each (16 is a non-portable cluster size) is
     // asked once per cluster size at the largest shared-memory footprint; a size it cannot hold goes to the split path.
     // A refusal by the runtime is not the frame's error (the caller falls back to the split kernels): it is cleared again.
-    static int schedulable[17] = {};           // 0 unknown, 1 yes, -1 no
-    if (schedulable[nrank] == 0) {
+    static int schedulable[2][17] = {};        // [EXT][nrank]: 0 unknown, 1 yes, -1 no
+    int &sched = schedulable[ext ? 1 : 0][nrank];
+    if (sched == 0) {
         cudaLaunchConfig_t probe = cfg;
         probe.dynamicSmemBytes = 200u * 1024u;
         int n_clusters = 0;
-        const cudaError_t e = cudaOccupancyMaxActiveClusters(&n_clusters, k_cluster_fused, &probe);
-        schedulable[nrank] = (e == cudaSuccess && n_clusters > 0) ? 1 : -1;
+        const cudaError_t e = ext ? cudaOccupancyMaxActiveClusters(&n_clusters, k_cluster_fused<true>, &probe)
+                                  : cudaOccupancyMaxActiveClusters(&n_clusters, k_cluster_fused<false>, &probe);
+        sched = (e == cudaSuccess && n_clusters > 0) ? 1 : -1;
         if (e != cudaSuccess) (void)cudaGetLastError();
     }
-    if (schedulable[nrank] < 0) return false;
+    if (sched < 0) return false;
     ++g_launches;
-    if (cudaLaunchKernelEx(&cfg, k_cluster_fused, R, L, fc, cb, stats) == cudaSuccess) return true;
+    const cudaError_t le = ext ? cudaLaunchKernelEx(&cfg, k_cluster_fused<true>, R, L, fc, cb, stats)
+                               : cudaLaunchKernelEx(&cfg, k_cluster_fused<false>, R, L, fc, cb, stats);
+    if (le == cudaSuccess) return true;
     (void)cudaGetLastError();
     return false;
 }
@@ -4654,7 +4682,9 @@ void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, co
         if (diff) { ++g_launches; k_shadow_diff_offsets<<<1, 1024, 0, st>>>(sb, sd, 0u, chunks_stride); }
         return;
     }
-    ++g_launches; k_shadow_cull<<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
+    ++g_launches;
+    if (sb.layers_ext != nullptr) k_shadow_cull<true><<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
+    else k_shadow_cull<false><<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
     const dim3 grid(n_chunks, sb.n_lights);
     if (sink.entities != nullptr) { ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active); }
     ++g_launches;

@@ -311,9 +311,11 @@ B200VIS_API int32_t b200vis_upload_bounds(b200vis_ctx *ctx, uint32_t first_row, 
                               const uint32_t *range_mask);
 /* ViewVisibility column (bit0 current, bit1 previous; visibility/mod.rs:226-242) */
 /* RenderLayers beyond the first 64 layers: the component is a SmallVec of 64-bit blocks (render_layers.rs:20-23) and
- * intersects() ORs the block-wise ANDs (:121-135).  Block 0 is the layer_mask of b200vis_upload_bounds / b200vis_view;
- * blocks[count][3] / blocks[3] are blocks 1..3 (layers 64..255) of the rows / of a view.  Lights keep to block 0
- * (b200vis_set_lights, shadow items). */
+ * intersects() ORs the block-wise ANDs over the blocks both sides have (:121-135).  Block 0 is the layer_mask of
+ * b200vis_upload_bounds / b200vis_view / b200vis_camera; blocks[count][3] / blocks[3] are blocks 1..3 (layers 64..255) of
+ * the rows / of a view.  A view's blocks serve both its camera cull and its cluster view (the camera of view v is the
+ * same camera in both stages).  Lights and shadow items take theirs from b200vis_set_light_render_layers_ext and
+ * b200vis_set_shadow_item_render_layers_ext; until then they have block 0 only. */
 B200VIS_API int32_t b200vis_upload_render_layers_ext(b200vis_ctx *ctx, uint32_t first_row, uint32_t count, const uint64_t *blocks);
 B200VIS_API int32_t b200vis_set_view_render_layers_ext(b200vis_ctx *ctx, uint32_t view, const uint64_t blocks[3]);
 B200VIS_API int32_t b200vis_upload_view_visibility(b200vis_ctx *ctx, uint32_t first_row, uint32_t count, const uint8_t *vv);
@@ -324,9 +326,18 @@ B200VIS_API int32_t b200vis_set_static_transform_optimizations(b200vis_ctx *ctx,
 /* ---- per-frame constants ----------------------------------------------------- */
 B200VIS_API int32_t b200vis_set_views(b200vis_ctx *ctx, uint32_t n_views, const b200vis_view *views);
 /* PointLight set (point_lights_query, assign.rs:146-153): light_row = the light entity's row (its
- * GlobalTransform translation and ViewVisibility are read on the device), in query order. */
+ * GlobalTransform translation and ViewVisibility are read on the device), in query order.  layer_mask = block 0 of each
+ * light's RenderLayers (NULL = the default layer); the call empties every light's blocks 1..3. */
 B200VIS_API int32_t b200vis_set_lights(b200vis_ctx *ctx, uint32_t n_lights, const uint32_t *light_row, const float *range,
                            const uint64_t *layer_mask /* nullable */);
+/* RenderLayers blocks 1..3 (layers 64..255) of the clustered lights: blocks[n_lights][3] in b200vis_set_lights ordinal
+ * order, NULL = all empty.  Call it after b200vis_set_lights, which empties them again.  The cluster stage then tests the
+ * light's whole RenderLayers against its view's (assign.rs:489, render_layers.rs:121-135): block 0 against the layer_mask
+ * of the cluster view, blocks 1..3 against the view's b200vis_set_view_render_layers_ext blocks.  Frame constants recorded
+ * (b200vis_record_frame_constants) while no light had blocks 1..3 replay with block 0 only.
+ * Errors: INVALID_ARG (n_lights is not the current light count), UNSUPPORTED (world_size > 1: the light records that
+ * travel between ranks carry block 0 only); nothing changes then. */
+B200VIS_API int32_t b200vis_set_light_render_layers_ext(b200vis_ctx *ctx, uint32_t n_lights, const uint64_t *blocks);
 B200VIS_API int32_t b200vis_set_cluster_view(b200vis_ctx *ctx, uint32_t view, const b200vis_cluster_view *params);
 /* Cluster grid dimensions of the view as last set (b200vis_set_cluster_view / b200vis_update_camera / b200vis_step);
  * zeros when clustering is off for the view.  The shim sizes Clusters::clusterable_objects from it. */
@@ -751,10 +762,17 @@ typedef struct b200vis_shadow_item {
     uint32_t light_row;          /* point / spot */
     float    range;              /* point / spot: PointLight::range / SpotLight::range */
     int32_t  range_view_index;
-    uint64_t layer_mask;         /* the light's RenderLayers (first block; default layer = 1) */
+    uint64_t layer_mask;         /* the light's RenderLayers, block 0 (default layer = 1); blocks 1..3:
+                                    b200vis_set_shadow_item_render_layers_ext */
     float    frusta[6][6][4];    /* point: the six CubemapFrusta faces; spot / cascade: frusta[0] */
 } b200vis_shadow_item;
 B200VIS_API int32_t b200vis_set_shadow_items(b200vis_ctx *ctx, uint32_t n_items, const b200vis_shadow_item *items, uint32_t list_capacity);
+/* RenderLayers blocks 1..3 (layers 64..255) of the installed shadow items: blocks[n_items][3] in item order, NULL = all
+ * empty.  Call it after b200vis_set_shadow_items / _ex / b200vis_set_shadow_lights, each of which empties them again.  The
+ * shadow cull then tests the light's whole RenderLayers against each row's (lib.rs:437, 611, 703; render_layers.rs:121-135):
+ * block 0 against the rows' layer_mask, blocks 1..3 against their b200vis_upload_render_layers_ext blocks.
+ * Errors: INVALID_ARG (n_items is not the installed item count), UNSUPPORTED (world_size > 1); nothing changes then. */
+B200VIS_API int32_t b200vis_set_shadow_item_render_layers_ext(b200vis_ctx *ctx, uint32_t n_items, const uint64_t *blocks);
 B200VIS_API int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx);
 B200VIS_API int32_t b200vis_download_shadow_visible(b200vis_ctx *ctx, uint32_t shadow_light, uint32_t face, uint32_t *rows,
                                                     uint32_t capacity, uint32_t *count);

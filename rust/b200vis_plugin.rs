@@ -20,7 +20,8 @@
 //! InheritedVisibility and VisibilityRange read by the device straight from the archetype tables by their change ticks
 //! (`b200vis_set_tables_ex`, `b200vis_set_table_cull_inputs`, `b200vis_set_table_visibility_ranges`,
 //! `b200vis_read_tables`), the range masks evaluated on the device; VisibilityClass and RenderLayers -> `upload_bounds`
-//! on change; results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
+//! on change (blocks 1..3, layers 64..255, with `upload_render_layers_ext`, `set_view_render_layers_ext` and
+//! `set_light_render_layers_ext`; a layer past 255 is an error); results -> pinned host buffers the GPU writes itself (`b200vis_set_result_sink`,
 //! and VisibleEntities as per-class Entity lists through `b200vis_set_visible_entities_sink`), read after one
 //! `b200vis_synchronize` per system; GlobalTransform and ViewVisibility with their change ticks straight into the archetype
 //! tables (`b200vis_writeback_tables`).
@@ -87,6 +88,9 @@ extern "C" {
     fn b200vis_upload_bounds(ctx: *mut b200vis_ctx, first: u32, count: u32, bounds: *const f32, flags: *const u8, class_mask: *const u8,
                              layer_mask: *const u64, range_mask: *const u32) -> i32;
     fn b200vis_upload_view_visibility(ctx: *mut b200vis_ctx, first: u32, count: u32, vv: *const u8) -> i32;
+    fn b200vis_upload_render_layers_ext(ctx: *mut b200vis_ctx, first: u32, count: u32, blocks: *const [u64; 3]) -> i32;
+    fn b200vis_set_view_render_layers_ext(ctx: *mut b200vis_ctx, view: u32, blocks: *const [u64; 3]) -> i32;
+    fn b200vis_set_light_render_layers_ext(ctx: *mut b200vis_ctx, n: u32, blocks: *const [u64; 3]) -> i32;
     fn b200vis_set_static_transform_optimizations(ctx: *mut b200vis_ctx, enabled: i32) -> i32;
     fn b200vis_set_views(ctx: *mut b200vis_ctx, n: u32, views: *const b200vis_view) -> i32;
     fn b200vis_set_lights(ctx: *mut b200vis_ctx, n: u32, light_row: *const u32, range: *const f32, layers: *const u64) -> i32;
@@ -149,6 +153,8 @@ pub struct B200Vis {
     table_entities: Vec<Vec<Entity>>, maps_epoch: u64,
     // the tables' VisibilityRange columns, attached while the VisibleEntityRanges resource exists (None = detached)
     table_ranges: Option<Vec<b200vis_table_visibility_ranges>>,
+    // some row has had a RenderLayers layer in 64..255: the rows' blocks 1..3 are uploaded with their block 0 from then on
+    rows_ext: bool,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -194,7 +200,7 @@ impl Plugin for B200VisibilityPlugin {
             entity_offsets: vec![[0; 9]; max_views],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
             planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_cull: Vec::new(), table_entities: Vec::new(),
-            maps_epoch: u64::MAX, table_ranges: None,
+            maps_epoch: u64::MAX, table_ranges: None, rows_ext: false,
         };
         // the sorted row lists stay on the device: VisibleEntities arrives as Entity values through the entities sink, and
         // GlobalTransform and ViewVisibility go straight into the archetype tables (b200vis_set_tables)
@@ -231,6 +237,20 @@ impl Plugin for B200VisibilityPlugin {
         ));
     }
 }
+
+/// Blocks 0..3 (layers 0..255) of an entity's RenderLayers (render_layers.rs:20-23; none = the default layer 0).  The device
+/// holds four blocks: a set layer past 255 is an error that names the entity, not a silent truncation.
+fn layer_blocks(entity: Entity, layers: Option<&RenderLayers>) -> Result<[u64; 4], BevyError> {
+    let Some(l) = layers else { return Ok([1, 0, 0, 0]) };
+    let bits = l.bits();
+    if bits.iter().skip(4).any(|&w| w != 0) {
+        return Err(format!("{entity}: {l:?} has a layer past 255; the device holds RenderLayers 0..=255").into());
+    }
+    let mut out = [0u64; 4];
+    for (o, w) in out.iter_mut().zip(bits) { *o = *w; }
+    Ok(out)
+}
+fn ext_of(b: &[u64; 4]) -> [u64; 3] { [b[1], b[2], b[3]] }
 
 fn pack_trs(t: &Transform, out: &mut Vec<f32>) {
     out.extend_from_slice(&[t.translation.x, t.translation.y, t.translation.z, t.rotation.x, t.rotation.y, t.rotation.z, t.rotation.w,
@@ -465,10 +485,12 @@ fn b200_check_visibility(
         vis.check(unsafe { b200vis_set_visibility_range_views(vis.ctx, range_entities.len() as u32, range_pos.as_ptr()) })?;
     }
     // ---- views: half spaces copied verbatim from `Frustum` (bit-identical by construction) ----
-    let mut views = Vec::new();
+    let (mut views, mut view_ext) = (Vec::new(), Vec::new());
     vis.view_entities.clear();
     for (entity, _, frustum, layers, camera, no_cpu_culling) in view_query.iter() {
-        let mut v = b200vis_view { half_spaces: [[0.0; 4]; 6], layer_mask: layers.map_or(1, |l| l.bits()[0]),
+        let blocks = layer_blocks(entity, layers)?;
+        view_ext.push(ext_of(&blocks));
+        let mut v = b200vis_view { half_spaces: [[0.0; 4]; 6], layer_mask: blocks[0],
                                    flags: (camera.is_active as u8 * VIEW_ACTIVE) | (no_cpu_culling as u8 * VIEW_NO_CPU_CULLING),
                                    range_view_index: -1, pad: [0; 6] };
         for (k, hs) in frustum.half_spaces.iter().enumerate() { v.half_spaces[k] = hs.normal_d().to_array(); }
@@ -479,6 +501,10 @@ fn b200_check_visibility(
         if views.len() == vis.max_views { break; }
     }
     vis.check(unsafe { b200vis_set_views(vis.ctx, views.len() as u32, views.as_ptr()) })?;
+    // blocks 1..3 of every view: its camera cull here, its cluster view in b200_assign_lights_to_clusters (same view index)
+    for (v, ext) in view_ext.iter().enumerate() {
+        vis.check(unsafe { b200vis_set_view_render_layers_ext(vis.ctx, v as u32, ext) })?;
+    }
     // ---- VisibilityClass and RenderLayers (which the device cannot read from the tables): every row after a renumbering,
     // otherwise only the rows whose class or layers changed, as contiguous ranges.
     // upload_bounds also takes the rows' current bounds and flags; the table read below, enqueued after it, then brings
@@ -492,6 +518,7 @@ fn b200_check_visibility(
     dirty.dedup();
     let k = dirty.len();
     let (mut bounds, mut flags, mut class, mut layer) = (vec![0f32; k * 6], vec![F_NO_CPU_CULLING; k], vec![0u8; k], vec![1u64; k]);
+    let mut layer_ext = vec![[0u64; 3]; k];
     for (i, &r) in dirty.iter().enumerate() {
         let e = vis.entity_of[r as usize];
         // a row outside visible_aabb_query stays NO_CPU_CULLING, as its table's cull inputs say
@@ -504,14 +531,20 @@ fn b200_check_visibility(
         }
         flags[i] = f;
         class[i] = vclass.as_ref().map_or(0, |c| c.iter().fold(0u8, |m, id| m | vis.class_bit(*id)));
-        layer[i] = layers.as_ref().map_or(1, |l| l.bits()[0]);
+        let blocks = layer_blocks(e, layers.as_deref())?;
+        layer[i] = blocks[0]; layer_ext[i] = ext_of(&blocks);
     }
+    // blocks 1..3 go to the device once some row uses them (the cull's block-0 path serves everyone else)
+    vis.rows_ext |= layer_ext.iter().any(|b| b.iter().any(|&w| w != 0));
     let mut i = 0;
     while i < k {                                               // coalesce into [first, first + count) ranges
         let mut j = i + 1;
         while j < k && dirty[j] == dirty[j - 1] + 1 { j += 1; }
         vis.check(unsafe { b200vis_upload_bounds(vis.ctx, dirty[i], (j - i) as u32, bounds[i * 6..].as_ptr(), flags[i..].as_ptr(),
             class[i..].as_ptr(), layer[i..].as_ptr(), core::ptr::null()) })?;
+        if vis.rows_ext {
+            vis.check(unsafe { b200vis_upload_render_layers_ext(vis.ctx, dirty[i], (j - i) as u32, layer_ext[i..].as_ptr()) })?;
+        }
         i = j;
     }
     // Aabb, Sphere, InheritedVisibility and VisibilityRange straight from the tables, by this system's own change ticks;
@@ -577,12 +610,17 @@ fn b200_assign_lights_to_clusters(
         || point_lights_query.iter().any(|(_, _, _, l, r)| l.is_changed() || r.is_some_and(|r| r.is_changed()));
     if lights_changed {
         vis.light_entities.clear();
-        let (mut rows, mut ranges, mut layers) = (Vec::new(), Vec::new(), Vec::new());
+        let (mut rows, mut ranges, mut layers, mut ext) = (Vec::new(), Vec::new(), Vec::new(), Vec::new());
         for (e, _, _, light, layer) in point_lights_query.iter() {
             let Some(&r) = vis.row_of.get(&e) else { continue };
-            vis.light_entities.push(e); rows.push(r); ranges.push(light.range); layers.push(layer.map_or(1, |l| l.bits()[0]));
+            let blocks = layer_blocks(e, layer.as_deref())?;
+            vis.light_entities.push(e); rows.push(r); ranges.push(light.range); layers.push(blocks[0]); ext.push(ext_of(&blocks));
         }
         vis.check(unsafe { b200vis_set_lights(vis.ctx, rows.len() as u32, rows.as_ptr(), ranges.as_ptr(), layers.as_ptr()) })?;
+        // set_lights emptied the lights' blocks 1..3: give them again where some light has a layer in 64..255
+        if ext.iter().any(|b| b.iter().any(|&w| w != 0)) {
+            vis.check(unsafe { b200vis_set_light_render_layers_ext(vis.ctx, ext.len() as u32, ext.as_ptr()) })?;
+        }
         vis.lights_epoch = vis.columns_epoch;
     }
     // ---- per view: the prologue of assign_objects_to_clusters (assign.rs:324-485) through the library's host helper, which
@@ -613,7 +651,8 @@ fn b200_assign_lights_to_clusters(
         let hs: Vec<[f32; 4]> = frustum.half_spaces.iter().map(|h| h.normal_d().to_array()).collect();
         let mut cv = core::mem::MaybeUninit::<b200vis_cluster_view>::zeroed();
         unsafe {
-            vis.check(b200vis_host_cluster_view_setup(&cfg, gt12.as_ptr(), cfv.as_ptr(), hs.as_ptr(), layers.map_or(1, |l| l.bits()[0]), &fb,
+            // block 0 here; blocks 1..3 are the view's, set by b200_check_visibility for the same view index
+            vis.check(b200vis_host_cluster_view_setup(&cfg, gt12.as_ptr(), cfv.as_ptr(), hs.as_ptr(), layer_blocks(entity, layers)?[0], &fb,
                                                       vis.planes_scratch.as_mut_ptr(), cv.as_mut_ptr()))?;
             vis.check(b200vis_set_cluster_view(vis.ctx, v as u32, cv.as_ptr()))?;
             order.push((entity, v, cv.assume_init()));
