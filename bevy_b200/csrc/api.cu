@@ -95,6 +95,10 @@ struct b200vis_ctx {
     WarpTile *d_wtiles = nullptr; uint8_t *d_sched = nullptr; uint32_t *d_wtopo = nullptr;   // k_tile_warp's view of the plan
     uint32_t *d_tile_counter = nullptr;
     uint32_t *d_tile_ticket = nullptr; uint32_t tile_ticket_base = 0;   // dynamic tile hand-out of the default kernel: never reset, the host tracks the base
+    // Full-world sweeps launched so far: every kernel 1b launch over a pass and every k_cull launch counts one.  Each sweep
+    // walks the rows opposite to the previous one (next_sweep_reversed), so it starts on the rows the previous sweep touched
+    // last, which are the ones still in L2.  Any order gives the same results; only the parity matters.
+    uint32_t sweep_count = 0;
     std::vector<uint32_t> pass_begin;   // tile index ranges per pass: [pass_begin[p], pass_begin[p+1])
     std::vector<uint32_t> pass_small;   // the first pass_small[p] tiles of pass p have <= 32 rows (B200VIS_SPLIT_DEEP_TILES)
     std::vector<uint8_t> pass_named;    // every tile of pass p is flat or walks with named level barriers (Tile::lvl_warps): the tile kernel may let a CTA's warps drift a tile apart
@@ -2324,6 +2328,19 @@ static int32_t view_diff_slots_of_run(b200vis_ctx *ctx, cudaStream_t tail, uint3
     return B200VIS_OK;
 }
 
+// B200VIS_SWEEP_ORDER=fixed (experiment switch, read once per process): every sweep walks the rows in ascending order
+static bool sweep_order_fixed() {
+    static int v = -1;
+    if (v < 0) { const char *e = getenv("B200VIS_SWEEP_ORDER"); v = (e && e[0] == 'f') ? 1 : 0; }
+    return v != 0;
+}
+// Direction of the context's next full-world sweep: 0 ascending rows, 1 descending, alternating from sweep to sweep.  L2 holds
+// about the last 40 MB a sweep touched; a sweep in the same direction reaches those rows last, after they have been evicted.
+static uint32_t next_sweep_reversed(b200vis_ctx *ctx) {
+    const uint32_t rev = ctx->sweep_count++ & 1u;
+    return sweep_order_fixed() ? 0u : rev;
+}
+
 extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
     CHECK_CTX();
     if (!ctx->topology_set) return fail(ctx, B200VIS_ERR_NOT_READY, "run: b200vis_set_topology has not been called");
@@ -2440,7 +2457,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
                 // the whole pass, small tiles (B200VIS_SPLIT_DEEP_TILES) included, through kernel 1b's marked instantiation
                 const uint32_t b = ctx->pass_begin[p];
                 launch_propagate_cull_ext(st, R, ctx->d_tiles + b, ctx->pass_begin[p + 1] - b, cvw, vb, ctx->d_stats, tile_stages,
-                                          (uint32_t)ctx->static_opt, cslot, ctx->d_tile_ticket, &ctx->tile_ticket_base);
+                                          (uint32_t)ctx->static_opt, cslot, ctx->d_tile_ticket, &ctx->tile_ticket_base,
+                                          next_sweep_reversed(ctx));
             }
             if (gt_ext) ctx->gt_ext_pending = false;
             for (uint32_t p = 0; p < n_pass && !gt_ext; ++p) {
@@ -2452,15 +2470,15 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
                 else
                     launch_propagate_cull(st, R, ctx->d_tiles + b + ns, ctx->pass_begin[p + 1] - b - ns,
                                           cvw, vb, ctx->d_stats, tile_stages, (uint32_t)ctx->static_opt, cslot, ctx->d_tile_ticket, &ctx->tile_ticket_base,
-                                          p < ctx->pass_named.size() && ctx->pass_named[p] != 0);
+                                          p < ctx->pass_named.size() && ctx->pass_named[p] != 0, next_sweep_reversed(ctx));
             }
         } else if (n_pass) {
-            launch_cull(st, R, cvw, vb, ctx->d_stats, cslot);
+            launch_cull(st, R, cvw, vb, ctx->d_stats, cslot, next_sweep_reversed(ctx));
         }
         for (uint32_t b = kMaxViews; view_groups && b < afc.n_views; b += kMaxViews) {
             CullViews g = make_cull_views(afc, b);
             if (ctx->have_layers_ext) memcpy(g.layers_ext, ctx->view_layers_ext[b], sizeof g.layers_ext);
-            launch_cull_group(st, R, g, vb, ctx->d_stats, cslot, b);
+            launch_cull_group(st, R, g, vb, ctx->d_stats, cslot, b, next_sweep_reversed(ctx));
         }
     }
     Lights lights = ctx->lights;

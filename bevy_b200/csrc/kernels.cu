@@ -2189,8 +2189,9 @@ k_tile_warp(Rows R, const WarpTile *__restrict__ tiles, const uint8_t *__restric
 // ------------------------------------------------------------------------------------------
 template <bool SIMPLE, bool MERGE>
 __global__ void __launch_bounds__(256, 4)
-k_cull(Rows R, const __grid_constant__ CullViews cvw, VisibleBufs vb, DevStats *__restrict__ stats, uint32_t parity) {
-    const uint32_t row = blockIdx.x * 256u + threadIdx.x;
+k_cull(Rows R, const __grid_constant__ CullViews cvw, VisibleBufs vb, DevStats *__restrict__ stats, uint32_t parity, uint32_t rev) {
+    // rev: the blocks walk the rows from the end (the CTAs are scheduled in blockIdx order), see next_sweep_reversed
+    const uint32_t row = (rev ? gridDim.x - 1u - blockIdx.x : blockIdx.x) * 256u + threadIdx.x;
     const bool active = row < R.n;
     const uint32_t lane = threadIdx.x & 31u;
     uint32_t f = 0, st8 = 0;
@@ -4428,7 +4429,8 @@ static void launch_scout_m(cudaStream_t st, const Rows &R, const Tile *tiles, ui
 }
 template <bool P, bool C, bool S, int KIND>      // KIND: 0 kernel 1b, 1 flow, 4 / 5 / 6 lean with that many CTAs per SM, 7 lean with drifting warps (PIPE), 8 kernel 1b with external GlobalTransform marks
 static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
-                       const VisibleBufs &vb, DevStats *stats, uint32_t static_opt, uint32_t parity, uint32_t *ticket, uint32_t *ticket_base) {
+                       const VisibleBufs &vb, DevStats *stats, uint32_t static_opt, uint32_t parity, uint32_t *ticket, uint32_t *ticket_base,
+                       uint32_t rev = 0) {
     static int grid = 0;
     static unsigned long long seen = 0;
     constexpr bool FLOW = KIND == 1;
@@ -4489,8 +4491,10 @@ static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32
             static int probe = -1;    // B200VIS_LEAN_PROBE: timing probes, wrong results (tools/ only)
             if (probe < 0) { const char *e = getenv("B200VIS_LEAN_PROBE"); probe = e ? atoi(e) : 0; }
             cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base, (uint32_t)flip | ((uint32_t)probe << 8));
-        } else {
+        } else if constexpr (KIND == 1) {
             cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base);
+        } else {      // kernel 1b: the one TMA kernel that takes the sweep direction (the experiment kernels keep ascending order)
+            cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base, rev);
         }
     });
 }
@@ -4508,7 +4512,7 @@ void launch_propagate_cull_small(cudaStream_t st, const Rows &R, const Tile *til
 }
 void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                            const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
-                           uint32_t *ticket, uint32_t *ticket_base, bool named_levels_only) {
+                           uint32_t *ticket, uint32_t *ticket_base, bool named_levels_only, uint32_t rev) {
     if (n_tiles == 0) return;
     const bool prop = stages & 1u, cull = stages & 2u;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
@@ -4525,7 +4529,7 @@ void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, ui
                                          else if (tile_kernel_choice() == 5 && lean_ctas_per_sm() == 4) launch_tma<P, C, S, 4>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
                                          else if (tile_kernel_choice() == 5 && lean_ctas_per_sm() == 6) launch_tma<P, C, S, 6>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
                                          else if (tile_kernel_choice() == 5) launch_tma<P, C, S, 5>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
-                                         else launch_tma<P, C, S, 0>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); } while (0)
+                                         else launch_tma<P, C, S, 0>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev); } while (0)
         if (prop && cull) { if (simple) B200VIS_LAUNCH_TMA(true, true, true); else B200VIS_LAUNCH_TMA(true, true, false); }
         else if (prop) B200VIS_LAUNCH_TMA(true, false, true);
         else if (cull) { if (simple) B200VIS_LAUNCH_TMA(false, true, true); else B200VIS_LAUNCH_TMA(false, true, false); }
@@ -4540,29 +4544,30 @@ void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, ui
 }
 void launch_propagate_cull_ext(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                                const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
-                               uint32_t *ticket, uint32_t *ticket_base) {
+                               uint32_t *ticket, uint32_t *ticket_base, uint32_t rev) {
     if (n_tiles == 0 || !(stages & 1u)) return;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
-    if (!(stages & 2u)) launch_tma<true, false, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
-    else if (simple) launch_tma<true, true, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
-    else launch_tma<true, true, false, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base);
+    if (!(stages & 2u)) launch_tma<true, false, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev);
+    else if (simple) launch_tma<true, true, true, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev);
+    else launch_tma<true, true, false, 8>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev);
 }
 bool tile_kernel_is_default() { return tile_kernel_choice() == 1; }
-void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity) {
+void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
+                 uint32_t rev) {
     if (!R.n) return;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
-    if (simple) { ++g_launches; k_cull<true, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
-    else { ++g_launches; k_cull<false, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity); }
+    if (simple) { ++g_launches; k_cull<true, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity, rev); }
+    else { ++g_launches; k_cull<false, false><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, vb, stats, parity, rev); }
 }
 void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
-                       uint32_t view_base) {
+                       uint32_t view_base, uint32_t rev) {
     if (!R.n) return;
     VisibleBufs g = vb;     // the group's masks and counter block: k_cull indexes views 0..7 of it
     g.mask = vb.mask + (size_t)view_base * vb.words_stride;
     g.chunk_count = vb.chunk_count + chunk_counter_index(0, view_base) * vb.chunks_stride;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
-    if (simple) { ++g_launches; k_cull<true, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity); }
-    else { ++g_launches; k_cull<false, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity); }
+    if (simple) { ++g_launches; k_cull<true, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity, rev); }
+    else { ++g_launches; k_cull<false, true><<<cdiv(R.n, 256), 256, 0, st>>>(R, cvw, g, stats, parity, rev); }
 }
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R) {
     if (R.n) { ++g_launches; k_mark_dirty_global<<<cdiv(R.n, 256), 256, 0, st>>>(R); }

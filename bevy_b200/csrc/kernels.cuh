@@ -6,25 +6,28 @@
 namespace b200vis {
 void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                            const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
-                           uint32_t *ticket = nullptr, uint32_t *ticket_base = nullptr, bool named_levels_only = false);
+                           uint32_t *ticket = nullptr, uint32_t *ticket_base = nullptr, bool named_levels_only = false,
+                           uint32_t rev = 0);
 void launch_propagate_cull_small(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                                  const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity);
 unsigned long long kernel_launch_count();
 // kernel 1b's instantiation for frames with pending external GlobalTransform marks (S_GT_EXT); stages must include PROPAGATE
 void launch_propagate_cull_ext(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                                const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
-                               uint32_t *ticket, uint32_t *ticket_base);
+                               uint32_t *ticket, uint32_t *ticket_base, uint32_t rev);
 bool tile_kernel_is_default();   // B200VIS_TILE_KERNEL selects kernel 1b (unset, or tma)
 bool tile_kernel_is_tma();
 bool tile_kernel_is_warp();
 bool tile_kernel_publishes_light_snapshot();
 void launch_tile_warp(cudaStream_t st, const Rows &R, const WarpTile *tiles, const uint8_t *sched, uint32_t n_tiles, const CullViews &cvw,
                       const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity, uint32_t *counter);
-void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity);
+// rev (kernel 1b and k_cull): 1 walks the tiles / rows in descending order, 0 ascending; the results do not depend on it
+void launch_cull(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
+                 uint32_t rev);
 // one group pass of a context with more than kMaxViews views: views view_base .. view_base + cvw.n_views - 1, merged into
 // the ViewVisibility state the tile pass left (k_cull's MERGE instantiation)
 void launch_cull_group(cudaStream_t st, const Rows &R, const CullViews &cvw, const VisibleBufs &vb, DevStats *stats, uint32_t parity,
-                       uint32_t view_base);
+                       uint32_t view_base, uint32_t rev);
 void launch_mark_dirty_global(cudaStream_t st, const Rows &R);
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views);

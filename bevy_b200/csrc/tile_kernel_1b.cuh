@@ -12,7 +12,7 @@ template <bool PROP, bool CULL, bool SIMPLE>
 __global__ void __launch_bounds__(kTileRows, 4)
 B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const __grid_constant__ CullViews cvw,
                 VisibleBufs vb, DevStats *__restrict__ stats, uint32_t static_opt, uint32_t parity,
-                uint32_t *__restrict__ ticket, uint32_t ticket_base) {
+                uint32_t *__restrict__ ticket, uint32_t ticket_base, uint32_t rev) {
     constexpr bool EXT = B200VIS_TILE_1B_EXT;
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TmaSmem &s = *reinterpret_cast<TmaSmem *>(smem_raw);
@@ -25,8 +25,12 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
     TP_BEGIN();
     // launched with programmatic stream serialization: everything above overlapped the previous kernel's tail
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    // rev: the pass walks its tiles from the last one (t below is the position in the walk, tile_at() the descriptor it takes).
+    // The tiles of one pass are independent of each other (out-of-tile parents sit in earlier passes), so the order changes
+    // no result.
+    auto tile_at = [&](uint32_t i) -> const Tile & { return tiles[rev ? n_tiles - 1u - i : i]; };
     uint32_t t = blockIdx.x;
-    if (lr == 0 && t < n_tiles) issue_tile_loads<PROP, CULL>(R, tiles[t], s.st[0], &s.bar[0]);
+    if (lr == 0 && t < n_tiles) issue_tile_loads<PROP, CULL>(R, tile_at(t), s.st[0], &s.bar[0]);
     uint32_t n_gt_total = 0, n_vv_total = 0;
     // Tile hand-out: a CTA starts on tile blockIdx.x and then takes the tiles the grid has not started yet in ticket order
     // (one atomic per tile, drawn by thread 0 when it prefetches, i.e. one tile ahead).  A fixed stride would leave a CTA with
@@ -35,7 +39,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
     for (uint32_t it = 0; t < n_tiles; ++it) {
         TP(0);
         const uint32_t sidx = it & 1u;
-        const Tile tile = tiles[t];
+        const Tile tile = tile_at(t);
         TP(1);
         mbar_wait(&s.bar[sidx], (it >> 1) & 1u);
         TP(2);
@@ -162,7 +166,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
             if (tn < n_tiles) {
                 asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stage's generic writes (bounds) -> TMA loads
-                issue_tile_loads<PROP, CULL>(R, tiles[tn], s.st[sidx ^ 1u], &s.bar[sidx ^ 1u]);
+                issue_tile_loads<PROP, CULL>(R, tile_at(tn), s.st[sidx ^ 1u], &s.bar[sidx ^ 1u]);
             }
             s.next_tile[sidx] = tn;      // read by everybody behind the tile's closing barrier
         }
