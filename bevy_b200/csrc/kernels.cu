@@ -491,12 +491,32 @@ __device__ unsigned long long g_tile_phase[8192 * 32];
     else { tp_acc_[(ph)] += now_ - tp_prev_; if (tp_n_ > 1u) tp_acc_[16 + (ph)] += now_ - tp_prev_; } \
     tp_prev_ = now_; } } while (0)
 #define TP_END() do { if (lr == 0 && blockIdx.x < 8192u) for (int k_ = 0; k_ < 32; ++k_) g_tile_phase[blockIdx.x * 32u + k_] = tp_acc_[k_]; } while (0)
+// CTA residency log (tools/tail_displacement.py): thread 0 of every CTA of kernel 1b (from the moment it may start its first
+// tile), of k_expand_visible and of k_cluster_fused appends one record with the %globaltimer at its start and at its exit
+// (the destructor runs on every return path) and the CTA's thread count.  kind 0 = kernel 1b, tagged with the launch's ticket
+// base; 1 = expand; 2 = clusters.
+struct ProbeRec { unsigned long long t0, t1; uint32_t kind, tag, blk, threads; };
+constexpr uint32_t kProbeCap = 1u << 18;
+__device__ ProbeRec g_probe[kProbeCap];
+__device__ uint32_t g_probe_n;
+__device__ __forceinline__ unsigned long long global_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
+struct ProbeScope {
+    unsigned long long t0; uint32_t kind, tag; bool on;
+    __device__ ProbeScope(uint32_t k, uint32_t tg) : t0(0), kind(k), tag(tg), on(threadIdx.x == 0) { if (on) t0 = global_ns(); }
+    __device__ ~ProbeScope() {
+        if (!on) return;
+        const uint32_t i = atomicAdd(&g_probe_n, 1u);
+        if (i < kProbeCap) g_probe[i] = ProbeRec{t0, global_ns(), kind, tag, blockIdx.x + (blockIdx.y << 16), blockDim.x};
+    }
+};
+#define PROBE_SCOPE(kind, tag) ProbeScope probe_scope_((kind), (tag))
 #else
 #define TT(slot) do { } while (0)
 #define TTW(slot) do { } while (0)
 #define TP_BEGIN() do { } while (0)
 #define TP(ph) do { } while (0)
 #define TP_END() do { } while (0)
+#define PROBE_SCOPE(kind, tag) do { } while (0)
 #endif
 #define B200VIS_TILE_1B k_propagate_cull_tma
 #define B200VIS_TILE_1B_EXT false
@@ -2340,12 +2360,21 @@ __global__ void k_mark_dirty_global(Rows R) {
 // serial `sort_unstable` (visibility/mod.rs:870-874) without a sort.  Also zeroes the mask it
 // consumed and the counters of the NEXT frame's parity.
 // ------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kChunkWords)
+// 256 threads per chunk (the size of one kernel-1b CTA: the kernel runs beside the next frame's tile pass), four words each.
+// The emit is warp-cooperative: a warp takes eight of the chunk's non-zero words at a time, lane l emits the row of bit l of
+// each, and the eight words' rank -> row and class loads are all issued before the first store, so no thread walks its
+// bits through a chain of dependent loads and the stores of one word are contiguous.
+constexpr uint32_t kExpandThreads = 256, kExpandWords = kChunkWords / kExpandThreads, kExpandBatch = 8;
+__global__ void __launch_bounds__(kExpandThreads, 4)
 k_expand_visible(VisibleBufs vb, DiffBufs db, const uint32_t *__restrict__ row_of_rank, const FrameConsts *__restrict__ fc,
                  DevStats *__restrict__ stats, uint32_t parity, uint32_t n_rows) {
-    __shared__ uint32_t s_warp[32], s_diff[32];
-    __shared__ uint32_t s_base, s_total;
-    const uint32_t v = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x;
+    constexpr uint32_t kWarps = kExpandThreads / 32;
+    __shared__ uint32_t s_warp[kWarps], s_diff[kWarps];
+    __shared__ uint32_t s_base, s_total, s_nnz;
+    __shared__ uint32_t s_w[kChunkWords];                               // the chunk's words
+    __shared__ uint32_t s_nz_word[kChunkWords], s_nz_pos[kChunkWords];  // its non-zero words in order: index, first list slot
+    PROBE_SCOPE(1u, 0u);
+    const uint32_t v = blockIdx.y, chunk = blockIdx.x, t = threadIdx.x, lane = t & 31u, warp = t >> 5;
     uint32_t *cc = vb.chunk_count + chunk_counter_index(parity, v) * vb.chunks_stride;
     const uint32_t zslot = (parity + 2u) % 3u;   // the slot frame f+2 will accumulate into
     uint32_t *cc_next = vb.chunk_count + chunk_counter_index(zslot, v) * vb.chunks_stride;
@@ -2362,33 +2391,42 @@ k_expand_visible(VisibleBufs vb, DiffBufs db, const uint32_t *__restrict__ row_o
         return;
     }
 
-    const uint32_t word = chunk * kChunkWords + t;
+    const uint32_t word0 = chunk * kChunkWords;
     uint32_t *mask = vb.mask + (size_t)v * vb.words_stride;
-    uint32_t w = 0;
-    if (word < vb.n_words) { w = mask[word]; if (w) mask[word] = 0; }
-    const uint32_t c = __popc(w);
-    if (db.prev != nullptr) {
-        // the lock-step march of update_cpu_culled_entities (bevy_render/src/view/visibility/mod.rs:194-249) as set
-        // algebra on the rank-ordered bit sets: added = new & ~old, removed = old & ~new
-        uint32_t a = 0, r = 0;
-        if (word < vb.n_words) {
+    uint32_t d = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < kExpandWords; ++k) {       // coalesced: word k * 256 + t of the chunk
+        const uint32_t lw = k * kExpandThreads + t, word = word0 + lw;
+        uint32_t w = 0;
+        if (word < vb.n_words) { w = mask[word]; if (w) mask[word] = 0; }
+        s_w[lw] = w;
+        if (db.prev != nullptr && word < vb.n_words) {
+            // the lock-step march of update_cpu_culled_entities (bevy_render/src/view/visibility/mod.rs:194-249) as set
+            // algebra on the rank-ordered bit sets: added = new & ~old, removed = old & ~new
             uint32_t *pv = db.prev + (size_t)v * vb.words_stride + word;
             const uint32_t old = *pv;
-            a = w & ~old; r = old & ~w;
+            const uint32_t a = w & ~old, r = old & ~w;
             if (old != w) *pv = w;
             db.words[(size_t)v * vb.words_stride + word] = a;
             db.words[((size_t)gridDim.y + v) * vb.words_stride + word] = r;
+            d += __popc(a) | (__popc(r) << 16);     // a chunk holds 32768 rows: both sums fit 16 bits
         }
-        uint32_t d = __popc(a) | (__popc(r) << 16);   // a chunk holds 32768 rows: both sums fit 16 bits
+    }
+    if (db.prev != nullptr) {
 #pragma unroll
         for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xFFFFFFFFu, d, o);
-        if ((t & 31u) == 0) s_diff[t >> 5] = d;
+        if (lane == 0) s_diff[warp] = d;
     }
-    // block exclusive scan of c
+    __syncthreads();
+    // block exclusive scan, in chunk order, of (set bits | non-zero words << 16) over thread t's words 4t .. 4t+3 (a chunk
+    // has at most 32768 set bits, so the low half never carries into the word count)
+    uint32_t mine[kExpandWords], c = 0;
+#pragma unroll
+    for (uint32_t k = 0; k < kExpandWords; ++k) { mine[k] = s_w[t * kExpandWords + k]; c += __popc(mine[k]) | (mine[k] ? 0x10000u : 0u); }
     uint32_t incl = c;
 #pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if ((t & 31u) >= (uint32_t)o) incl += y; }
-    if ((t & 31u) == 31u) s_warp[t >> 5] = incl;
+    for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, incl, o); if (lane >= (uint32_t)o) incl += y; }
+    if (lane == 31u) s_warp[warp] = incl;
     // base = sum of the counts of the preceding chunks (<= a few hundred values)
     uint32_t part = 0, tot = 0;
     if (t < 32) {
@@ -2400,26 +2438,50 @@ k_expand_visible(VisibleBufs vb, DiffBufs db, const uint32_t *__restrict__ row_o
     __syncthreads();
     if (t < 32) {
         if (db.prev != nullptr) {
-            uint32_t d = s_diff[t];
+            uint32_t dd = t < kWarps ? s_diff[t] : 0u;
 #pragma unroll
-            for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xFFFFFFFFu, d, o);
-            if (t == 0) db.chunk[(size_t)v * vb.chunks_stride + chunk] = d;
+            for (int o = 16; o > 0; o >>= 1) dd += __shfl_xor_sync(0xFFFFFFFFu, dd, o);
+            if (t == 0) db.chunk[(size_t)v * vb.chunks_stride + chunk] = dd;
         }
-        uint32_t x = s_warp[t];
+        uint32_t x = t < kWarps ? s_warp[t] : 0u;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (t >= (uint32_t)o) x += y; }
-        s_warp[t] = x;   // inclusive over warps
+        if (t < kWarps) s_warp[t] = x;   // inclusive over warps
+        if (t == 31) s_nnz = x >> 16;
     }
     __syncthreads();
-    uint32_t pos = s_base + (incl - c) + ((t >> 5) ? s_warp[(t >> 5) - 1] : 0u);
+    uint32_t ex = (incl - c) + (warp ? s_warp[warp - 1] : 0u);
+    uint32_t pos = ex & 0xFFFFu, nz = ex >> 16;
+#pragma unroll
+    for (uint32_t k = 0; k < kExpandWords; ++k) {
+        if (mine[k]) { s_nz_word[nz] = t * kExpandWords + k; s_nz_pos[nz] = pos; ++nz; }
+        pos += __popc(mine[k]);
+    }
+    __syncthreads();
+    const uint32_t nnz = s_nnz, base = s_base, below = (1u << lane) - 1u;
     uint32_t *out = vb.lists + (size_t)v * vb.list_stride;
     uint8_t *out_cls = vb.classes ? vb.classes + (size_t)v * vb.list_stride : nullptr;
-    while (w) {
-        const uint32_t b = __ffs(w) - 1; w &= w - 1;
-        const uint32_t rk = word * 32u + b;
-        const uint32_t rw = row_of_rank ? row_of_rank[rk] : rk;
-        if (out_cls) out_cls[pos] = vb.cls[rw];       // one push per class of the row (visibility/mod.rs:852-857): the shim splits
-        out[pos++] = rw;
+    for (uint32_t b0 = warp * kExpandBatch; b0 < nnz; b0 += kWarps * kExpandBatch) {
+        uint32_t wv[kExpandBatch], rw[kExpandBatch], cl[kExpandBatch];
+#pragma unroll
+        for (uint32_t k = 0; k < kExpandBatch; ++k) {
+            const uint32_t i = b0 + k;
+            const uint32_t lw = i < nnz ? s_nz_word[i] : 0u;
+            wv[k] = i < nnz ? s_w[lw] : 0u;
+            const uint32_t rk = (word0 + lw) * 32u + lane;
+            rw[k] = ((wv[k] >> lane) & 1u) ? (row_of_rank ? row_of_rank[rk] : rk) : 0u;
+        }
+        if (out_cls) {
+#pragma unroll
+            for (uint32_t k = 0; k < kExpandBatch; ++k) cl[k] = ((wv[k] >> lane) & 1u) ? vb.cls[rw[k]] : 0u;
+        }
+#pragma unroll
+        for (uint32_t k = 0; k < kExpandBatch; ++k) {
+            if (!((wv[k] >> lane) & 1u)) continue;
+            const uint32_t p = base + s_nz_pos[b0 + k] + __popc(wv[k] & below);
+            if (out_cls) out_cls[p] = (uint8_t)cl[k];     // one push per class of the row (visibility/mod.rs:852-857): the shim splits
+            out[p] = rw[k];
+        }
     }
     if (chunk == 0 && t == 0) stats->visible_count[v] = s_total;
     (void)n_rows;
@@ -2684,7 +2746,10 @@ k_cluster_assign(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBu
 // no global bit matrix, no clear kernel, no re-count.  Ascending light ordinal per cluster = the reference's push order
 // (the outer loop runs over lights, assign.rs:487).
 // ------------------------------------------------------------------------------------------
-constexpr uint32_t kFusedThreads = 1024;
+// A CTA owns kMaxClusters / nrank clusters with one thread each, so its size follows the cluster size: 1024 threads at 4
+// CTAs per view, 512 at 8 (the default), 256 at 16.  In pipelined frames the kernel runs beside the next frame's tile pass,
+// and at the 64 registers the 1024-thread bound allows a 512-thread CTA holds the registers of two kernel-1b CTAs, not four.
+constexpr uint32_t kFusedMaxThreads = kMaxClusters / 4;
 __device__ __forceinline__ uint32_t cluster_ctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ uint32_t cluster_nctarank() { uint32_t r; asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(r)); return r; }
 __device__ __forceinline__ void cluster_sync_all() {
@@ -2711,14 +2776,15 @@ __device__ __forceinline__ uint32_t ld_acquire_sys(const uint32_t *p) {
     return v;
 }
 template <bool EXT>   // as k_cluster_assign; EXT is never set for the gathered light records (per_rank)
-__global__ void __launch_bounds__(kFusedThreads)
+__global__ void __launch_bounds__(kFusedMaxThreads)
 k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBufs cb, DevStats *__restrict__ stats) {
     extern __shared__ __align__(16) uint8_t smem_fused[];
     __shared__ float4 s_planes[kStagedPlanes];
     __shared__ float s_thr[kStagedPlanes];
     __shared__ uint32_t s_warp[32];
     __shared__ uint32_t s_total, s_far, s_base, s_farmax;
-    const uint32_t v = blockIdx.y, t = threadIdx.x, lane = t & 31u, warp = t >> 5;
+    PROBE_SCOPE(2u, 0u);
+    const uint32_t v = blockIdx.y, t = threadIdx.x, lane = t & 31u, warp = t >> 5, nthr = blockDim.x;
     const uint32_t rank = cluster_ctarank(), nrank = cluster_nctarank();
     uint32_t *offsets = cb.offsets + (size_t)v * (kMaxClusters + 1);
     // early outs are uniform over the cluster (they depend on the view only): nobody is left waiting at a cluster barrier
@@ -2741,7 +2807,7 @@ k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBuf
     }
     const uint32_t nc = cv.n_clusters, per = (nc + nrank - 1) / nrank, words = (L.n + 31u) / 32u;
     uint32_t *s_mask = reinterpret_cast<uint32_t *>(smem_fused);      // [words][per]
-    for (uint32_t i = t; i < words * per; i += kFusedThreads) s_mask[i] = 0;
+    for (uint32_t i = t; i < words * per; i += nthr) s_mask[i] = 0;
     if (t == 0) { s_total = 0; s_far = 0; }
     const uint32_t nx = cv.dims[0] + 1, ny_p = cv.dims[1] + 1, nz = cv.dims[2] + 1;
     const bool staged = nx + ny_p + nz <= kStagedPlanes;
@@ -2749,10 +2815,10 @@ k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBuf
         const float4 *gx = reinterpret_cast<const float4 *>(cb.blob + cv.x_off);
         const float4 *gy = reinterpret_cast<const float4 *>(cb.blob + cv.y_off);
         const float4 *gz = reinterpret_cast<const float4 *>(cb.blob + cv.z_off);
-        for (uint32_t i = t; i < nx; i += kFusedThreads) s_planes[i] = gx[i];
-        for (uint32_t i = t; i < ny_p; i += kFusedThreads) s_planes[nx + i] = gy[i];
-        for (uint32_t i = t; i < nz; i += kFusedThreads) s_planes[nx + ny_p + i] = gz[i];
-        for (uint32_t i = t; i + 1 < cv.dims[2]; i += kFusedThreads) s_thr[i] = cb.blob[cv.thr_off + i];
+        for (uint32_t i = t; i < nx; i += nthr) s_planes[i] = gx[i];
+        for (uint32_t i = t; i < ny_p; i += nthr) s_planes[nx + i] = gy[i];
+        for (uint32_t i = t; i < nz; i += nthr) s_planes[nx + ny_p + i] = gz[i];
+        for (uint32_t i = t; i + 1 < cv.dims[2]; i += nthr) s_thr[i] = cb.blob[cv.thr_off + i];
     }
     cluster_sync_all();                    // every CTA's matrix is zeroed before the first remote bit arrives
     ClusterTables tb;
@@ -2761,7 +2827,7 @@ k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBuf
     tb.yp = staged ? s_planes + nx : reinterpret_cast<const float4 *>(cb.blob + cv.y_off);
     tb.zp = staged ? s_planes + nx + ny_p : reinterpret_cast<const float4 *>(cb.blob + cv.z_off);
     // ---- assign: light li is handled by warp (li / nrank) % 32 of CTA li % nrank
-    for (uint32_t li = rank + nrank * warp; li < L.n; li += nrank * (kFusedThreads / 32)) {
+    for (uint32_t li = rank + nrank * warp; li < L.n; li += nrank * (nthr / 32u)) {
         float px, py, pz;
         if (L.snap != nullptr || L.per_rank) {
             const float4 sp = light_snap_of(L, li);
@@ -2795,7 +2861,7 @@ k_cluster_fused(Rows R, Lights L, const FrameConsts *__restrict__ fc, ClusterBuf
     if (lane == 31u) s_warp[warp] = incl;
     __syncthreads();
     if (t < 32) {
-        uint32_t x = s_warp[t];
+        uint32_t x = t < nthr / 32u ? s_warp[t] : 0u;
 #pragma unroll
         for (int o = 1; o < 32; o <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, o); if (t >= (uint32_t)o) x += y; }
         s_warp[t] = x;          // inclusive over warps
@@ -4575,7 +4641,7 @@ void launch_mark_dirty_global(cudaStream_t st, const Rows &R) {
 void launch_expand_visible(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, const uint32_t *row_of_rank, const FrameConsts *fc,
                            DevStats *stats, uint32_t parity, uint32_t n_rows, uint32_t max_views) {
     if (vb.n_chunks == 0) return;
-    ++g_launches; k_expand_visible<<<dim3(vb.n_chunks, max_views), kChunkWords, 0, st>>>(vb, db, row_of_rank, fc, stats, parity, n_rows);
+    ++g_launches; k_expand_visible<<<dim3(vb.n_chunks, max_views), kExpandThreads, 0, st>>>(vb, db, row_of_rank, fc, stats, parity, n_rows);
     if (db.prev != nullptr) { ++g_launches; k_emit_visible_diff<<<dim3(vb.n_chunks, max_views), kChunkWords, 0, st>>>(vb, db, row_of_rank, fc); }
 }
 void launch_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, const uint32_t *row_of_rank,
@@ -4602,7 +4668,8 @@ void launch_cluster_assign(cudaStream_t st, const Rows &R, const Lights &L, cons
     if (L.layers_ext != nullptr) k_cluster_assign<true><<<dim3(cdiv(L.n, 8), max_views), 256, 0, st>>>(R, L, fc, cb, stats);
     else k_cluster_assign<false><<<dim3(cdiv(L.n, 8), max_views), 256, 0, st>>>(R, L, fc, cb, stats);
 }
-// assign + lists of every view in one launch (single GPU): thread-block clusters of 8 (16 beyond ~3200 lights) CTAs per view
+// assign + lists of every view in one launch (single GPU): thread-block clusters of 8 CTAs of 512 threads per view (16 of
+// 256 beyond ~3200 lights; B200VIS_CLUSTER_CTAS)
 // Can the one-launch cluster stage hold `n_lights` mask bits per cluster in a thread-block cluster's shared memory?
 bool cluster_fused_fits(uint32_t n_lights) {
     const char *e = getenv("B200VIS_CLUSTER_KERNEL");
@@ -4630,13 +4697,12 @@ bool launch_cluster_fused(cudaStream_t st, const Rows &R, const Lights &L, const
     if (!enabled) return false;
     const uint32_t words = (L.n + 31u) / 32u;
     // every CTA popcounts, scans and emits its kMaxClusters / nrank owned clusters with one thread each: nrank >= 4
-    static_assert(kMaxClusters / 4 <= kFusedThreads, "a CTA of the fused cluster kernel owns more clusters than it has threads");
     uint32_t nrank = (nrank_env == 4 || nrank_env == 8 || nrank_env == 16) ? (uint32_t)nrank_env : 8u;
     size_t smem = (size_t)words * (kMaxClusters / nrank) * 4;
     if (smem > 200u * 1024u) { nrank = 16; smem = (size_t)words * (kMaxClusters / nrank) * 4; }
     if (smem > 200u * 1024u) return false;                    // more lights than the distributed matrix can hold: split path
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(nrank, max_views); cfg.blockDim = dim3(kFusedThreads); cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cfg.gridDim = dim3(nrank, max_views); cfg.blockDim = dim3(kMaxClusters / nrank); cfg.dynamicSmemBytes = smem; cfg.stream = st;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeClusterDimension;
     attr[0].val.clusterDim.x = nrank; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
@@ -5042,5 +5108,16 @@ extern "C" __attribute__((visibility("default"))) int b200vis_debug_tile_timing(
 extern "C" __attribute__((visibility("default"))) int b200vis_debug_tile_phases(unsigned long long *out, unsigned n_ctas) {
     if (n_ctas > 8192u) n_ctas = 8192u;
     return (int)cudaMemcpyFromSymbol(out, b200vis::g_tile_phase, (size_t)n_ctas * 32 * sizeof(unsigned long long));
+}
+// copies up to `cap` residency records (32 bytes each) out, empties the log and returns how many were appended since the
+// last call (more than cap: the rest were dropped); negative: a CUDA error.  Call with the device idle.
+extern "C" __attribute__((visibility("default"))) long long b200vis_debug_probe(void *out, unsigned cap) {
+    uint32_t n = 0;
+    cudaError_t e = cudaMemcpyFromSymbol(&n, b200vis::g_probe_n, sizeof n);
+    const uint32_t k = std::min(std::min(n, cap), b200vis::kProbeCap);
+    if (e == cudaSuccess && k) e = cudaMemcpyFromSymbol(out, b200vis::g_probe, (size_t)k * sizeof(b200vis::ProbeRec));
+    const uint32_t zero = 0;
+    if (e == cudaSuccess) e = cudaMemcpyToSymbol(b200vis::g_probe_n, &zero, sizeof zero);
+    return e == cudaSuccess ? (long long)n : -(long long)e;
 }
 #endif

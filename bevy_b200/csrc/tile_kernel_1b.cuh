@@ -25,6 +25,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
     TP_BEGIN();
     // launched with programmatic stream serialization: everything above overlapped the previous kernel's tail
     asm volatile("griddepcontrol.wait;" ::: "memory");
+    PROBE_SCOPE(0u, ticket_base);
     // rev: the pass walks its tiles from the last one (t below is the position in the walk, tile_at() the descriptor it takes).
     // The tiles of one pass are independent of each other (out-of-tile parents sit in earlier passes), so the order changes
     // no result.
