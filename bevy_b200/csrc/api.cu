@@ -95,6 +95,10 @@ struct b200vis_ctx {
     WarpTile *d_wtiles = nullptr; uint8_t *d_sched = nullptr; uint32_t *d_wtopo = nullptr;   // k_tile_warp's view of the plan
     uint32_t *d_tile_counter = nullptr;
     uint32_t *d_tile_ticket = nullptr; uint32_t tile_ticket_base = 0;   // dynamic tile hand-out of the default kernel: never reset, the host tracks the base
+    // kernel 1b's staging hint, one byte per tile descriptor (indexed like d_tiles): non-zero = stage all three old
+    // GlobalTransform rows, 0 = row 0 alone (tile_kernel_1b.cuh).  Every new plan starts at all three; any value is correct.
+    uint8_t *d_tile_hint = nullptr; uint32_t hint_cap = 0;
+    bool gt_stage_full = false;     // B200VIS_GT_STAGE=full (experiment switch, read at create): always stage all three rows
     // Full-world sweeps launched so far: every kernel 1b launch over a pass and every k_cull launch counts one.  Each sweep
     // walks the rows opposite to the previous one (next_sweep_reversed), so it starts on the rows the previous sweep touched
     // last, which are the ones still in L2.  Any order gives the same results; only the parity matters.
@@ -267,7 +271,7 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
     Rows &r = ctx->rows;
     void *dev[] = {r.trsA, r.trsB, r.trsC, r.gt0, r.gt1, r.gt2, r.bndA, r.bndB, r.flags, r.state, r.topo,
                    ctx->d_parent, ctx->d_layers, ctx->d_range, ctx->d_rank, ctx->d_row_of_rank, ctx->d_dirty,
-                   ctx->d_layers_ext, ctx->d_vv_shadow, ctx->d_gt_aos, ctx->d_tiles, ctx->d_wtiles, ctx->d_sched, ctx->d_wtopo, ctx->d_tile_counter, ctx->d_tile_ticket, ctx->d_blob2[0], ctx->d_blob2[1], ctx->d_blob2[2], ctx->d_lrec, ctx->d_lrec_all, ctx->d_tag_flag, ctx->d_light_ord,
+                   ctx->d_layers_ext, ctx->d_vv_shadow, ctx->d_gt_aos, ctx->d_tiles, ctx->d_wtiles, ctx->d_sched, ctx->d_wtopo, ctx->d_tile_counter, ctx->d_tile_ticket, ctx->d_tile_hint, ctx->d_blob2[0], ctx->d_blob2[1], ctx->d_blob2[2], ctx->d_lrec, ctx->d_lrec_all, ctx->d_tag_flag, ctx->d_light_ord,
                    ctx->vis.mask, ctx->vis.chunk_count, ctx->vis.lists, ctx->vis.classes, ctx->d_cls, ctx->d_stats, ctx->d_light_row,
                    ctx->d_light_range, ctx->d_light_layers, ctx->d_slab, ctx->cl.offsets, ctx->cl.indices, ctx->d_stage,
                    ctx->diff.prev, ctx->diff.words, ctx->diff.chunk, ctx->diff.lists, ctx->diff.count,
@@ -381,6 +385,7 @@ extern "C" int32_t b200vis_create(const b200vis_config *cfg, b200vis_ctx **out) 
         for (cudaEvent_t &e : ctx->ev_side) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         for (cudaEvent_t &e : ctx->ev_expand) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
         { const char *e = getenv("B200VIS_PIPELINE"); if (e && e[0] == '0') ctx->pipeline = false; }
+        { const char *e = getenv("B200VIS_GT_STAGE"); ctx->gt_stage_full = e && e[0] == 'f'; }
         for (int i = 0; i < b200vis_ctx::kRing; ++i) {
             CU(cudaMallocHost(&ctx->h_ring[i], ctx->blob_cap));
             CU(cudaEventCreateWithFlags(&ctx->ring_ev[i], cudaEventDisableTiming));
@@ -1000,6 +1005,20 @@ static int32_t tables_unmap_rows(b200vis_ctx *ctx, uint32_t n_rows, const uint32
 static void tables_renumber(b200vis_ctx *ctx, const std::vector<uint32_t> &old_to_new);
 static int32_t flush_table_updates(b200vis_ctx *ctx);
 
+// A new plan (set, edit or compaction of the topology): kernel 1b's staging hints are sized to the tile descriptors and
+// start at full staging.  Ordered on `st` behind the plan's upload.
+static int32_t reset_tile_hints(b200vis_ctx *ctx, cudaStream_t st) {
+    if (ctx->hint_cap < ctx->tiles_cap) {
+        CU(cudaStreamSynchronize(st));
+        cudaFree(ctx->d_tile_hint);
+        ctx->d_tile_hint = nullptr; ctx->hint_cap = 0;
+        CU(dalloc(&ctx->d_tile_hint, ctx->tiles_cap));
+        ctx->hint_cap = ctx->tiles_cap;
+    }
+    CU(cudaMemsetAsync(ctx->d_tile_hint, 1, ctx->hint_cap, st));
+    return B200VIS_OK;
+}
+
 extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint32_t *parent, const uint64_t *entity_bits) {
     CHECK_CTX_JOIN();
     if (n && (!parent || !entity_bits)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "set_topology: null array");
@@ -1036,6 +1055,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
     CU(cudaMemcpy(ctx->rows.topo, topo.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_parent, parent, (size_t)n * 4, cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_tiles, tiles.data(), tiles.size() * sizeof(Tile), cudaMemcpyHostToDevice));
+    if ((rc = reset_tile_hints(ctx, st))) return rc;
     CU(cudaMemcpy(ctx->d_wtiles, plan.wtiles.data(), plan.wtiles.size() * sizeof(WarpTile), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_sched, plan.sched.data(), plan.sched.size(), cudaMemcpyHostToDevice));
     CU(cudaMemcpy(ctx->d_wtopo, plan.wtopo.data(), (size_t)n * 4, cudaMemcpyHostToDevice));
@@ -1255,6 +1275,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
         return B200VIS_OK;
     };
     if ((rc = put(ctx->d_tiles, hp.tiles.data(), T * sizeof(Tile)))) return rc;
+    if ((rc = reset_tile_hints(ctx, st))) return rc;
     if ((rc = put(ctx->d_wtiles, hp.wtiles.data(), T * sizeof(WarpTile)))) return rc;
     for (const auto &rg : er.ranges) {
         const size_t a = rg.first, c = (size_t)(rg.second - rg.first) * 4;
@@ -1539,6 +1560,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
     if ((rc = put(ctx->d_wtopo, q.wtopo.data(), (size_t)n2 * 4))) return rc;
     if ((rc = put(ctx->d_parent, q.parent.data(), (size_t)n2 * 4))) return rc;
     if ((rc = put(ctx->d_tiles, q.tiles.data(), (size_t)T * sizeof(Tile)))) return rc;
+    if ((rc = reset_tile_hints(ctx, st))) return rc;
     if ((rc = put(ctx->d_wtiles, q.wtiles.data(), (size_t)T * sizeof(WarpTile)))) return rc;
     if ((rc = put(ctx->d_sched, q.sched.data(), q.sched.size()))) return rc;
     CU(cudaEventRecord(ctx->ev_edit, st));
@@ -2470,7 +2492,8 @@ extern "C" int32_t b200vis_run(b200vis_ctx *ctx, uint32_t stages) {
                 else
                     launch_propagate_cull(st, R, ctx->d_tiles + b + ns, ctx->pass_begin[p + 1] - b - ns,
                                           cvw, vb, ctx->d_stats, tile_stages, (uint32_t)ctx->static_opt, cslot, ctx->d_tile_ticket, &ctx->tile_ticket_base,
-                                          p < ctx->pass_named.size() && ctx->pass_named[p] != 0, next_sweep_reversed(ctx));
+                                          p < ctx->pass_named.size() && ctx->pass_named[p] != 0, next_sweep_reversed(ctx),
+                                          ctx->gt_stage_full ? nullptr : ctx->d_tile_hint + b + ns);
             }
         } else if (n_pass) {
             launch_cull(st, R, cvw, vb, ctx->d_stats, cslot, next_sweep_reversed(ctx));

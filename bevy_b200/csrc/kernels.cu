@@ -407,6 +407,8 @@ struct TmaSmem {
                                      //            and have looked at the NEXT tile's change flags (climb[s ^ 1] is final)
     uint32_t next_tile[2];           // k_propagate_cull_tma: the tile this CTA processes after the one in stage s
     uint32_t climb[2];               // climb[s] == it: a non-root row of the tile of iteration it (stage s) has Changed<Transform>
+    uint32_t gt_full[2];             // k_propagate_cull_tma: stage s holds all three old GlobalTransform rows (0: row 0 only)
+    uint32_t gt_fb[2];               // k_propagate_cull_tma: a row of the tile in stage s was not proven changed by row 0
     uint16_t parent[kTileRows];
     uint8_t pst[kTileRows];      // bit0 visited, bit1 gt changed
     uint8_t dirty[kTileRows];
@@ -458,14 +460,16 @@ __device__ __forceinline__ void cp_async_16(void *dst, const void *src) {
 __device__ __forceinline__ void cp_async_8(void *dst, const void *src) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 8;" ::"r"(smem_u32(dst)), "l"(src) : "memory");
 }
+// gt12 = false stages old GlobalTransform row 0 only (kernel 1b's row-0 tiles): the slots of rows 1-2 keep whatever they held
 template <bool PROP, bool CULL>
-__device__ __forceinline__ void issue_tile_loads(const Rows &R, const Tile &t, TileStage &S, unsigned long long *bar) {
+__device__ __forceinline__ void issue_tile_loads(const Rows &R, const Tile &t, TileStage &S, unsigned long long *bar, bool gt12 = true) {
     const uint32_t a = t.base & ~15u;
     const uint32_t cnt = ((t.base - a) + t.n_rows + 15u) & ~15u;
-    uint32_t bytes = cnt * (48u + 2u);
+    uint32_t bytes = cnt * ((gt12 ? 48u : 16u) + 2u);
     if (PROP) bytes += cnt * (40u + 4u);
     mbar_expect_tx(bar, bytes);
-    bulk_g2s(S.gt0, R.gt0 + a, cnt * 16u, bar); bulk_g2s(S.gt1, R.gt1 + a, cnt * 16u, bar); bulk_g2s(S.gt2, R.gt2 + a, cnt * 16u, bar);
+    bulk_g2s(S.gt0, R.gt0 + a, cnt * 16u, bar);
+    if (gt12) { bulk_g2s(S.gt1, R.gt1 + a, cnt * 16u, bar); bulk_g2s(S.gt2, R.gt2 + a, cnt * 16u, bar); }
     bulk_g2s(S.flags, R.flags + a, cnt, bar); bulk_g2s(S.state, R.state + a, cnt, bar);
     if (PROP) {
         bulk_g2s(S.trsA, R.trsA + a, cnt * 16u, bar); bulk_g2s(S.trsB, R.trsB + a, cnt * 16u, bar);
@@ -4496,7 +4500,7 @@ static void launch_scout_m(cudaStream_t st, const Rows &R, const Tile *tiles, ui
 template <bool P, bool C, bool S, int KIND>      // KIND: 0 kernel 1b, 1 flow, 4 / 5 / 6 lean with that many CTAs per SM, 7 lean with drifting warps (PIPE), 8 kernel 1b with external GlobalTransform marks
 static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                        const VisibleBufs &vb, DevStats *stats, uint32_t static_opt, uint32_t parity, uint32_t *ticket, uint32_t *ticket_base,
-                       uint32_t rev = 0) {
+                       uint32_t rev = 0, uint8_t *gt_hint = nullptr) {
     static int grid = 0;
     static unsigned long long seen = 0;
     constexpr bool FLOW = KIND == 1;
@@ -4560,7 +4564,7 @@ static void launch_tma(cudaStream_t st, const Rows &R, const Tile *tiles, uint32
         } else if constexpr (KIND == 1) {
             cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base);
         } else {      // kernel 1b: the one TMA kernel that takes the sweep direction (the experiment kernels keep ascending order)
-            cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base, rev);
+            cudaLaunchKernelEx(&cfg, kern, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, tk, base, rev, gt_hint);
         }
     });
 }
@@ -4578,7 +4582,7 @@ void launch_propagate_cull_small(cudaStream_t st, const Rows &R, const Tile *til
 }
 void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                            const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
-                           uint32_t *ticket, uint32_t *ticket_base, bool named_levels_only, uint32_t rev) {
+                           uint32_t *ticket, uint32_t *ticket_base, bool named_levels_only, uint32_t rev, uint8_t *gt_hint) {
     if (n_tiles == 0) return;
     const bool prop = stages & 1u, cull = stages & 2u;
     const bool simple = R.layers == nullptr && R.layers_ext == nullptr && R.range == nullptr && R.rank == nullptr;
@@ -4595,7 +4599,7 @@ void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, ui
                                          else if (tile_kernel_choice() == 5 && lean_ctas_per_sm() == 4) launch_tma<P, C, S, 4>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
                                          else if (tile_kernel_choice() == 5 && lean_ctas_per_sm() == 6) launch_tma<P, C, S, 6>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
                                          else if (tile_kernel_choice() == 5) launch_tma<P, C, S, 5>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base); \
-                                         else launch_tma<P, C, S, 0>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev); } while (0)
+                                         else launch_tma<P, C, S, 0>(st, R, tiles, n_tiles, cvw, vb, stats, static_opt, parity, ticket, ticket_base, rev, (P) ? gt_hint : nullptr); } while (0)
         if (prop && cull) { if (simple) B200VIS_LAUNCH_TMA(true, true, true); else B200VIS_LAUNCH_TMA(true, true, false); }
         else if (prop) B200VIS_LAUNCH_TMA(true, false, true);
         else if (cull) { if (simple) B200VIS_LAUNCH_TMA(false, true, true); else B200VIS_LAUNCH_TMA(false, true, false); }

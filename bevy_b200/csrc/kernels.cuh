@@ -7,7 +7,9 @@ namespace b200vis {
 void launch_propagate_cull(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                            const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity,
                            uint32_t *ticket = nullptr, uint32_t *ticket_base = nullptr, bool named_levels_only = false,
-                           uint32_t rev = 0);
+                           uint32_t rev = 0, uint8_t *gt_hint = nullptr);
+// gt_hint (kernel 1b's PROPAGATE instantiations): one byte per tile of `tiles`, non-zero = stage all three old GlobalTransform
+// rows, 0 = row 0 alone; the kernel rewrites it after every tile.  nullptr: always all three rows
 void launch_propagate_cull_small(cudaStream_t st, const Rows &R, const Tile *tiles, uint32_t n_tiles, const CullViews &cvw,
                                  const VisibleBufs &vb, DevStats *stats, uint32_t stages, uint32_t static_opt, uint32_t parity);
 unsigned long long kernel_launch_count();

@@ -8,17 +8,29 @@
 //                        S_GT_HANDED to children in later passes; the row's own Changed<GlobalTransform> stays `changed`.  The pass
 //                        consumes the marks.
 // One source for both keeps the unmarked kernel's code exactly what it is without the feature.
+//
+// Row-0 staging (the unmarked PROP instantiations, gt_hint != nullptr).  set_if_neq reads the old GlobalTransform only to
+// decide `changed` and to keep the old bits when nothing changed.  A differing row 0 (X.x, Y.x, Z.x, T.x) proves a change by
+// IEEE != on its own (NaN compares unequal, so it lands there too); only when row 0 is equal (including a +0 / -0
+// difference) do rows 1-2 decide.  So a tile can be staged with old row 0 alone: 32 B/row less TMA traffic, 136 instead of
+// 168 B/row in all.  In such a tile every row that row 0 does not prove changed -- a row no level visited, an unwritten root,
+// a row whose new row 0 equals the old one -- reads its old rows 1-2 from HBM into its own slots, before its level hand-over
+// (its children read them), the cull and the bulk store (which read all three rows).  Thread 0 picks the staging per tile
+// from gt_hint[tile]: non-zero when the tile's last run had such a row (static tiles then cost what full staging costs), and
+// every run writes it back.  It is only a hint: either staging gives the same bits.
 template <bool PROP, bool CULL, bool SIMPLE>
 __global__ void __launch_bounds__(kTileRows, 4)
 B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const __grid_constant__ CullViews cvw,
                 VisibleBufs vb, DevStats *__restrict__ stats, uint32_t static_opt, uint32_t parity,
-                uint32_t *__restrict__ ticket, uint32_t ticket_base, uint32_t rev) {
+                uint32_t *__restrict__ ticket, uint32_t ticket_base, uint32_t rev, uint8_t *__restrict__ gt_hint) {
     constexpr bool EXT = B200VIS_TILE_1B_EXT;
+    constexpr bool ROW0 = PROP && !EXT;      // instantiations that may stage old GlobalTransform row 0 alone
     extern __shared__ __align__(128) uint8_t smem_raw[];
     TmaSmem &s = *reinterpret_cast<TmaSmem *>(smem_raw);
     const uint32_t lr = threadIdx.x;
     if (lr == 0) {
         mbar_init(&s.bar[0], 1); mbar_init(&s.bar[1], 1);
+        s.gt_fb[0] = 0u; s.gt_fb[1] = 0u;
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
@@ -29,9 +41,16 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
     // rev: the pass walks its tiles from the last one (t below is the position in the walk, tile_at() the descriptor it takes).
     // The tiles of one pass are independent of each other (out-of-tile parents sit in earlier passes), so the order changes
     // no result.
-    auto tile_at = [&](uint32_t i) -> const Tile & { return tiles[rev ? n_tiles - 1u - i : i]; };
+    auto tile_idx = [&](uint32_t i) { return rev ? n_tiles - 1u - i : i; };
+    auto tile_at = [&](uint32_t i) -> const Tile & { return tiles[tile_idx(i)]; };
+    // thread 0 picks the staging of a tile when it issues its loads, and publishes it in s.gt_full before the mbarrier arrive
+    auto stage_full = [&](uint32_t i) -> bool { return !ROW0 || gt_hint == nullptr || gt_hint[tile_idx(i)] != 0; };
     uint32_t t = blockIdx.x;
-    if (lr == 0 && t < n_tiles) issue_tile_loads<PROP, CULL>(R, tile_at(t), s.st[0], &s.bar[0]);
+    if (lr == 0 && t < n_tiles) {
+        const bool full = stage_full(t);
+        if (ROW0) s.gt_full[0] = full;
+        issue_tile_loads<PROP, CULL>(R, tile_at(t), s.st[0], &s.bar[0], full);
+    }
     uint32_t n_gt_total = 0, n_vv_total = 0;
     // Tile hand-out: a CTA starts on tile blockIdx.x and then takes the tiles the grid has not started yet in ticket order
     // (one atomic per tile, drawn by thread 0 when it prefetches, i.e. one tile ahead).  A fixed stride would leave a CTA with
@@ -45,6 +64,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         mbar_wait(&s.bar[sidx], (it >> 1) & 1u);
         TP(2);
         TileStage &S = s.st[sidx];
+        const bool row0 = ROW0 && !s.gt_full[sidx];      // this tile's old rows 1-2 are not staged
         const uint32_t off = tile.base & 15u;
         const uint32_t li = off + lr;                 // index into the staged window
         const bool active = lr < tile.n_rows;
@@ -92,21 +112,33 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
             if (CULL && active) { cp_async_16(&S.trsA[li], R.bndA + row); cp_async_8(&S.trsC[li], R.bndB + row); }
             const uint32_t my_level = (active && !(topo & T_DETACHED)) ? depth : 0xFFFFFFFFu;
             if (active && (topo & T_DETACHED) && has_children) s.pst[lr] = 0;
+            // set_if_neq of a visited row: row 0 first (see the top of this file); when it is equal, rows 1-2 decide, read
+            // from HBM into the row's own slots in a row-0 tile, where they stay as the kept bits if nothing changed
+            auto set_if_neq = [&](const Aff &n) -> bool {
+                bool c = row_neq(n.r0, S.gt0[li]);
+                if (!c) {
+                    s.gt_fb[sidx] = 1u;
+                    if (row0) { S.gt1[li] = R.gt1[row]; S.gt2[li] = R.gt2[row]; }
+                    c = row_neq(n.r1, S.gt1[li]) | row_neq(n.r2, S.gt2[li]);
+                }
+                if (c) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
+                return c;
+            };
             if (my_level == 0) {
-                Aff n = l;
                 if (topo & T_ROOT) {
                     visited = has_children ? (!static_opt || dirty) : tchanged;
                     changed = visited;
+                    if (changed) { S.gt0[li] = l.r0; S.gt1[li] = l.r1; S.gt2[li] = l.r2; }
                 } else {
                     const uint32_t pr = R.parent[row];
                     const uint32_t ps = R.state[pr];
                     visited = (ps & S_VISITED) && !(static_opt && !dirty && !(ps & (EXT ? S_GT_HANDED : S_GT_CHANGED)));
                     if (visited) {
+                        Aff n;
                         n.r0 = affine_mul_row(R.gt0[pr], l); n.r1 = affine_mul_row(R.gt1[pr], l); n.r2 = affine_mul_row(R.gt2[pr], l);
-                        changed = row_neq(n.r0, S.gt0[li]) | row_neq(n.r1, S.gt1[li]) | row_neq(n.r2, S.gt2[li]);
+                        changed = set_if_neq(n);
                     }
                 }
-                if (changed) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
                 if (has_children) s.pst[lr] = (uint8_t)((visited ? 1u : 0u) | ((changed || (visited && ext_mark)) ? 2u : 0u));
             }
             TP(4);
@@ -118,8 +150,7 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                 if (visited) {
                     Aff n;
                     n.r0 = affine_mul_row(S.gt0[pi], l); n.r1 = affine_mul_row(S.gt1[pi], l); n.r2 = affine_mul_row(S.gt2[pi], l);
-                    changed = row_neq(n.r0, S.gt0[li]) | row_neq(n.r1, S.gt1[li]) | row_neq(n.r2, S.gt2[li]);   // set_if_neq
-                    if (changed) { S.gt0[li] = n.r0; S.gt1[li] = n.r1; S.gt2[li] = n.r2; }
+                    changed = set_if_neq(n);
                 }
                 if (has_children) s.pst[lr] = (uint8_t)((visited ? 1u : 0u) | ((changed || (visited && ext_mark)) ? 2u : 0u));
             };
@@ -156,6 +187,12 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
                     if (my_level == lvl) walk_row();
                 }
             }
+            // a row no level visited keeps its old matrix, which the cull and the bulk store read (children of an unvisited
+            // row are not visited, so nothing reads it earlier); the cp.async lands behind the cp.async.wait_all below
+            if (active && !visited) {
+                s.gt_fb[sidx] = 1u;
+                if (row0) { cp_async_16(&S.gt1[li], R.gt1 + row); cp_async_16(&S.gt2[li], R.gt2 + row); }
+            }
             if (active && tchanged) R.flags[row] = (uint8_t)(f & ~F_TCHANGED);
         }
         TP(5);
@@ -165,9 +202,11 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         if (lr == 0) {
             const uint32_t tn = ticket ? gridDim.x + (atomicAdd(ticket, 1u) - ticket_base) : t + gridDim.x;
             if (tn < n_tiles) {
+                const bool full = stage_full(tn);
                 asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
                 asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the stage's generic writes (bounds) -> TMA loads
-                issue_tile_loads<PROP, CULL>(R, tile_at(tn), s.st[sidx ^ 1u], &s.bar[sidx ^ 1u]);
+                if (ROW0) s.gt_full[sidx ^ 1u] = full;
+                issue_tile_loads<PROP, CULL>(R, tile_at(tn), s.st[sidx ^ 1u], &s.bar[sidx ^ 1u], full);
             }
             s.next_tile[sidx] = tn;      // read by everybody behind the tile's closing barrier
         }
@@ -294,9 +333,15 @@ B200VIS_TILE_1B(Rows R, const Tile *__restrict__ tiles, uint32_t n_tiles, const 
         // end of tile: everybody is done with this stage; count changes; write the tile's matrices back
         n_gt_total += (PROP && changed) ? 1u : 0u;      // per-thread tallies, reduced once at the end of the kernel
         n_vv_total += vv_changed ? 1u : 0u;
+        if (ROW0 && !CULL && row0) asm volatile("cp.async.wait_all;" ::: "memory");   // old rows 1-2 of unvisited rows
         TP(7);
         const int any_gt = __syncthreads_or(PROP && changed);
         TP(8);
+        if (ROW0 && lr == 0) {      // the tile's staging for its next run
+            const uint32_t fb = s.gt_fb[sidx];
+            if (gt_hint != nullptr && fb != s.gt_full[sidx]) gt_hint[tile_idx(t)] = (uint8_t)fb;
+            s.gt_fb[sidx] = 0u;
+        }
         t = s.next_tile[sidx];
         if (lr == 0) {
             if (PROP && any_gt) {
