@@ -451,6 +451,7 @@ _SIGNATURES = {
     "b200vis_run_shadow_culling": (C.c_int32, [_vp]),
     "b200vis_download_shadow_visible": (C.c_int32, [_vp, C.c_uint32, C.c_uint32, _vp, C.c_uint32, _P(C.c_uint32)]),
     "b200vis_set_shadow_entities_sink": (C.c_int32, [_vp, _P(ShadowEntitiesSink)]),
+    "b200vis_emit_shadow_entities": (C.c_int32, [_vp]),
     "b200vis_set_shadow_diff_sink": (C.c_int32, [_vp, _P(ShadowDiffSink)]),
     "b200vis_set_shadow_items_ex": (C.c_int32, [_vp, C.c_uint32, _vp, C.c_uint32, _vp]),
     "b200vis_set_view_diff_sink": (C.c_int32, [_vp, _P(ViewDiffSink)]),
@@ -990,6 +991,11 @@ class Context:
         s = ShadowEntitiesSink(ptr(entities), cap, mi, ptr(offsets), ptr(active))
         self._check(self._lib.b200vis_set_shadow_entities_sink(self._h, C.byref(s)))
         self._shadow_sink = (entities, offsets, active)
+
+    def emit_shadow_entities(self):
+        """b200vis_emit_shadow_entities: the last run_shadow_culling's offsets, active flags and Entity lists again, into
+        the entity sink registered now (after a too-small sink: register a larger one, emit, synchronize)."""
+        self._check(self._lib.b200vis_emit_shadow_entities(self._h))
 
     def set_shadow_diff_sink(self, added, removed, added_offsets, removed_offsets, max_slots=0, added_capacity=None,
                              removed_capacity=None, max_items=None):

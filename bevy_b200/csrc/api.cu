@@ -178,6 +178,9 @@ struct b200vis_ctx {
     uint32_t *d_ent_counts = nullptr; uint32_t ent_chunks = 0;
     // b200vis_set_shadow_entities_sink: device aliases (entities == nullptr: none), its max_items, and the device offsets
     ShadowSink shsink{}; uint32_t shsink_max_items = 0; uint32_t *d_shadow_off = nullptr; size_t shadow_off_cap = 0;
+    // b200vis_emit_shadow_entities: the last run's mask bits (copied while an entity sink is registered), and whether they
+    // still describe the installed items over the current rows (cleared by new items and by every topology change)
+    uint32_t *d_shadow_kept = nullptr; size_t shadow_kept_cap = 0; bool shadow_emit_ready = false;
     // b200vis_set_shadow_diff_sink: the device state (added == nullptr: none) and the host's side of it: max_items / max_slots,
     // the installed items' slots, and which slots may hold entries (the ones a run named since they were last emptied)
     ShadowDiff sdiff{}; uint32_t sdiff_max_items = 0, sdiff_max_slots = 0;
@@ -283,7 +286,8 @@ extern "C" void b200vis_destroy(b200vis_ctx *ctx) {
                    ctx->d_tab_cull, ctx->d_tab_fresh, ctx->d_ent_counts, ctx->d_shadow_off, ctx->d_tab_caster,
                    ctx->d_tab_range, const_cast<uint32_t *>(ctx->sdiff.slot), ctx->sdiff.prev, ctx->sdiff.prev_count,
                    ctx->sdiff.words, ctx->sdiff.chunk, ctx->sdiff.dev_offsets, ctx->vdiff.prev, ctx->vdiff.prev_count,
-                   ctx->vdiff.words, ctx->vdiff.chunk, ctx->vdiff.dev_offsets, ctx->d_light_layers_ext, ctx->d_shadow_layers_ext};
+                   ctx->vdiff.words, ctx->vdiff.chunk, ctx->vdiff.dev_offsets, ctx->d_light_layers_ext, ctx->d_shadow_layers_ext,
+                   ctx->d_shadow_kept};
     for (void *p : dev) if (p) cudaFree(p);
     for (const auto &r : ctx->host_regs) cudaHostUnregister(reinterpret_cast<void *>(r.first));
     cudaGetLastError();
@@ -1026,6 +1030,7 @@ extern "C" int32_t b200vis_set_topology(b200vis_ctx *ctx, uint32_t n, const uint
     Plan plan;
     int32_t rc = plan_world(ctx, n, parent, plan);
     if (rc != B200VIS_OK) return rc;
+    ctx->shadow_emit_ready = false;   // rows and rank order change: the last shadow run's bits name other entities
     std::vector<uint32_t> &topo = plan.topo; std::vector<Tile> &tiles = plan.tiles;
     if (tiles.size() > ctx->tiles_cap) {
         void *old[] = {ctx->d_tiles, ctx->d_wtiles, ctx->d_sched};
@@ -1200,6 +1205,7 @@ extern "C" int32_t b200vis_edit_topology(b200vis_ctx *ctx, uint32_t n_despawn, c
     for (uint32_t i = 1; i < n_spawn; ++i)
         if (spawn_entity_bits[ord[i]] == spawn_entity_bits[ord[i - 1]])
             return fail(ctx, B200VIS_ERR_INVALID_ARG, "edit_topology: entity bits %llx spawned twice", (unsigned long long)spawn_entity_bits[ord[i]]);
+    ctx->shadow_emit_ready = false;   // rows and rank order change: the last shadow run's bits name other entities
     bool append = ctx->rank_identity;
     for (uint32_t k = 0; k < n_spawn && append; ++k)
         append = k ? spawn_entity_bits[k] > spawn_entity_bits[k - 1] : (n == 0 || spawn_entity_bits[0] > ctx->max_key);
@@ -1336,6 +1342,7 @@ extern "C" int32_t b200vis_compact_topology(b200vis_ctx *ctx, uint32_t n_reparen
     if (!ctx->topology_set || !ctx->hplan) return fail(ctx, B200VIS_ERR_NOT_READY, "compact_topology: b200vis_set_topology has not been called");
     if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "compact_topology: world_size > 1 (use set_topology)");
     if (n_reparent && (!reparent_rows || !new_parent)) return fail(ctx, B200VIS_ERR_INVALID_ARG, "compact_topology: null array");
+    ctx->shadow_emit_ready = false;   // rows and rank order change: the last shadow run's bits name other entities
     Plan &hp = *ctx->hplan;
     const uint32_t n = ctx->n, V = ctx->cfg.max_views;
     cudaStream_t st = ctx->stream;
@@ -2798,6 +2805,7 @@ static int32_t install_shadow_items(b200vis_ctx *ctx, uint32_t n_items, uint32_t
         ctx->shadow_cap_lights = (uint32_t)nl; ctx->shadow_cap_list = (uint32_t)lc;
     }
     if (n_items) CU(cudaMemcpy(ctx->d_shadow_lights, ctx->h_shadow.data(), n_items * sizeof(ShadowLight), cudaMemcpyHostToDevice));
+    ctx->shadow_emit_ready = false;             // the lists of the last run belong to other items
     ctx->shadow_ext_on = false;                 // every item's RenderLayers blocks 1..3 are empty again
     ctx->shadow.n_lights = n_items; ctx->shadow.lights = ctx->d_shadow_lights; ctx->shadow.caster = ctx->d_caster;
     ctx->shadow.list_cap = ctx->shadow_cap_list;
@@ -2895,7 +2903,9 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
             ctx->sdiff_held[s] = named[s];
         }
     }
+    ctx->shadow_emit_ready = false;
     if (!ctx->shadow.n_lights) {                // the sinks' one offset: a memset, no launch
+        ctx->shadow_emit_ready = ctx->shsink.entities != nullptr;
         if (ctx->shsink.entities) CU(cudaMemsetAsync(ctx->shsink.offsets, 0, 4, st));
         if (ctx->sdiff.added) {
             CU(cudaMemsetAsync(ctx->sdiff.added_offsets, 0, 4, st));
@@ -2919,8 +2929,40 @@ extern "C" int32_t b200vis_run_shadow_culling(b200vis_ctx *ctx) {
     sink.keys = ctx->d_keys;                    // a compaction swaps the key buffers
     ShadowDiff sd = ctx->sdiff;
     sd.keys = ctx->d_keys;
-    launch_shadow_cull(st, R, sb, ctx->diff.prev, active_consts(ctx).n_views, ctx->vis.n_words, ctx->vis.n_chunks,
-                       ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u, sink, sd);
+    // with an entity sink, keep the masks for b200vis_emit_shadow_entities (a sink too small for this run is grown and
+    // filled from them)
+    const size_t kept = ctx->shsink.entities ? (size_t)sb.n_lights * 6 * ctx->vis.words_stride : 0;
+    if (kept > ctx->shadow_kept_cap) {
+        if (ctx->d_shadow_kept) cudaFree(ctx->d_shadow_kept);
+        ctx->d_shadow_kept = nullptr; ctx->shadow_kept_cap = 0;
+        CU(dalloc(&ctx->d_shadow_kept, (size_t)ctx->shadow_cap_lights * 6 * ctx->vis.words_stride));
+        ctx->shadow_kept_cap = (size_t)ctx->shadow_cap_lights * 6 * ctx->vis.words_stride;
+    }
+    CU(launch_shadow_cull(st, R, sb, ctx->diff.prev, active_consts(ctx).n_views, ctx->vis.n_words, ctx->vis.n_chunks,
+                          ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->d_stats, (ctx->frame + 2u) % 3u, sink, sd,
+                          kept ? ctx->d_shadow_kept : nullptr));
+    CU(cudaGetLastError());
+    ctx->shadow_emit_ready = kept != 0;
+    return B200VIS_OK;
+}
+extern "C" int32_t b200vis_emit_shadow_entities(b200vis_ctx *ctx) {
+    CHECK_CTX_JOIN();
+    if (ctx->cfg.world_size > 1) return fail(ctx, B200VIS_ERR_UNSUPPORTED, "emit_shadow_entities: world_size > 1");
+    if (!ctx->shsink.entities) return fail(ctx, B200VIS_ERR_NOT_READY, "emit_shadow_entities: no shadow entity sink registered");
+    if (!ctx->shadow_emit_ready)
+        return fail(ctx, B200VIS_ERR_NOT_READY, "emit_shadow_entities: no b200vis_run_shadow_culling with an entity sink since the items "
+                    "or the topology were last set");
+    // registering a sink and installing items both refuse this combination already; checked again because the expansion
+    // would write past the sink's offsets otherwise
+    if (ctx->shsink_max_items < ctx->shadow.n_lights)
+        return fail(ctx, B200VIS_ERR_CAPACITY, "emit_shadow_entities: max_items %u < %u installed shadow items", ctx->shsink_max_items,
+                    ctx->shadow.n_lights);
+    cudaStream_t st = ctx->stream;
+    if (!ctx->shadow.n_lights) { CU(cudaMemsetAsync(ctx->shsink.offsets, 0, 4, st)); return B200VIS_OK; }
+    ShadowSink sink = ctx->shsink;
+    sink.keys = ctx->d_keys;
+    CU(launch_emit_shadow_entities(st, ctx->shadow, ctx->d_shadow_kept, ctx->rows.n, ctx->vis.n_words, ctx->vis.n_chunks,
+                                   ctx->vis.words_stride, ctx->vis.chunks_stride, ctx->rank_identity ? nullptr : ctx->d_row_of_rank, sink));
     CU(cudaGetLastError());
     return B200VIS_OK;
 }

@@ -4746,22 +4746,27 @@ void launch_publish_clusters(cudaStream_t st, const FrameConsts *fc, const Clust
     ++g_launches; k_publish_clusters<<<dim3(kMaxClusters / 256 + 1, max_views), 256, 0, st>>>(fc, cb.offsets, cb.indices, cb.index_cap, host_offsets, host_indices,
                                                                                 host_cap, stats, host_stats, changed_slot, frame, host_view_stats);
 }
-void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
-                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
-                        const ShadowSink &sink, const ShadowDiff &sd) {
+cudaError_t launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
+                               uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats,
+                               uint32_t changed_slot, const ShadowSink &sink, const ShadowDiff &sd, uint32_t *kept_masks) {
     const bool diff = sd.added != nullptr;
-    if (!sb.n_lights || (!R.n && sink.entities == nullptr && !diff)) return;
+    if (!sb.n_lights || (!R.n && sink.entities == nullptr && !diff)) return cudaSuccess;
     ++g_launches; k_shadow_select<<<cdiv(sb.n_lights, 128), 128, 0, st>>>(sb, R.rank, view_sets, words_stride, n_views);
     if (!R.n) {                                       // no rows: every list is empty, the sinks still get offsets and flags
         if (sink.entities != nullptr) { ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, 0u, chunks_stride, sink.dev_offsets, sink.offsets, sink.active); }
         if (diff) { ++g_launches; k_shadow_diff_offsets<<<1, 1024, 0, st>>>(sb, sd, 0u, chunks_stride); }
-        return;
+        return cudaSuccess;
     }
     ++g_launches;
     if (sb.layers_ext != nullptr) k_shadow_cull<true><<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
     else k_shadow_cull<false><<<cdiv(R.n, 256), 256, 0, st>>>(R, sb, words_stride, chunks_stride, stats, changed_slot);
     const dim3 grid(n_chunks, sb.n_lights);
     if (sink.entities != nullptr) { ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active); }
+    // the expansion clears the mask words it reads: b200vis_emit_shadow_entities expands this run's lists again from the copy
+    if (kept_masks != nullptr) {
+        const cudaError_t e = cudaMemcpyAsync(kept_masks, sb.mask, (size_t)sb.n_lights * 6 * words_stride * 4, cudaMemcpyDeviceToDevice, st);
+        if (e != cudaSuccess) return e;
+    }
     ++g_launches;
     if (sink.entities == nullptr && !diff)
         k_expand_shadow<false, false><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
@@ -4775,9 +4780,31 @@ void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, co
     else
         k_expand_shadow<true, true><<<grid, kChunkWords, 0, st>>>(sb, n_words, n_chunks, words_stride, chunks_stride, R.row_of_rank,
                                                                   sink.keys, sink.dev_offsets, sink.entities, sink.capacity, sd);
-    if (!diff) return;
+    if (!diff) return cudaSuccess;
     ++g_launches; k_shadow_diff_offsets<<<1, 1024, 0, st>>>(sb, sd, n_chunks, chunks_stride);
     ++g_launches; k_emit_shadow_diff<<<grid, kChunkWords, 0, st>>>(sd, n_words, words_stride, chunks_stride);
+    return cudaSuccess;
+}
+cudaError_t launch_emit_shadow_entities(cudaStream_t st, const ShadowBufs &sb, const uint32_t *kept_masks, uint32_t n_rows, uint32_t n_words,
+                                        uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, const uint32_t *row_of_rank,
+                                        const ShadowSink &sink) {
+    if (!sb.n_lights) return cudaSuccess;
+    if (!n_rows) {
+        ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, 0u, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
+        return cudaSuccess;
+    }
+    // the run's expansion left the masks zero; the copy puts its bits back, and this expansion clears them again
+    const cudaError_t e = cudaMemcpyAsync(sb.mask, kept_masks, (size_t)sb.n_lights * 6 * words_stride * 4, cudaMemcpyDeviceToDevice, st);
+    if (e != cudaSuccess) return e;
+    ++g_launches; k_shadow_offsets<<<1, 1024, 0, st>>>(sb, n_chunks, chunks_stride, sink.dev_offsets, sink.offsets, sink.active);
+    ShadowBufs rb = sb;
+    rb.list_cap = 0;                                  // the row lists keep what the run wrote (count gets the same totals again)
+    ShadowDiff none{};
+    ++g_launches;
+    k_expand_shadow<true, false><<<dim3(n_chunks, sb.n_lights), kChunkWords, 0, st>>>(rb, n_words, n_chunks, words_stride, chunks_stride,
+                                                                                      row_of_rank, sink.keys, sink.dev_offsets,
+                                                                                      sink.entities, sink.capacity, none);
+    return cudaSuccess;
 }
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views) {
     if (bb.mode) { ++g_launches; k_pack_cluster_bindings<<<dim3(16, max_views), 256, 0, st>>>(fc, cb, bb); }

@@ -41,10 +41,17 @@ void launch_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd
 void launch_emit_view_diff(cudaStream_t st, const VisibleBufs &vb, const ViewDiff &vd, const ViewSlots &vs, uint32_t n_views,
                            uint32_t slotted_views);
 // sink.entities != nullptr: also the Entity lists, offsets and active flags of b200vis_set_shadow_entities_sink;
-// sd.added != nullptr: also the added / removed Entity lists and offsets of b200vis_set_shadow_diff_sink
-void launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
-                        uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats, uint32_t changed_slot,
-                        const ShadowSink &sink, const ShadowDiff &sd);
+// sd.added != nullptr: also the added / removed Entity lists and offsets of b200vis_set_shadow_diff_sink;
+// kept_masks != nullptr: [n_lights * 6][words_stride], gets a copy of the run's mask bits before the expansion clears them;
+// returns the copy's error (launch errors are left for cudaGetLastError)
+cudaError_t launch_shadow_cull(cudaStream_t st, const Rows &R, const ShadowBufs &sb, const uint32_t *view_sets, uint32_t n_views,
+                               uint32_t n_words, uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, DevStats *stats,
+                               uint32_t changed_slot, const ShadowSink &sink, const ShadowDiff &sd, uint32_t *kept_masks);
+// b200vis_emit_shadow_entities: the offsets, active flags and Entity lists of the last launch_shadow_cull into `sink`, expanded
+// again from kept_masks and the chunk counts that run left; no select, no cull, no diff, the row lists untouched
+cudaError_t launch_emit_shadow_entities(cudaStream_t st, const ShadowBufs &sb, const uint32_t *kept_masks, uint32_t n_rows, uint32_t n_words,
+                                        uint32_t n_chunks, uint32_t words_stride, uint32_t chunks_stride, const uint32_t *row_of_rank,
+                                        const ShadowSink &sink);
 void launch_pack_cluster_bindings(cudaStream_t st, const FrameConsts *fc, const ClusterBufs &cb, const BindingBufs &bb, uint32_t max_views);
 void launch_publish_visible_diff(cudaStream_t st, const VisibleBufs &vb, const DiffBufs &db, uint32_t *host_rows, uint32_t host_stride,
                                  uint32_t *host_counts, uint32_t n_views, uint32_t max_views);

@@ -805,6 +805,21 @@ typedef struct b200vis_shadow_entities_sink {
     uint8_t  *active;     /* [max_items] */
 } b200vis_shadow_entities_sink;
 B200VIS_API int32_t b200vis_set_shadow_entities_sink(b200vis_ctx *ctx, const b200vis_shadow_entities_sink *sink);
+/* Writes the lists of the last b200vis_run_shadow_culling again, into the entity sink registered now: offsets, active
+ * flags and entities exactly as that run would have written them into this sink.  This is how a caller recovers from a
+ * sink that was too small: run, b200vis_synchronize, see offsets[n_items*6] > capacity, register a larger sink, emit,
+ * b200vis_synchronize.  Running the shadow stage again instead would not give the same result, because every run moves the
+ * shadow-diff slots forward.
+ * Enqueued on the context's stream.  It runs no cull and changes nothing else: not the ViewVisibility bits or change
+ * flags, not the frame statistics, not the row lists of b200vis_download_shadow_visible, and not the shadow-diff slots or
+ * the diff sink's outputs.  For this, every run made while an entity sink is registered keeps a device copy of its
+ * bit sets (n_items x 6 x max_entities / 8 bytes, copied before the lists are expanded).
+ * Errors, with nothing enqueued: NOT_READY (no entity sink registered; no run with an entity sink registered since the
+ * last b200vis_set_shadow_items / _ex, b200vis_set_shadow_lights, b200vis_set_topology, b200vis_edit_topology or
+ * b200vis_compact_topology, any of which may change the items, the rows or their rank order), CAPACITY (the sink's
+ * max_items below the installed item count: a safeguard, since b200vis_set_shadow_entities_sink and the item setters
+ * already refuse that combination), UNSUPPORTED (world_size > 1). */
+B200VIS_API int32_t b200vis_emit_shadow_entities(b200vis_ctx *ctx);
 /* The shadow lists' changes: what collect_visible_cpu_culled_entities computes for the light subviews (render
  * view/visibility/mod.rs:333-381 calling update_cpu_culled_entities, :194-249), as Entity values.  The caller gives each
  * item a diff slot with b200vis_set_shadow_items_ex: a persistent identity for the item's RetainedViewEntity (one per

@@ -2,13 +2,20 @@
 //! compile it in a crate that depends on bevy 0.20 and links `b200vis`).  `tests/host_shim.c` performs the same sequence
 //! through the same C ABI in plain C and is run against the CPU oracle on the GPU box.
 //!
-//! The plugin removes three reference system sets from `PostUpdate` / `PostStartup` and adds replacements **with the same
+//! The plugin removes four reference system sets from `PostUpdate` / `PostStartup` and adds replacements **with the same
 //! query signatures, in the same sets**, that call the C ABI of `include/b200vis.h`:
 //!   propagate  <- mark_dirty_trees / propagate_parent_transforms / sync_simple_transforms
 //!                 (crates/bevy_transform/src/systems.rs:42, 111, 506; registered at plugins.rs:37-47)
-//!   cull       <- check_visibility_cpu_culling (crates/bevy_camera/src/visibility/mod.rs:748)
+//!   cull       <- check_visibility_cpu_culling (crates/bevy_camera/src/visibility/mod.rs:748) and check_visibility_ranges
+//!                 (visibility/range.rs:230: the device evaluates the ranges itself from the tables' VisibilityRange columns)
 //!   cluster    <- assign_objects_to_clusters   (crates/bevy_light/src/cluster/assign.rs:137; the only member of
 //!                 SimulationLightSystems::AssignLightsToClusters, crates/bevy_light/src/lib.rs:187-191)
+//!   light      <- check_point_light_mesh_visibility / check_dir_light_mesh_visibility (crates/bevy_light/src/lib.rs:342, 517;
+//!                 SimulationLightSystems::CheckLightVisibility): the shadow lists come back as Entity lists through
+//!                 `b200vis_set_shadow_entities_sink`, their set_visible() goes into the tables as a second write-back
+//! The `VisibleEntityRanges` resource stays initialised and stays empty: nothing fills it once check_visibility_ranges is
+//! gone, and neither the device's camera cull nor its shadow cull reads it (both test the ranges on the device).  Its
+//! presence still switches range culling on, as in the reference (visibility/mod.rs:813-819).
 //! `reset_view_visibility` and `mark_newly_hidden_entities_invisible` are private and share their sets with systems that
 //! must stay, so in an UNFORKED Bevy they keep running on the CPU: the device applies `set_visible()` to the ViewVisibility
 //! byte of every slot whose entity is visible in >= 1 view, straight in the archetype tables (`B200VIS_WB_SET_VISIBLE`),
@@ -28,12 +35,13 @@
 #![allow(non_camel_case_types, clippy::too_many_arguments, clippy::type_complexity)]
 use bevy::camera::primitives::{Aabb, Frustum, Sphere};
 use bevy::camera::visibility::*;
-use bevy::camera::ShadowLodOrigin;
+use bevy::camera::{RenderTarget, ShadowLodOrigin};
 use bevy::ecs::component::Tick;
 use bevy::ecs::entity::EntityHashMap;
 use bevy::ecs::schedule::ScheduleCleanupPolicy::RemoveSystemsOnly;
 use bevy::ecs::system::SystemChangeTick;
-use bevy::light::{cluster::*, PointLight, SimulationLightSystems};
+use bevy::camera::primitives::{CascadesFrusta, CubemapFrusta};
+use bevy::light::{cluster::*, get_shadow_lod_origin, DirectionalLight, NotShadowCaster, PointLight, SimulationLightSystems, SpotLight};
 use bevy::prelude::*;
 use bevy::transform::{systems::*, TransformSystems};
 use core::any::TypeId;
@@ -74,6 +82,9 @@ pub struct b200vis_table_cull_inputs { aabbs: *const Aabb, aabb_changed_ticks: *
 #[repr(C)] pub struct b200vis_visibility_range_layout { stride: u32, start: u32, end: u32, use_aabb: u32 }
 #[repr(C)] #[derive(Clone, Copy, PartialEq)]
 pub struct b200vis_table_visibility_ranges { ranges: *const VisibilityRange, changed_ticks: *const Tick }
+#[repr(C)] pub struct b200vis_shadow_item { kind: u32, light_row: u32, range: f32, range_view_index: i32, layer_mask: u64,
+                                           frusta: [[[f32; 4]; 6]; 6] }
+#[repr(C)] pub struct b200vis_shadow_entities_sink { entities: *mut u64, capacity: u32, max_items: u32, offsets: *mut u32, active: *mut u8 }
 
 #[link(name = "b200vis")]
 extern "C" {
@@ -112,6 +123,12 @@ extern "C" {
     fn b200vis_set_table_visibility_ranges(ctx: *mut b200vis_ctx, n: u32, ranges: *const b200vis_table_visibility_ranges,
                                            layout: *const b200vis_visibility_range_layout) -> i32;
     fn b200vis_set_visibility_range_views(ctx: *mut b200vis_ctx, n: u32, positions: *const f32) -> i32;
+    fn b200vis_set_table_shadow_casters(ctx: *mut b200vis_ctx, n: u32, is_caster: *const u8) -> i32;
+    fn b200vis_set_shadow_items(ctx: *mut b200vis_ctx, n: u32, items: *const b200vis_shadow_item, list_capacity: u32) -> i32;
+    fn b200vis_set_shadow_item_render_layers_ext(ctx: *mut b200vis_ctx, n: u32, blocks: *const [u64; 3]) -> i32;
+    fn b200vis_run_shadow_culling(ctx: *mut b200vis_ctx) -> i32;
+    fn b200vis_set_shadow_entities_sink(ctx: *mut b200vis_ctx, sink: *const b200vis_shadow_entities_sink) -> i32;
+    fn b200vis_emit_shadow_entities(ctx: *mut b200vis_ctx) -> i32;
 }
 const NO_PARENT: u32 = 0xFFFF_FFFF; const DETACHED: u32 = 0xFFFF_FFFE;
 const STAGE_PROPAGATE: u32 = 1; const STAGE_CULL: u32 = 2; const STAGE_CLUSTER: u32 = 12;
@@ -120,6 +137,7 @@ const RD_TRANSFORM: u32 = 1; const RD_GLOBAL_TRANSFORM: u32 = 2; const RD_CULL_I
 const F_INHERITED: u8 = 0x01; const F_AABB: u8 = 0x02; const F_SPHERE: u8 = 0x04; const F_NO_FRUSTUM: u8 = 0x08;
 const F_RANGE: u8 = 0x10; const F_NO_CPU_CULLING: u8 = 0x20; const F_SPHERE_FROM_GT: u8 = 0x40;
 const VIEW_ACTIVE: u8 = 1; const VIEW_NO_CPU_CULLING: u8 = 2;
+const SHADOW_POINT: u32 = 0; const SHADOW_SPOT: u32 = 1; const SHADOW_DIRECTIONAL_CASCADE: u32 = 2;
 const ERR_HIERARCHY_CYCLE: i32 = 4;
 const MAX_CAMERAS: usize = 32; const MAX_CLUSTERS: usize = 4096;
 
@@ -155,6 +173,15 @@ pub struct B200Vis {
     table_ranges: Option<Vec<b200vis_table_visibility_ranges>>,
     // some row has had a RenderLayers layer in 64..255: the rows' blocks 1..3 are uploaded with their block 0 from then on
     rows_ext: bool,
+    // the table -> shadow-caster bytes attached with b200vis_set_table_shadow_casters (attached after every cull-input attach)
+    table_casters: Vec<u8>,
+    // the range views b200_check_visibility gave b200vis_set_visibility_range_views this frame (their bit = their position)
+    range_views: Vec<Entity>,
+    // the shadow entity sink: every shadow list of a run as Entity::to_bits(), its offsets and active flags.  It grows, up to
+    // max_shadow_entries entries, when a run's lists do not fit; a replaced sink's buffers stay alive with the context,
+    // because the library keeps their registration
+    shadow_entities: Vec<u64>, shadow_offsets: Vec<u32>, shadow_active: Vec<u8>, shadow_max_items: usize,
+    max_shadow_entries: usize, retired_shadow_sinks: Vec<(Vec<u64>, Vec<u32>, Vec<u8>)>,
 }
 unsafe impl Send for B200Vis {}
 unsafe impl Sync for B200Vis {}
@@ -167,6 +194,17 @@ impl B200Vis {
         // crates/bevy_transform/src/systems.rs:715 panics on a malformed hierarchy; keep that behaviour
         if rc == ERR_HIERARCHY_CYCLE { panic!("Malformed hierarchy: {msg}"); }
         Err(format!("b200vis error {rc}: {msg}").into())
+    }
+    /// Registers a shadow entity sink of `capacity` entries for `max_items` items in place of the current one.
+    fn set_shadow_sink(&mut self, capacity: usize, max_items: usize) -> Result<(), BevyError> {
+        let old = (core::mem::replace(&mut self.shadow_entities, vec![0; capacity.max(1)]),
+                   core::mem::replace(&mut self.shadow_offsets, vec![0; max_items * 6 + 1]),
+                   core::mem::replace(&mut self.shadow_active, vec![0; max_items.max(1)]));
+        if !old.0.is_empty() { self.retired_shadow_sinks.push(old); }
+        self.shadow_max_items = max_items;
+        let s = b200vis_shadow_entities_sink { entities: self.shadow_entities.as_mut_ptr(), capacity: self.shadow_entities.len() as u32,
+            max_items: max_items as u32, offsets: self.shadow_offsets.as_mut_ptr(), active: self.shadow_active.as_mut_ptr() };
+        self.check(unsafe { b200vis_set_shadow_entities_sink(self.ctx, &s) })
     }
     fn class_bit(&mut self, id: TypeId) -> u8 {
         if let Some(k) = self.classes.iter().position(|c| *c == id) { return 1 << k; }
@@ -181,7 +219,10 @@ impl B200Vis {
 /// `max_entities` entries per view: a view whose visible entities are in more than `max_entities` class lists in all (an
 /// entity counts once per VisibilityClass it carries) makes the cull system return an error, so an app whose entities
 /// carry several classes sets `max_entities` to cover that total.
-pub struct B200VisibilityPlugin { pub max_entities: u32, pub max_lights: u32, pub max_cameras: u32 }
+/// `max_shadow_entries`: the most entries all shadow lists of a frame may hold together (every point-light face, spot
+/// light and directional cascade list, an entity counting once per list it is in).  The sink starts small and doubles
+/// when a frame needs more; a frame that needs more than this makes the light-visibility system return an error.
+pub struct B200VisibilityPlugin { pub max_entities: u32, pub max_lights: u32, pub max_cameras: u32, pub max_shadow_entries: u32 }
 
 impl Plugin for B200VisibilityPlugin {
     fn build(&self, app: &mut App) {
@@ -200,7 +241,9 @@ impl Plugin for B200VisibilityPlugin {
             entity_offsets: vec![[0; 9]; max_views],
             cluster_offsets: vec![0; max_views * (MAX_CLUSTERS + 1)], cluster_indices: vec![0; max_views * cluster_cap], cluster_cap,
             planes_scratch: vec![0.0; 3 * 4097 * 4], tables: Vec::new(), table_inputs: Vec::new(), table_cull: Vec::new(), table_entities: Vec::new(),
-            maps_epoch: u64::MAX, table_ranges: None, rows_ext: false,
+            maps_epoch: u64::MAX, table_ranges: None, rows_ext: false, table_casters: Vec::new(), range_views: Vec::new(),
+            shadow_entities: Vec::new(), shadow_offsets: Vec::new(), shadow_active: Vec::new(), shadow_max_items: 0,
+            max_shadow_entries: self.max_shadow_entries as usize, retired_shadow_sinks: Vec::new(),
         };
         // the sorted row lists stay on the device: VisibleEntities arrives as Entity values through the entities sink, and
         // GlobalTransform and ViewVisibility go straight into the archetype tables (b200vis_set_tables)
@@ -213,6 +256,7 @@ impl Plugin for B200VisibilityPlugin {
             assert_eq!(b200vis_set_result_sink(ctx, &rs), 0); assert_eq!(b200vis_set_visible_entities_sink(ctx, &es), 0);
             assert_eq!(b200vis_set_view_stats_sink(ctx, vis.view_stats.as_mut_ptr()), 0);   // per-view stats of every view
         }
+        vis.set_shadow_sink((1usize << 16).min(vis.max_shadow_entries.max(1)), 64).expect("b200vis_set_shadow_entities_sink");
         app.insert_resource(vis);
         // CPU clustering mode, so that `Clusters` holds `ClusterableObjects::Cpu`, which the cluster system fills (SURVEY.md 0)
         app.insert_resource(GlobalClusterSettings { gpu_clustering: None, supports_storage_buffers: true,
@@ -226,14 +270,20 @@ impl Plugin for B200VisibilityPlugin {
             app.add_systems(schedule, (b200_sync_tables, b200_propagate).chain().in_set(TransformSystems::Propagate));
         }
         app.remove_systems_in_set(PostUpdate, check_visibility_cpu_culling, RemoveSystemsOnly);
-        // check_visibility_ranges stays: the device evaluates the ranges the cull uses from the tables' VisibilityRange
-        // columns, but the CPU light-visibility systems, which this plugin does not replace yet, read VisibleEntityRanges
-        // (DESIGN.md section 9 item 0).
+        // the device evaluates the ranges from the tables' VisibilityRange columns for both culls, so nothing reads
+        // what check_visibility_ranges would write
+        app.remove_systems_in_set(PostUpdate, check_visibility_ranges, RemoveSystemsOnly);
         app.remove_systems_in_set(PostUpdate, SimulationLightSystems::AssignLightsToClusters, RemoveSystemsOnly);
+        app.remove_systems_in_set(PostUpdate, SimulationLightSystems::CheckLightVisibility, RemoveSystemsOnly);
         app.add_systems(PostUpdate, (
             (b200_sync_tables, b200_check_visibility).chain().in_set(VisibilitySystems::CheckVisibility),
             b200_assign_lights_to_clusters.in_set(SimulationLightSystems::AssignLightsToClusters)
                 .after(TransformSystems::Propagate).after(VisibilitySystems::CheckVisibility),
+            // the reference's ordering of the light-visibility systems (bevy_light/src/lib.rs:217-230)
+            (b200_sync_tables, b200_check_light_visibility).chain().in_set(SimulationLightSystems::CheckLightVisibility)
+                .after(VisibilitySystems::CalculateBounds).after(TransformSystems::Propagate)
+                .after(SimulationLightSystems::UpdateLightFrusta).after(VisibilitySystems::CheckVisibility)
+                .before(VisibilitySystems::MarkNewlyHiddenEntitiesInvisible),
         ));
     }
 }
@@ -349,6 +399,10 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     let markers = [(world.component_id::<NoFrustumCulling>(), F_NO_FRUSTUM), (world.component_id::<VisibilityRange>(), F_RANGE),
                    (world.component_id::<NoCpuCulling>(), F_NO_CPU_CULLING)];
     let light_id = world.component_id::<PointLight>();
+    // the archetypes of the light systems' visible_entity_query (lib.rs:526-537): With<Mesh3d>, Without<NotShadowCaster>,
+    // Without<DirectionalLight>
+    let (mesh_id, not_caster_id, dir_id) = (world.component_id::<Mesh3d>(), world.component_id::<NotShadowCaster>(),
+                                            world.component_id::<DirectionalLight>());
     // VisibilityRange is repr(Rust) too.  Without the VisibleEntityRanges resource the reference does not range-cull at
     // all (visibility/mod.rs:813-819), so nothing is attached then.
     let range_layout = b200vis_visibility_range_layout { stride: size_of::<VisibilityRange>() as u32,
@@ -360,6 +414,7 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
     world.resource_scope(|world, mut vis: Mut<B200Vis>| {
         let vis = &mut *vis;
         let (mut descs, mut inputs, mut culls, mut entities, mut ranges) = (Vec::new(), Vec::new(), Vec::new(), Vec::new(), Vec::new());
+        let mut casters = Vec::new();
         for table in world.storages().tables.iter() {
             if !table.has_column(gt_id) { continue; }
             // SAFETY: the columns hold GlobalTransform / ViewVisibility.  Only raw pointers are kept; the GPU writes through
@@ -395,6 +450,7 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             if has(light_id) && aabb.is_null() && !sphere.is_null() { flags |= F_SPHERE_FROM_GT; }
             culls.push(b200vis_table_cull_inputs { aabbs: aabb, aabb_changed_ticks: aabb_t, spheres: sphere, sphere_changed_ticks: sphere_t,
                                                    inherited_visibility: iv, iv_changed_ticks: iv_t, flags: flags as u32 });
+            casters.push((has(mesh_id) && !has(not_caster_id) && !has(dir_id)) as u8);
             // the VisibilityRange column goes with the table's F_RANGE bit, as the library requires
             let (range, range_t) = column::<VisibilityRange>(table, range_id);
             ranges.push(b200vis_table_visibility_ranges { ranges: range, changed_ticks: range_t });
@@ -415,6 +471,13 @@ fn b200_sync_tables(world: &mut World) -> Result<(), BevyError> {
             }
             vis.check(unsafe { b200vis_set_table_cull_inputs(vis.ctx, culls.len() as u32, culls.as_ptr(), &bounds_layout) })?;
             vis.table_cull = culls;
+            vis.table_casters.clear();              // attached again below, before the frame's cull read
+        }
+        // the shadow-caster byte of every table, read with the cull inputs.  The first attach also switches on the
+        // visible-set bookkeeping the shadow stage reads, so it must precede the frame's CULL read.
+        if !vis.tables.is_empty() && casters != vis.table_casters {
+            vis.check(unsafe { b200vis_set_table_shadow_casters(vis.ctx, casters.len() as u32, casters.as_ptr()) })?;
+            vis.table_casters = casters;
         }
         // the VisibilityRange columns the cull read takes the range parameters from (an attach after none reads every
         // ranged table in full)
@@ -484,6 +547,8 @@ fn b200_check_visibility(
         }
         vis.check(unsafe { b200vis_set_visibility_range_views(vis.ctx, range_entities.len() as u32, range_pos.as_ptr()) })?;
     }
+    // the light-visibility system gives each shadow item the bit of its view among these
+    vis.range_views.clone_from(&range_entities);
     // ---- views: half spaces copied verbatim from `Frustum` (bit-identical by construction) ----
     let (mut views, mut view_ext) = (Vec::new(), Vec::new());
     vis.view_entities.clear();
@@ -680,6 +745,149 @@ fn b200_assign_lights_to_clusters(
         clusters.clusterable_objects = ClusterableObjects::Cpu(cells);
         clusters.last_frame_total_cluster_index_count = Some(vis.view_stats[v][1] as usize);
         clusters.last_frame_farthest_z = Some(f32::from_bits(vis.view_stats[v][2]));     // assign.rs:810-811
+    }
+    Ok(())
+}
+
+/// Where a shadow item's lists go.
+enum ShadowDest { Point(Entity), Spot(Entity), Cascade { light: Entity, view: Entity, cascade: usize } }
+
+/// light: check_point_light_mesh_visibility and check_dir_light_mesh_visibility (bevy_light/src/lib.rs:342-749) as one
+/// device pass.  The items come from the lights' own components (CubemapFrusta, Frustum, CascadesFrusta copied verbatim);
+/// whether a point or spot light is in some view's VisibleEntities, the caster bytes and the shadow LOD origin's range
+/// bit are decided on the device.  The lists come back sorted, as Entity values.
+fn b200_check_light_visibility(
+    this_run: SystemChangeTick,
+    mut vis: ResMut<B200Vis>,
+    mut point_lights: Query<(Entity, &PointLight, &CubemapFrusta, &mut CubemapVisibleEntities, Option<&RenderLayers>)>,
+    mut spot_lights: Query<(Entity, &SpotLight, &Frustum, &mut VisibleMeshEntities, Option<&RenderLayers>)>,
+    mut directional_lights: Query<(Entity, &DirectionalLight, &CascadesFrusta, &mut CascadesVisibleEntities, Option<&RenderLayers>),
+                                  Without<SpotLight>>,
+    // write access to every ViewVisibility column: the write-backs below set bytes and change ticks in the tables while
+    // this system runs (the reference's check_point_light_mesh_visibility holds &mut ViewVisibility too, lib.rs:537).
+    // The directional lights' own visibility is read through it.
+    view_visibility: Query<&mut ViewVisibility>,
+    // get_shadow_lod_origin's lenses, as check_point_light_mesh_visibility builds them (lib.rs:561-565)
+    mut camera_query: Query<(Entity, &RenderTarget), With<Camera>>,
+    mut shadow_lod_origin_query: Query<Entity, With<ShadowLodOrigin>>,
+    mut point_and_spot_light_query: Query<Entity, Or<(With<PointLight>, With<SpotLight>)>>,
+) -> Result<(), BevyError> {
+    let vis = &mut *vis;
+    // no table holds GlobalTransform yet: no light or mesh has a row, and the shadow stage has no caster column
+    if vis.table_casters.is_empty() { return Ok(()); }
+    let lod_origin = get_shadow_lod_origin(camera_query.transmute_lens_filtered(), shadow_lod_origin_query.transmute_lens_filtered(),
+                                           point_and_spot_light_query.transmute_lens_filtered());
+    // the bit of a view in the device's range masks: its position among this frame's range views, -1 = not among them
+    let range_bit = |e: Option<Entity>, views: &[Entity]| e.and_then(|e| views.iter().position(|r| *r == e)).map_or(-1, |i| i as i32);
+    let lod_bit = range_bit(lod_origin, &vis.range_views);
+    let (mut items, mut ext, mut dest) = (Vec::new(), Vec::new(), Vec::new());
+    let item = |kind, light_row, range, range_view_index, layer_mask| b200vis_shadow_item { kind, light_row, range, range_view_index,
+                                                                                            layer_mask, frusta: [[[0.0; 4]; 6]; 6] };
+    // ---- one point item per PointLight with shadow maps, one spot item per SpotLight with shadow maps ----
+    for (e, light, frusta, _, layers) in point_lights.iter() {
+        if !light.shadow_maps_enabled { continue; }
+        let Some(&row) = vis.row_of.get(&e) else { continue };
+        let blocks = layer_blocks(e, layers)?;
+        let mut it = item(SHADOW_POINT, row, light.range, lod_bit, blocks[0]);
+        for (f, face) in frusta.frusta.iter().enumerate() {
+            for (k, hs) in face.half_spaces.iter().enumerate() { it.frusta[f][k] = hs.normal_d().to_array(); }
+        }
+        items.push(it); ext.push(ext_of(&blocks)); dest.push(ShadowDest::Point(e));
+    }
+    for (e, light, frustum, _, layers) in spot_lights.iter() {
+        if !light.shadow_maps_enabled { continue; }
+        let Some(&row) = vis.row_of.get(&e) else { continue };
+        let blocks = layer_blocks(e, layers)?;
+        let mut it = item(SHADOW_SPOT, row, light.range, lod_bit, blocks[0]);
+        for (k, hs) in frustum.half_spaces.iter().enumerate() { it.frusta[0][k] = hs.normal_d().to_array(); }
+        items.push(it); ext.push(ext_of(&blocks)); dest.push(ShadowDest::Spot(e));
+    }
+    // ---- one cascade item per (view, cascade) of a directional light with shadow maps that is visible (lib.rs:395-399) ----
+    let light_visible = |e: Entity| view_visibility.get(e).is_ok_and(|v| v.get());
+    for (e, light, frusta, _, layers) in directional_lights.iter() {
+        if !light.shadow_maps_enabled || !light_visible(e) { continue; }
+        let blocks = layer_blocks(e, layers)?;
+        for (view, view_frusta) in &frusta.frusta {
+            let view_bit = range_bit(Some(*view), &vis.range_views);
+            for (c, frustum) in view_frusta.iter().enumerate() {
+                let mut it = item(SHADOW_DIRECTIONAL_CASCADE, 0, 0.0, view_bit, blocks[0]);
+                for (k, hs) in frustum.half_spaces.iter().enumerate() { it.frusta[0][k] = hs.normal_d().to_array(); }
+                items.push(it); ext.push(ext_of(&blocks)); dest.push(ShadowDest::Cascade { light: e, view: *view, cascade: c });
+            }
+        }
+    }
+    let n = items.len();
+    // a sink for fewer items than these would make b200vis_set_shadow_items refuse them: grow it first
+    if n > vis.shadow_max_items {
+        let cap = vis.shadow_entities.len();
+        vis.set_shadow_sink(cap, n.max(2 * vis.shadow_max_items))?;
+    }
+    // list_capacity 1: the lists come from the entity sink, the row lists are never read
+    unsafe {
+        vis.check(b200vis_set_shadow_items(vis.ctx, n as u32, items.as_ptr(), 1))?;
+        if ext.iter().any(|b| b.iter().any(|&w| w != 0)) {
+            vis.check(b200vis_set_shadow_item_render_layers_ext(vis.ctx, n as u32, ext.as_ptr()))?;
+        }
+        vis.check(b200vis_run_shadow_culling(vis.ctx))?;
+        // set_visible() of the rows only lights see, with this system's tick (the rows the cameras made visible hold
+        // their bit already).  Forked, the device's bytes are written instead.
+        #[cfg(not(feature = "forked-bevy"))]
+        vis.check(b200vis_writeback_tables(vis.ctx, WB_SET_VISIBLE, 0, this_run.this_run().get()))?;
+        #[cfg(feature = "forked-bevy")]
+        vis.check(b200vis_writeback_tables(vis.ctx, WB_VIEW_VISIBILITY, 0, this_run.this_run().get()))?;
+        vis.check(b200vis_synchronize(vis.ctx))?;
+    }
+    // ---- a sink too small for this frame: grow it and have the same lists written again (running the stage again would
+    // not do: it would move the shadow diff forward) ----
+    let total = vis.shadow_offsets[n * 6] as usize;
+    if total > vis.shadow_entities.len() {
+        if total > vis.max_shadow_entries {
+            return Err(format!("the shadow lists of this frame hold {total} entries, more than B200VisibilityPlugin::max_shadow_entries \
+                                ({}): raise it", vis.max_shadow_entries).into());
+        }
+        let cap = total.max(2 * vis.shadow_entities.len()).min(vis.max_shadow_entries);
+        let max_items = vis.shadow_max_items;
+        vis.set_shadow_sink(cap, max_items)?;
+        unsafe { vis.check(b200vis_emit_shadow_entities(vis.ctx))?; vis.check(b200vis_synchronize(vis.ctx))?; }
+    }
+    // SAFETY: every entry is the to_bits() of a live Entity, given to b200vis_set_topology (layout asserted in
+    // b200_check_visibility)
+    let all = unsafe { core::slice::from_raw_parts(vis.shadow_entities.as_ptr() as *const Entity, total) };
+    let off = &vis.shadow_offsets;
+    let list = |l: usize| &all[off[l] as usize..off[l + 1] as usize];
+    // ---- CubemapVisibleEntities faces and spot VisibleMeshEntities: only active items.  An inactive light is not in any
+    // view's VisibleEntities: the reference `continue`s past it and its component keeps what it held ----
+    for (i, d) in dest.iter().enumerate() {
+        if vis.shadow_active[i] == 0 { continue; }
+        match *d {
+            ShadowDest::Point(e) => {
+                let Ok((_, _, _, mut faces, _)) = point_lights.get_mut(e) else { continue };
+                for (f, face) in faces.iter_mut().enumerate() { face.entities.clear(); face.entities.extend_from_slice(list(i * 6 + f)); }
+            }
+            ShadowDest::Spot(e) => {
+                let Ok((_, _, _, mut visible, _)) = spot_lights.get_mut(e) else { continue };
+                visible.entities.clear(); visible.entities.extend_from_slice(list(i * 6));
+            }
+            ShadowDest::Cascade { .. } => {}
+        }
+    }
+    // ---- CascadesVisibleEntities, as check_dir_light_mesh_visibility keeps it (lib.rs:380-404): every view's vector sized
+    // to its cascades, views that left CascadesFrusta dropped and new ones added, everything cleared for a light without
+    // shadow maps or not visible; then each cascade's list replaced ----
+    for (e, light, frusta, mut visible, _) in directional_lights.iter_mut() {
+        let visible = &mut *visible;
+        visible.entities.retain(|view, _| frusta.frusta.contains_key(view));
+        for (view, view_frusta) in &frusta.frusta {
+            visible.entities.entry(*view).or_default().resize(view_frusta.len(), Default::default());
+        }
+        if !light.shadow_maps_enabled || !light_visible(e) { visible.entities.clear(); }
+    }
+    for (i, d) in dest.iter().enumerate() {
+        let ShadowDest::Cascade { light, view, cascade } = *d else { continue };
+        let Ok((_, _, _, mut visible, _)) = directional_lights.get_mut(light) else { continue };
+        let Some(lists) = visible.entities.get_mut(&view) else { continue };
+        let dst = &mut lists[cascade].entities;
+        dst.clear(); dst.extend_from_slice(list(i * 6));
     }
     Ok(())
 }
